@@ -12,7 +12,7 @@ overlapped with the backward pass), fused SGD step.  Prints ONE JSON line (rank 
              `Trainer.train()` runs: the next batch staged and enqueued while the current one runs, every loss read back), CUDA-event
              timed over all K steps, max over ranks.
   e2e      : the same loop with the batches in pinned HOST memory: host->device copies and the loss read-back inside the timed region.
-  roofline : the dominant kernel (conv_tcgen05_split_kernel: sparse-conv forward / data-gradient) -- algorithmic bytes
+  roofline : the dominant kernel (conv_wgmma_kernel<split>: sparse-conv forward / data-gradient) -- algorithmic bytes
              (BASELINE.md section 2) of all its launches in one step / their CUDA-event time (events recorded by the library
              around every launch, `pcb_profile_enable`), vs the measured HBM peak.
   cpu_baseline : the oracle (ME-0.4.3-algorithm CPU restatement) timed on this box's host cores: full training steps on
@@ -20,11 +20,16 @@ overlapped with the backward pass), fused SGD step.  Prints ONE JSON line (rank 
 
 --impl reference times that CPU restatement as the whole measurement (the reference's own arithmetic layer,
 MinkowskiEngine 0.4.3, is not in the reference tree and not installable offline -- DESIGN.md): the reference's own
-`model/res16unet.py` (when /root/reference or its staged copy oracle/_ref is present) on the oracle operators, the thread
+`model/res16unet.py` (when its staged copy oracle/_ref is present, see oracle/stage_ref.py) on the oracle operators, the thread
 count chosen by a measured sweep; it never loads libpcb200.so.
 
 --workload c4: BASELINE configs[4], S3DIS-shaped full-scene inference (5 cm voxels, eval-mode BatchNorm, 13 classes, forward only,
 `downstream/semseg/lib/test.py:95-117`); metric scenes/sec.
+
+--dump-outputs DIR: after the timed steps, writes what the timed path computed in its last step as DIR/<name>.npy (float32 / float64,
+64 MB at most; a fixed seeded sample where the full output is larger): the loss, both views' per-point features and the updated
+parameters (c4: logits and predictions; --impl reference: loss and features).  Inputs and sampling are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import json
@@ -60,6 +65,7 @@ def parse():
     ap.add_argument("--workload", default="c1", choices=list(WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--profile-json", default=None, help="write the per-launch conv profile of one step here")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs here as .npy files")
     return ap.parse_args()
 
 
@@ -75,7 +81,31 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
+
+
+# ----------------------------------------------------------------------------------------------- output dump
+DUMP_SAMPLE = 4_000_000          # values kept of an output larger than this (float32: 16 MB)
+
+
+def seeded_sample(t, n=DUMP_SAMPLE):
+    """`t` flattened, or a fixed seeded sample of n of its values (in index order) when it is larger."""
+    flat = t.detach().reshape(-1)
+    if flat.numel() > n:
+        idx = np.sort(np.random.default_rng(0).choice(flat.numel(), n, replace=False))
+        flat = flat[torch.from_numpy(idx).to(flat.device)]
+    return flat.cpu()
+
+
+def dump_outputs(out_dir, arrays):
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        total += a.nbytes
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+    assert total <= 64 << 20, f"dumped outputs are {total} bytes"
 
 
 # ----------------------------------------------------------------------------------------------- clocks sampler
@@ -130,8 +160,8 @@ def usable_cores():
 
 # ----------------------------------------------------------------------------------------------- CPU oracle leg
 def _oracle_model_ctor():
-    """Res16UNet34C on the oracle operators: the REFERENCE's own model file when it is present (/root/reference in the build
-    container, the staged copy under oracle/_ref on the GPU box) -- nothing of this package's CUDA side is imported then --
+    """Res16UNet34C on the oracle operators: the REFERENCE's own model file when it is present (PCB_REFERENCE_ROOT, or the
+    copy staged under oracle/_ref) -- nothing of this package's CUDA side is imported then --
     else this package's model file (same graph, checked module by module in tests/test_host.py)."""
     from oracle import me_cpu as OR
     from tests import refload
@@ -143,7 +173,7 @@ def _oracle_model_ctor():
     return res16unet.Res16UNet34C, refload.default_config(), "this package's model file (reference tree absent)"
 
 
-def cpu_oracle_steps(workload, steps, warmup, loss_kind, sweep=True):
+def cpu_oracle_steps(workload, steps, warmup, loss_kind, sweep=True, record=None):
     """ME-0.4.3-algorithm CPU restatement (the oracle), fp32.  Every step is a full training step (2x forward, loss, backward,
     SGD) on ONE full-size scene pair of the workload -- a quarter of a 'c1' per-rank batch, no shrinking, no extrapolation.
     The torch thread count is chosen by timing one step at each of {8, 16, 32, all usable} (more threads are slower on big hosts)."""
@@ -176,6 +206,8 @@ def cpu_oracle_steps(workload, steps, warmup, loss_kind, sweep=True):
             loss = a + b
         loss.backward()
         opt.step()
+        if record is not None:                              # the last step's outputs, for --dump-outputs
+            record.update(loss=loss.detach(), F0=F[0], F1=F[1])
         return time.perf_counter() - t0
 
     torch.set_num_threads(min(cores, 16))
@@ -201,7 +233,12 @@ def run_reference(args):
     if rank != 0:
         return
     wl = "c1" if args.workload == "c4" else args.workload
-    cb, ms = cpu_oracle_steps(wl, args.steps, args.warmup, args.loss)
+    last = {}
+    cb, ms = cpu_oracle_steps(wl, args.steps, args.warmup, args.loss, record=last)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"loss": np.asarray([float(last["loss"])], dtype=np.float64),
+                                         "F0_sample": seeded_sample(last["F0"]).numpy().astype(np.float32),
+                                         "F1_sample": seeded_sample(last["F1"]).numpy().astype(np.float32)})
     line = {"impl": "reference", "metric": METRIC, "value": cb["value"], "unit": "pairs/s", "n_gpus": args.gpus, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32", "data": "synthetic", "config": static_config(args, int(os.environ.get("WORLD_SIZE", "1"))),
@@ -296,9 +333,17 @@ def run_ours(args):
     # The timed loop is the trainer's own loop (`Trainer.iter_losses`: batch i+1 staged and enqueued while batch i runs, every loss read
     # back) over DEVICE-resident batches.  Calling `train_step(batch)` back to back instead builds each batch's coordinate manager inline
     # and never reads a loss: at 8 ranks that loop showed 3-4 steps of 45-80 ms among the first ten (all ranks wait in the all-reduce
-    # for one late rank), the trainer's loop none in 60 (profiles/r2_results.md, runs 17 / 23).
+    # for one late rank), the trainer's loop none in 60.
     import itertools
     it_dev = itertools.cycle(dev_batches)
+    last_feats = {}
+    if args.dump_outputs:           # keep the per-point features of the latest step (nothing is enqueued after the last timed one)
+        forward_views = trainer._forward_views
+
+        def _forward_views(input_dict):
+            last_feats["F"] = forward_views(input_dict)
+            return last_feats["F"]
+        trainer._forward_views = _forward_views
     for _ in trainer.iter_losses(it_dev, args.warmup):
         pass
     sync_all()
@@ -321,6 +366,12 @@ def run_ours(args):
     host_ms_per_step = (t_wall1 - t_wall0) * 1e3 / args.steps
     clk = clocks.stop(t_wall0, t_wall1) if clocks else None
     pairs_per_step = wl["batch"] * world
+    if args.dump_outputs and rank == 0:
+        # what the last timed step computed: its loss, the per-point features of both views, and the parameters its SGD step produced
+        dump_outputs(args.dump_outputs, {
+            "loss": np.asarray([float(x) for x in (loss if isinstance(loss, tuple) else (loss,))], dtype=np.float64),
+            "F0_sample": seeded_sample(last_feats["F"][0]).numpy(), "F1_sample": seeded_sample(last_feats["F"][1]).numpy(),
+            "params_sample": seeded_sample(torch.cat([q.detach().reshape(-1) for q in trainer.model.parameters()])).numpy()})
     value = pairs_per_step * args.steps / (ms_total / 1e3)
 
     # ---- end-to-end through the public trainer call, host (pinned) batches
@@ -370,20 +421,14 @@ def run_ours(args):
         agg = {}
         for r in prof:
             b, f = conv_alg_bytes(r)
-            key = ("conv_tcgen05_split_kernel" if r["kind"] in ("fwd", "dgrad") else "wgrad_tcgen05_kernel") if r["tc"] \
+            key = ("conv_wgmma_kernel<split>" if r["kind"] in ("fwd", "dgrad") else "wgrad_wgmma_kernel") if r["tc"] \
                 else "fp32 SIMT (3-channel stem conv / wgrad)"
             a = agg.setdefault(key, dict(bytes=0, flops=0, ms=0.0, launches=0))
             a["bytes"] += b; a["flops"] += f; a["ms"] += r["ms"]; a["launches"] += 1
             r["bytes"], r["flops"] = b, f
         dom = max(agg, key=lambda k: agg[k]["ms"])
         a = agg[dom]
-        traffic, traffic_note = None, "no ncu pass of this schedule committed"
-        try:        # dram__bytes_read+write per launch of this kernel, from the committed ncu pass of THIS schedule (profiles/traffic.json)
-            tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-            traffic = tj["kernels"][dom]["dram_bytes_per_launch"]
-            traffic_note = tj.get("note", "")
-        except Exception:
-            pass
+        traffic, traffic_note = None, "no measured DRAM traffic of this schedule committed"
         conv_ms = sum(v["ms"] for v in agg.values())
         conv_bytes = sum(v["bytes"] for v in agg.values())
         step_ms = ms_total / args.steps
@@ -413,7 +458,7 @@ def run_ours(args):
                 "config": static_config(args, world),
                 "details": {"voxels_per_view_per_rank": [n0, n1],
                             "schedule": "both views stacked in one pass (per-view BatchNorm statistics)" if fused.PAIR else "two forward calls",
-                            "l2": "per-step working set (activations + kernel maps, GBs) far exceeds the 126 MB L2; 2 distinct batches cycled",
+                            "l2": "per-step working set (activations + kernel maps, GBs) far exceeds the 50 MB L2; 2 distinct batches cycled",
                             "final_loss": float(loss[0] if isinstance(loss, tuple) else loss),
                             "per_step_ms": {"median": float(np.median(per_step)), "min": float(np.min(per_step)), "max": float(np.max(per_step)),
                                             "p90": float(np.percentile(per_step, 90))},
@@ -441,16 +486,20 @@ def run_c4(args):
     devb = [(torch.from_numpy(s["feats"]).cuda(), torch.from_numpy(s["coords"]).cuda()) for s in scenes]
     host = [(torch.from_numpy(s["feats"]).pin_memory(), torch.from_numpy(s["coords"]).pin_memory()) for s in scenes]
 
+    last = {}
+
     def run(batches, n, to_host):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         torch.cuda.synchronize(); e0.record()
         for i in range(n):
             f, c = batches[i % len(batches)]
             with torch.no_grad():
-                pred = net(me.SparseTensor(f, coords=c).to("cuda")).F.argmax(1)
+                logits = net(me.SparseTensor(f, coords=c).to("cuda")).F
+                pred = logits.argmax(1)
             if to_host:
                 pred = pred.cpu()
         e1.record(); torch.cuda.synchronize()
+        last.update(logits=logits, pred=pred)
         return e0.elapsed_time(e1) / n
     run(devb, args.warmup, False)
     clocks = Clocks(0)
@@ -459,6 +508,9 @@ def run_c4(args):
     launches = _lib.launch_count() - l0
     t1 = time.time()
     clk = clocks.stop(t0, t1)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"logits_sample": seeded_sample(last["logits"]).numpy().astype(np.float32),
+                                         "pred": last["pred"].cpu().numpy().astype(np.float64)})
     ms_e2e = run(host, args.steps, True)
     nvox = sum(len(s["coords"]) for s in scenes) / len(scenes)
     h2d = int(np.mean([f.numel() * 4 + c.numel() * 4 for f, c in host]))

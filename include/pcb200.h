@@ -1,8 +1,8 @@
 /*
- * pcb200.h -- C ABI of libpcb200.so: the B200 (sm_100a) replacement for the native half of the
+ * pcb200.h -- C ABI of libpcb200.so: the H100 (sm_90a) replacement for the native half of the
  * MinkowskiEngine v0.4.3 operator library on PointContrast's Res16UNet34C hot path.
  *
- * What each entry point replaces (reference call sites are relative to /root/reference; the ME
+ * What each entry point replaces (reference call sites are relative to the original PointContrast repository; the ME
  * native sources are an external, un-vendored dependency pinned at README.md:24,34):
  *
  *   pcb_coords_* / pcb_hash_* / pcb_kernel_map*   ME CoordsManager (CPU hash map): initialize, stride, getKernelMap.
@@ -48,7 +48,7 @@ extern "C" {
 #define PCB_MAX_KERNEL_VOLUME 27
 
 const char* pcb_last_error(void);
-/* "pcb200 <version> sm_100a" */
+/* "pcb200 <version> sm_90a" */
 const char* pcb_version(void);
 /* Number of kernels this library has launched on this process since load (bench.py's gpu_launches). */
 uint64_t pcb_launch_count(void);
@@ -111,8 +111,8 @@ int pcb_weight_prep(const float* W, int K, int Cin, int Cout, uint16_t* w_hi, ui
 /* Y[j, :] = bias + sum_k X[tbl[kmap[k]][j], :] . W[k]      (j < n_out)      -- fp32 operands (the modular ME-style surface)
  *   X  : [*, Cin] row stride ldx (floats);  Y: [n_out, Cout] row stride ldy.
  *   wk_hi/wk_lo : the weights of THIS call's roles as bf16 hi/lo planes, K-major = [K][Cout][Cin] (pcb_weight_prep: the wt_* planes for
- *               the forward roles; the w_* planes with swapped channel counts for the data gradient).  Tensor-core path (tcgen05, fp32 rows
- *               split to bf16 hi/lo in the producers' registers, fp32 accumulate in TMEM): Cin % 32 == 0, Cout % 32 == 0, K <= 27.
+ *               the forward roles; the w_* planes with swapped channel counts for the data gradient).  Tensor-core path (wgmma, fp32 rows
+ *               split to bf16 hi/lo in the producers' registers, fp32 accumulate in registers): Cin % 32 == 0, Cout % 32 == 0, K <= 27.
  *   w_f32     : fp32 weights [K][Cin][Cout] for the exact SIMT path (other widths, the 3-channel stem, PCB_CONV_FORCE_SIMT); may be NULL
  *               when the tensor-core path applies.
  *   kmap      : HOST int32 [K] table row used by weight k (NULL = identity). */
@@ -121,7 +121,7 @@ int pcb_weight_prep(const float* W, int K, int Cin, int Cout, uint16_t* w_hi, ui
 #define PCB_PLANES_A_FP16 8    /* split-operand calls: the GATHERED operand's planes are fp16 hi/lo (default: bf16 hi/lo) */
 #define PCB_PLANES_B_FP16 16   /* pcb_conv_forward_split: the weight tiles are fp16 x 2^10 (pcb_weight_tile with this flag);
                                   pcb_conv_wgrad_split: the ROW-ALIGNED operand's planes are fp16.  Both operands of a call must
-                                  use the same format (tcgen05.mma.kind::f16 rejects fp16 x bf16): set both flags or neither. */
+                                  use the same format (wgmma takes one 16-bit format for both operands): set both flags or neither. */
 /* Small levels split the (offset, channel-chunk) loop over extra CTAs and reduce through `ws` (deterministic). */
 size_t pcb_conv_forward_ws_bytes(int K, int64_t n_out, int Cin, int Cout);
 int pcb_conv_forward(const float* X, int ldx, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap, int K,
@@ -143,7 +143,7 @@ int pcb_conv_wgrad(const float* A, int lda, const float* B, int ldb, const int32
                    int64_t n_out, int Ca, int Cb, float* dW, int transpose_out, void* ws, size_t ws_bytes,
                    int flags, void* stream);
 
-/* Split-operand variants (tcgen05 only): the gathered / row-aligned operands are bf16 hi/lo planes (see pcb_split_rows),
+/* Split-operand variants (tensor-core path only): the gathered / row-aligned operands are bf16 hi/lo planes (see pcb_split_rows),
  * row strides lds/lda/ldb in ELEMENTS (multiples of 8).  Same semantics as pcb_conv_forward / pcb_conv_wgrad; the kernels'
  * operand staging is then a pure asynchronous copy (cp.async, zero-filled where a neighbour is missing). */
 /* pcb_weight_tile: fp32 W[K][Cin][Cout] -> split weights pre-tiled as the shared-memory images of the split conv kernel (one
@@ -207,7 +207,7 @@ int pcb_bn_backward_seg(const float* dY, int lddy, const float* X, int ldx, cons
                         uint16_t* dXlo, int lds, void* ws, size_t ws_bytes, void* stream);
 /* "Split" operand format of the tensor-core conv kernels: an fp32 matrix stored as two 16-bit planes, x ~= hi + lo: bf16 planes
  * (2^-17 relative, fp32's exponent range: gradients) or, with PCB_PLANES_A_FP16, fp16 planes (2^-22 relative, |x| < 65504: the
- * activations gathered by the FORWARD convolutions -- the forward pass sets the whole-network gradient error, profiles/r2_results.md);
+ * activations gathered by the FORWARD convolutions -- the forward pass sets the whole-network gradient error);
  * row stride lds in ELEMENTS.  The elementwise producers above can emit it directly (Yhi/Ylo, dXhi/dXlo; NULL = off; dX may
  * then be NULL), so the conv kernels' gather becomes a pure asynchronous copy.  pcb_split_rows converts an fp32 matrix. */
 int pcb_split_rows(const float* X, int ldx, int64_t n, int C, uint16_t* hi, uint16_t* lo, int lds, int flags, void* stream);
@@ -244,7 +244,7 @@ typedef struct pcb_unit {
   float* mean; float* invstd;                       /* [segments][Cout], written by forward, read by backward */
   const float* x_p; int32_t x_ld; const uint16_t* x_hi; const uint16_t* x_lo; int32_t x_lds;
   const uint16_t* x_bhi; const uint16_t* x_blo;     /* PCB_UNIT_FP16_FORWARD: x once more as bf16 hi/lo planes (the weight gradient pairs it
-                                                       with the bf16 gradient planes: tcgen05.mma takes ONE format for both operands) */
+                                                       with the bf16 gradient planes: wgmma takes ONE format for both operands) */
   float* z_p; int32_t z_ld;
   float* out_p; int32_t out_ld; uint16_t* out_hi; uint16_t* out_lo; int32_t out_lds;
   uint16_t* out_bhi; uint16_t* out_blo;             /* PCB_UNIT_FP16_FORWARD: bf16 hi/lo copy of `out` (row stride out_lds) */
@@ -260,8 +260,7 @@ typedef struct pcb_unit {
 #define PCB_UNIT_FP16_FORWARD 2     /* activations are gathered by the forward convolutions as fp16 hi/lo planes (x_hi/x_lo, out_hi/out_lo)
                                        against fp16 weight tiles (pcb_weight_tile with PCB_PLANES_B_FP16): 2^-22 products in the
                                        forward pass.  Gradients (dz) and the data-gradient tiles stay bf16 hi/lo (fp32's exponent
-                                       range); tcgen05.mma.kind::f16 rejects mixed fp16 x bf16 operands (illegal instruction,
-                                       profiles/probes/mixed_fmt_probe.cu), so every activation also carries bf16 hi/lo planes
+                                       range); wgmma takes one 16-bit format for both operands, so every activation also carries bf16 hi/lo planes
                                        (x_bhi/x_blo, out_bhi/out_blo) for the weight gradient. */
 #define PCB_UNIT_EVAL 4             /* forward only, eval-mode BatchNorm: normalise with running_mean / running_var (not updated) */
 size_t pcb_unit_ws_bytes(int K, int64_t n_in, int64_t n_out, int Cin, int Cout);
@@ -271,7 +270,7 @@ int pcb_unit_backward(const pcb_unit* u, void* stream);
 /* ----------------------------------------------------------------------------------------------- losses */
 /* PointInfoNCE on gathered rows q,k [n, D]: loss = mean_i(logsumexp_j(q_i.k_j/T) - q_i.k_i/T).
  * Writes loss (device float), dq, dk (= d loss / d q, d k).  ws: pcb_nce_ws_bytes(n).
- * D = 32 or 64: fused tcgen05 kernels (nce_tc5.cu) -- q k^T tiles in Tensor Memory from fp16 hi/lo operands (|q|,|k| <= ~1: the
+ * D = 32 or 64: fused wgmma kernels (nce_wgmma.cu) -- q k^T tiles on the tensor cores from fp16 hi/lo operands (|q|,|k| <= ~1: the
  * L2-normalised features), softmax statistics and both gradients straight from the tiles, the n x n logits never stored.
  * Other widths (or PCB_NCE_SIMT=1): exact fp32 SIMT kernels that materialise the logits in ws. */
 size_t pcb_nce_ws_bytes(int64_t n);

@@ -2,8 +2,8 @@
 
 A CPU restatement (numpy for the integer coordinate work, torch CPU tensors + autograd for the
 floating-point work) of the MinkowskiEngine v0.4.3 semantics that PointContrast's hot path
-exercises (`/root/reference/README.md:24,34` pins the version; the library itself is NOT under
-/root/reference, not installed and not fetchable -- SURVEY.md section 8c).
+exercises (the original repository's `README.md:24,34` pins the version; the library itself is not part of that
+repository, and not installable offline -- SURVEY.md section 8c).
 
 PARITY UNPINNED at the ME boundary: the reference holds no golden vectors for this path and
 MinkowskiEngine cannot be run here.  What *is* pinned (tests/test_oracle_*.py):

@@ -1,4 +1,4 @@
-// Shared helpers for libpcb200 (sm_100a).  Not part of the public ABI.
+// Shared helpers for libpcb200 (sm_90a).  Not part of the public ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -74,7 +74,7 @@ inline int current_device() { int dev = 0; cudaGetDevice(&dev); return (dev >= 0
 inline int num_sms() {
   static int n[64] = {};
   const int dev = current_device();
-  if (!n[dev]) { cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev); if (n[dev] <= 0) n[dev] = 148; }
+  if (!n[dev]) { cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev); if (n[dev] <= 0) n[dev] = 132; }
   return n[dev];
 }
 

@@ -21,7 +21,7 @@ namespace {
 
 struct KMap { int v[PCB_MAX_KERNEL_VOLUME]; };
 
-constexpr int BM = 128;        // output rows per CTA tile of the tensor-core kernels (conv_tc5.cu)
+constexpr int BM = 128;        // output rows per CTA tile of the tensor-core kernels (conv_wgmma.cu)
 constexpr int BK = 32;         // input channels per pipeline step
 
 
@@ -249,9 +249,9 @@ int pick_tile(int C) {      // largest of {128, 96, 64, 32} dividing C
 int conv_splits(int K, int64_t n_out, int Cin, int Cout) {
   int bn = pick_tile(Cout);
   int64_t base = ((n_out + BM - 1) / BM) * (Cout / bn);
-  const int64_t one_wave = 2ll * num_sms();
+  const int64_t one_wave = num_sms();          // the tensor-core kernel runs one CTA per SM
   if (base >= one_wave) return 1;
-  static double waves = 0.0;        // CTAs to aim for on a small level, in units of one resident wave (measured on C1: 0.25-0.5 best; 2 costs 4 ms/step)
+  static double waves = 0.0;        // CTAs to aim for on a small level, in units of one resident wave
   if (waves == 0.0) { const char* e = getenv("PCB_CONV_SPLIT_WAVES"); waves = e ? atof(e) : 0.5; if (waves < 0.05) waves = 0.05; }
   int64_t s = ((int64_t)(waves * one_wave) + base - 1) / base;
   int64_t T = (int64_t)K * (Cin / BK);
@@ -284,10 +284,10 @@ extern "C" int pcb_weight_prep(const float* W, int K, int Cin, int Cout, uint16_
 
 namespace pcb {
 int wgrad_group();
-int launch_wgrad_tcgen05(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
+int launch_wgrad_wgmma(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
                          const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int Ca, int Cb, int rows_per_split, int splits,
                          float* partial, int transpose_out, int tn, cudaStream_t st, int a_fp16 = 0, int b_fp16 = 0);
-int launch_conv_tcgen05(const float* X, int ldx, const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl,
+int launch_conv_wgmma(const float* X, int ldx, const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl,
                         int64_t tbl_stride, const int* kmap, int K, int64_t n_out,
                         int Cin, int Cout, const uint16_t* wk_hi, const uint16_t* wk_lo, const float* bias, float* Y, int ldy,
                         float* partial, int nsplit, int bn, int accumulate, cudaStream_t st, int x_fp16 = 0, int w_fp16 = 0);
@@ -312,7 +312,7 @@ extern "C" int pcb_conv_forward(const float* X, int ldx, const int32_t* tbl, int
   for (int k = 0; k < K; ++k) { km.v[k] = kmap ? kmap[k] : k; PCB_ARG(km.v[k] >= 0 && km.v[k] < PCB_MAX_KERNEL_VOLUME); }
   const bool tc_ok = (Cin % 32 == 0) && (Cout % 32 == 0) && (ldx % 4 == 0) && wk_hi && wk_lo && !(flags & PCB_CONV_FORCE_SIMT);
   if (!tc_ok) {
-    if (flags & PCB_CONV_ACCUMULATE) { set_error("PCB_CONV_ACCUMULATE needs the tcgen05 path"); return PCB_ERR_ARG; }
+    if (flags & PCB_CONV_ACCUMULATE) { set_error("PCB_CONV_ACCUMULATE needs the tensor-core path"); return PCB_ERR_ARG; }
     if (!w_f32) { set_error("pcb_conv_forward: SIMT path needs w_f32 (Cin=%d Cout=%d)", Cin, Cout); return PCB_ERR_ARG; }
     if (Cin == 3 && Cout == 32) {         // the stem layer
       launch_kernel(conv_stem_kernel<3>, (unsigned)((n_out + 127) / 128), 128, 0, st, X, ldx, tbl, tbl_stride, km, K, n_out, w_f32, bias, Y, ldy);
@@ -323,13 +323,13 @@ extern "C" int pcb_conv_forward(const float* X, int ldx, const int32_t* tbl, int
                                                                       w_f32, bias, Y, ldy);
     return check_launch("conv_simt_kernel");
   }
-  // tensor-core path: the tcgen05 kernel on fp32 inputs (split to bf16 hi/lo in the producers' registers), K-major weight planes
+  // tensor-core path: the wgmma kernel on fp32 inputs (split to bf16 hi/lo in the producers' registers), K-major weight planes
   if (!(wk_hi && wk_lo && ldy % 4 == 0)) { set_error("pcb_conv_forward: the tensor-core path needs the K-major planes wk_hi / wk_lo"); return PCB_ERR_ARG; }
   const int nsplit = conv_splits(K, n_out, Cin, Cout);
   if (nsplit > 1) PCB_ARG(ws && ws_bytes >= (size_t)nsplit * n_out * Cout * sizeof(float));
   const int accumulate = (flags & PCB_CONV_ACCUMULATE) ? 1 : 0;
-  if (int e = launch_conv_tcgen05(X, ldx, nullptr, nullptr, 0, nullptr, tbl, tbl_stride, km.v, K, n_out, Cin, Cout, wk_hi, wk_lo, bias, Y, ldy,
-                                  nsplit > 1 ? (float*)ws : nullptr, nsplit, pick_tile(Cout), accumulate, st)) return e;
+  if (int e = launch_conv_wgmma(X, ldx, nullptr, nullptr, 0, nullptr, tbl, tbl_stride, km.v, K, n_out, Cin, Cout, wk_hi, wk_lo, bias, Y, ldy,
+                                nsplit > 1 ? (float*)ws : nullptr, nsplit, pick_tile(Cout), accumulate, st)) return e;
   if (nsplit > 1) {
     int64_t n4 = n_out * (Cout / 4);
     launch_kernel(conv_split_reduce_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, (const float*)ws, nsplit, n_out, Cout, bias, Y, ldy, accumulate);
@@ -399,7 +399,7 @@ extern "C" int pcb_conv_wgrad(const float* A, int lda, const float* B, int ldb, 
 
 // ------------------------------------------------------------------------------------------------ split-operand entry points
 // Weights as shared-memory images for the split conv kernel: per (offset k, 32-channel chunk kc, BN-column block nb) one blob
-//   [hi plane | lo plane], plane = 4 k8-groups x (BN/8 core matrices x 128 B + 16 B pad)   (UMMA K-major, no swizzle)
+//   [hi plane | lo plane], plane = 4 k8-groups x (BN/8 core matrices x 128 B + 16 B pad)   (wgmma K-major, no swizzle)
 // so that a pipeline stage's weight tile is ONE contiguous TMA bulk copy.
 namespace {
 __host__ __device__ inline int64_t tile_plane_bytes(int bn) { return 4ll * ((bn / 8) * 128 + 16); }
@@ -566,7 +566,7 @@ int bn_reduce_stats_launch(const float* P, int nsplit, float* Y, int ldy, int64_
 // bn != NULL: a BatchNorm follows this convolution (no bias, no accumulate).  When the convolution runs offset-split (small levels)
 // its reduction pass also produces the BatchNorm statistics (one read of the partial planes instead of reduce + a column-sum pass
 // over Y) and *bn_done = 1; in direct mode nothing changes and *bn_done = 0 (the caller runs pcb_bn_stats_seg: fusing the column
-// sums into the TMEM epilogue was measured SLOWER than the separate pass, profiles/r2_results.md).
+// sums into the epilogue is not done: each thread holds scattered fragment rows, the separate pass reads Y once, coalesced).
 struct BnFuse { int64_t n0; float eps, momentum; float* mean; float* invstd; float* running_mean; float* running_var; void* ws; size_t ws_bytes; };
 int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap,
                             int K, int64_t n_out, int Cin, int Cout, const void* w_tiles, const float* bias, float* Y, int ldy, void* ws,
@@ -583,9 +583,9 @@ int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, c
   const int nsplit = conv_splits(K, n_out, Cin, Cout);
   if (nsplit > 1) PCB_ARG(ws && ws_bytes >= (size_t)nsplit * n_out * Cout * sizeof(float));
   if (bn) PCB_ARG(!bias && !accumulate && bn->n0 >= 1 && bn->n0 <= n_out && bn_done);
-  if (int e = launch_conv_tcgen05(nullptr, 0, Xhi, Xlo, lds, w_tiles, tbl, tbl_stride, km, K, n_out, Cin, Cout, nullptr, nullptr, bias, Y, ldy,
-                                  nsplit > 1 ? (float*)ws : nullptr, nsplit, pick_tile(Cout), accumulate, st,
-                                  (flags & PCB_PLANES_A_FP16) ? 1 : 0, (flags & PCB_PLANES_B_FP16) ? 1 : 0)) return e;
+  if (int e = launch_conv_wgmma(nullptr, 0, Xhi, Xlo, lds, w_tiles, tbl, tbl_stride, km, K, n_out, Cin, Cout, nullptr, nullptr, bias, Y, ldy,
+                                nsplit > 1 ? (float*)ws : nullptr, nsplit, pick_tile(Cout), accumulate, st,
+                                (flags & PCB_PLANES_A_FP16) ? 1 : 0, (flags & PCB_PLANES_B_FP16) ? 1 : 0)) return e;
   if (nsplit > 1) {
     if (bn) {
       *bn_done = 1;
@@ -611,11 +611,13 @@ extern "C" int pcb_conv_forward_split(const uint16_t* Xhi, const uint16_t* Xlo, 
 namespace {
 int wgrad_split_splits(int K, int64_t n_out, int Ca, int Cb) {
   int tn = pick_tile(Cb);
-  const int gk = pcb::wgrad_group();          // 4 offsets per CTA, one CTA per SM -- or 2 and two CTAs per SM
+  const int gk = pcb::wgrad_group();          // offsets per CTA
   int64_t base = (int64_t)((K + gk - 1) / gk) * ((Ca + 127) / 128) * (Cb / tn);      // CTAs per split: offset groups x channel blocks
   static double wwaves = 0.0;
-  if (wwaves == 0.0) { const char* e = getenv("PCB_WGRAD_SPLIT_WAVES"); wwaves = e ? atof(e) : 1.0; if (wwaves < 0.05) wwaves = 0.05; }      // measured on C1: 1 wave best (0.5 under-fills, 2-3 add reduce traffic)
-  int64_t s = (int64_t)(wwaves * num_sms() * (gk == 2 ? 2 : 1)) / base;       // whole waves of resident CTAs, never a nearly-empty extra one
+  if (wwaves == 0.0) { const char* e = getenv("PCB_WGRAD_SPLIT_WAVES"); wwaves = e ? atof(e) : 1.0; if (wwaves < 0.05) wwaves = 0.05; }
+  // heuristic, not tuned on H100: aim for 2 x num_sms CTAs (two waves of a kernel that fits once per SM), never a nearly-empty extra
+  // wave; shorter row ranges per split also keep each fp32 accumulator's sum short
+  int64_t s = (int64_t)(wwaves * 2 * num_sms()) / base;
   int64_t max_s = (n_out + 63) / 64;          // small levels: rather many short CTAs than a few long serial ones
   if (s > max_s) s = max_s;
   if (s < 1) s = 1;
@@ -641,15 +643,15 @@ extern "C" int pcb_conv_wgrad_split(const uint16_t* Ahi, const uint16_t* Alo, in
     return PCB_OK;
   }
   PCB_ARG(Ahi && Alo && Bhi && Blo && tbl && ws && tbl_stride >= n_out);
-  // tcgen05.mma.kind::f16 takes ONE 16-bit format for both operands (fp16 x bf16 is an illegal instruction)
+  // wgmma takes ONE 16-bit format for both operands
   PCB_ARG(((flags & PCB_PLANES_A_FP16) != 0) == ((flags & PCB_PLANES_B_FP16) != 0));
   ProfScope prof(st, 1);
   const int splits = wgrad_split_splits(K, n_out, Ca, Cb);
   PCB_ARG(ws_bytes >= (size_t)splits * nW * sizeof(float));
   int64_t rps = (n_out + splits - 1) / splits;
   rps = (rps + 15) / 16 * 16;
-  if (int e = launch_wgrad_tcgen05(Ahi, Alo, lda, Bhi, Blo, ldb, tbl, tbl_stride, K, n_out, Ca, Cb, (int)rps, splits, (float*)ws,
-                                   transpose_out, pick_tile(Cb), st, (flags & PCB_PLANES_A_FP16) ? 1 : 0, (flags & PCB_PLANES_B_FP16) ? 1 : 0)) return e;
+  if (int e = launch_wgrad_wgmma(Ahi, Alo, lda, Bhi, Blo, ldb, tbl, tbl_stride, K, n_out, Ca, Cb, (int)rps, splits, (float*)ws,
+                                 transpose_out, pick_tile(Cb), st, (flags & PCB_PLANES_A_FP16) ? 1 : 0, (flags & PCB_PLANES_B_FP16) ? 1 : 0)) return e;
   launch_kernel(wgrad_reduce_kernel, (unsigned)((nW + 255) / 256), 256, 0, st, (const float*)ws, splits, nW, dW,
                                                                     (flags & PCB_CONV_ACCUMULATE) ? 1 : 0);
   return check_launch("wgrad_reduce_kernel");

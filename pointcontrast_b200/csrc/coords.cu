@@ -16,7 +16,7 @@ void set_error(const char* fmt, ...) {
 using namespace pcb;
 
 extern "C" const char* pcb_last_error(void) { return pcb::g_err; }
-extern "C" const char* pcb_version(void) { return "pcb200 0.1 sm_100a"; }
+extern "C" const char* pcb_version(void) { return "pcb200 0.1 sm_90a"; }
 extern "C" uint64_t pcb_launch_count(void) { return pcb::g_launches.load(); }
 extern "C" int pcb_set_device(int device) { PCB_CUDA(cudaSetDevice(device)); return PCB_OK; }
 

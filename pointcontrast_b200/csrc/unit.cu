@@ -1,6 +1,6 @@
 // Fused "units" of the Res16UNet graph: convolution -> BatchNorm -> (+ residual) -> (ReLU) issued from one C call, and the
 // reverse sweep of the same unit (include/pcb200.h: pcb_unit).  Host-side sequencing only -- the kernels live in
-// conv_tc5.cu / conv.cu / bn.cu; what this file adds over calling them one by one from the host language:
+// conv_wgmma.cu / conv.cu / bn.cu; what this file adds over calling them one by one from the host language:
 //   * the BatchNorm statistics come from the convolution's own epilogue (or from its offset-split reduction pass), so the
 //     separate column-sum pass over z and its launch disappear;
 //   * one boundary crossing per unit instead of three to five.

@@ -34,8 +34,7 @@ PAIR = os.environ.get("PCB_PAIR", "1") == "1"
 VIEW1_BATCH_OFFSET = 1 << 14      # batch indices of view 1 in a stacked tensor (packed keys hold batch < 65535)
 # Coordinate-manager build on a side stream (0: on the current stream, as the modular `SparseTensor(...)` path always does).
 SIDE_STREAM = os.environ.get("PCB_COORDS_STREAM", "1") == "1"
-# CUDA stream priority of that stream (0 = default, -1 = high).  Same-box A/B (profiles/r2_results.md): 158.9 vs 159.8 pairs/s end to end,
-# 165.7 vs 166.0 device-resident: no effect, default kept.
+# CUDA stream priority of that stream (0 = default, -1 = high).
 SIDE_PRIORITY = int(os.environ.get("PCB_COORDS_PRIORITY", "0"))
 # Cross-check switch: BatchNorm statistics by a separate pass over z instead of the convolution epilogue.
 SEPARATE_STATS = os.environ.get("PCB_SEPARATE_STATS", "0") == "1"

@@ -1,4 +1,4 @@
-"""MinkowskiEngine-compatible operator surface backed by libpcb200 (hand-written sm_100a CUDA, include/pcb200.h).
+"""MinkowskiEngine-compatible operator surface backed by libpcb200 (hand-written sm_90a CUDA, include/pcb200.h).
 
 This module provides the names PointContrast's hot path imports from `MinkowskiEngine` v0.4.3
 (`pretrain/pointcontrast/model/res16unet.py:10-12`, `model/resnet.py:8-9`, `model/modules/common.py:9,21,53-62,
@@ -385,13 +385,13 @@ class SparseTensor:
 import os as _os
 
 FORCE_SIMT = False      # tests flip this to run the exact fp32 kernels
-SIMT_OPS = set()        # diagnostics (profiles/grad_precision_ab.py): subset of {"fwd", "dgrad", "wgrad"} forced onto the exact fp32 kernels (modular path)
-CONV_IMPL = "tcgen05"   # the only tensor-core implementation (the round-1 mma.sync kernels are gone); kept as a name for callers
+SIMT_OPS = set()        # diagnostics: subset of {"fwd", "dgrad", "wgrad"} forced onto the exact fp32 kernels (modular path)
+CONV_IMPL = "wgmma"     # the only tensor-core implementation; kept as a name for callers
 # bench.py sets this to a list: every convolution / weight-gradient entry-point call then appends its description here, in
 # issue order -- the same order in which the library (pcb_profile_enable) brackets those calls with CUDA events.
 PROFILE = None
 # Fused executor: activations travel as fp16 hi/lo planes and the forward weight tiles are fp16 (22 mantissa bits per operand instead of
-# bf16 hi/lo's 16): the forward pass is what sets the whole-network gradient error (profiles/r2_results.md).  0: bf16 everywhere.
+# bf16 hi/lo's 16): the forward pass is what sets the whole-network gradient error.  0: bf16 everywhere.
 FWD_FP16 = _os.environ.get("PCB_FWD_FP16", "1") == "1"
 PLANES_A_FP16, PLANES_B_FP16 = 8, 16
 
@@ -424,7 +424,7 @@ class _PreparedWeights:
         self._tiles = None
 
     def tiles(self, kernel):
-        """(forward, data-gradient) weights pre-tiled as shared-memory images for the split tcgen05 kernel (TMA bulk loads)."""
+        """(forward, data-gradient) weights pre-tiled as shared-memory images for the split wgmma kernel (TMA bulk loads)."""
         tag = (kernel.data_ptr(), kernel._version, tuple(kernel.shape), _WEIGHTS_EPOCH[0], FWD_FP16)
         if tag != self.tile_tag:
             K, Cin, Cout = kernel.shape

@@ -7,11 +7,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-REFERENCE = "/root/reference"
-
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a machine with an H100)")
     import torch
     # the CPU oracle is many small torch ops: on a 100+-core host the default thread count is several times SLOWER than 16 threads
     torch.set_num_threads(min(torch.get_num_threads(), 16))
@@ -25,8 +23,3 @@ def pytest_collection_modifyitems(config, items):
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)
-
-
-@pytest.fixture(scope="session")
-def have_reference():
-    return os.path.isdir(os.path.join(REFERENCE, "pretrain", "pointcontrast"))

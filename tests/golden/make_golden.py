@@ -1,11 +1,11 @@
-"""Generates tests/golden/c0_res16unet34c.npz  (run in the build container, where /root/reference exists):
+"""Generates tests/golden/c0_res16unet34c.npz  (needs the original repository: PCB_REFERENCE_ROOT=/path/to/PointContrast):
 
     python tests/golden/make_golden.py
 
-The REFERENCE's own model graph (`/root/reference/pretrain/pointcontrast/model/res16unet.py`, imported unmodified)
+The REFERENCE's own model graph (`pretrain/pointcontrast/model/res16unet.py`, imported unmodified)
 is executed on the CPU oracle (oracle/me_cpu.py, fp64) for BASELINE config C0: one synthetic scene pair (~4k voxels
 per view), Res16UNet34C, PointInfoNCE (T = 0.4, npos = 4096), deterministic weights (tests/helpers.det_init).
-Stored: the inputs, per-point output features of both views, the loss, the chosen positive indices, the gradient
+Stored: the inputs, per-point output features of both views (a fixed seeded two thirds of the rows, `F0_rows` / `F1_rows`), the loss, the chosen positive indices, the gradient
 norm of every parameter, slices of three gradients, and -- because the backward pass of this network is ill-conditioned
 (BatchNorm backward cancels the common-mode part of the gradient; DESIGN.md "Numerics") -- the relative error that the
 SAME graph run in plain fp32 has against fp64, per parameter (`grad_relerr_f32`): the floor of any fp32 implementation.  tests/test_gpu_model.py replays it on the GPU.
@@ -67,6 +67,9 @@ def main():
                g_final=sd["final.kernel"].grad.numpy().astype(np.float32),
                g_b8=sd["block8.1.conv2.kernel"].grad.numpy()[13].astype(np.float32), bn_running_mean_l1=bn_rm,
                grad_relerr_f32=f32_err, feat_relerr_f32=np.float64(f32_feat_err))
+    for v in "01":      # a fixed seeded two thirds of the feature rows: the file stays under 1 MB
+        rows = np.sort(np.random.default_rng(int(v)).choice(len(out["F" + v]), (2 * len(out["F" + v])) // 3, replace=False))
+        out["F" + v], out[f"F{v}_rows"] = out["F" + v][rows], rows.astype(np.int64)
     path = os.path.join(ROOT, "tests", "golden", "c0_res16unet34c.npz")
     np.savez_compressed(path, **out)
     print("wrote", path, os.path.getsize(path), "bytes; loss", loss.item(), "N0", len(batch["sinput0_C"]))

@@ -1,4 +1,4 @@
-"""Generates tests/golden/loss_curve_100.npz  (run in the build container; ~6 minutes of CPU):
+"""Generates tests/golden/loss_curve_100.npz  (~6 minutes of CPU):
 
     python tests/golden/make_loss_curve.py
 

@@ -214,7 +214,7 @@ def _split(x, flags=0):
 @pytest.mark.parametrize("Ca,Cb,tr", [(96, 96, 0), (128, 96, 0), (32, 32, 0), (64, 64, 1), (256, 256, 0), (384, 256, 0),
                                        (192, 128, 1), (96, 32, 0), (256, 128, 1), (32, 96, 0)])
 def test_split_operand_wgrad_tcgen05_matches_exact_fp32_kernel(Ca, Cb, tr):
-    """tcgen05 weight-gradient on bf16 hi/lo planes (MN-major UMMA operands) vs the exact fp32 SIMT kernel of the library."""
+    """Tensor-core weight-gradient on bf16 hi/lo planes (MN-major wgmma operands) vs the exact fp32 SIMT kernel of the library."""
     from pointcontrast_b200 import me
     from pointcontrast_b200._lib import check, lib, ptr, stream
     rng = np.random.default_rng(Ca + Cb)
@@ -353,7 +353,7 @@ def test_l2_normalize_matches_torch(n, C):
 
 @pytest.mark.parametrize("n,D,T", [(2000, 64, 0.4), (300, 32, 0.07)])
 def test_point_nce_tensor_core_and_simt_paths_agree(n, D, T, monkeypatch):
-    """The fused tcgen05 PointInfoNCE (D = 32 / 64) against the oracle AND against the exact-fp32 SIMT kernels of the same
+    """The fused tensor-core PointInfoNCE (D = 32 / 64) against the oracle AND against the exact-fp32 SIMT kernels of the same
     library (`PCB_NCE_SIMT` is read once per process, so the SIMT side is reached through a width the tiling does not cover)."""
     from pointcontrast_b200 import losses
     g = torch.Generator().manual_seed(n + D)
