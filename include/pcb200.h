@@ -289,6 +289,39 @@ int pcb_l2norm_backward(const float* dY, const float* Y, const float* inv_norm, 
 int pcb_pdist_rowmin(const float* A, int64_t P, const float* B, int64_t S, int D, float* minval, int32_t* argmin,
                      uint64_t* packed, void* stream);
 
+/* ----------------------------------------------------------------------------------------------- PointNet++ operators (DESIGN.md 8f-5) */
+/* The native operators of VoteNet's PointNet++ backbone and heads (`downstream/votenet_det_new/models/backbone/pointnet2/_ext_src`),
+ * with their shapes: xyz fp32 [B, N, 3], features fp32 [B, C, N] (channels first), indices int32.  Distances are fp32 with one
+ * rounding per operation, d = ((dx*dx + dy*dy) + dz*dz): index results are bit-reproducible on the host.  Sizes >= 2^31, npoint < 1,
+ * nsample < 1 and radius <= 0 return PCB_ERR_ARG before anything is launched.
+ *
+ * Furthest-point sampling: idx [B, npoint]; idx[0] = 0, running min-distance from 1e10, points with |p|^2 <= 1e-3 never chosen (index 0
+ * when nothing is left); ties go to the SMALLEST index.  One thread-block cluster per scene.  ws: pcb_furthest_point_sampling_ws_bytes
+ * (0 unless N exceeds what a cluster holds on chip; ws may then be NULL). */
+size_t pcb_furthest_point_sampling_ws_bytes(int64_t B, int64_t N);
+int pcb_furthest_point_sampling(const float* xyz, int64_t B, int64_t N, int64_t npoint, int32_t* idx, void* ws, size_t ws_bytes, void* stream);
+/* idx [B, M, nsample]: the first nsample k (ascending) with |new_xyz[m] - xyz[k]|^2 < radius^2; the remaining slots repeat the first hit;
+ * a row with no hit is all zeros. */
+int pcb_ball_query(const float* new_xyz, const float* xyz, int64_t B, int64_t M, int64_t N, float radius, int nsample, int32_t* idx,
+                   void* stream);
+/* dist2, idx [B, n, 3]: the three nearest known points of each unknown point (squared distances; ties keep the earlier k); when m < 3
+ * the missing entries are dist2 = inf, idx = 0. */
+int pcb_three_nn(const float* unknown, const float* known, int64_t B, int64_t n, int64_t m, float* dist2, int32_t* idx, void* stream);
+/* out[b, c, p] = features[b, c, idx[b, p]], p < L: gather_points (idx [B, M], L = M) and group_points (idx [B, M, S], L = M * S,
+ * out [B, C, M, S]).  An index outside [0, N) reads 0. */
+int pcb_gather_points(const float* features, const int32_t* idx, int64_t B, int64_t C, int64_t N, int64_t L, float* out, void* stream);
+/* out[b, c, j] = (f[i1] * w1 + f[i2] * w2) + f[i3] * w3 over features [B, C, m], idx / weight [B, n, 3]; out [B, C, n]. */
+int pcb_three_interpolate(const float* features, const int32_t* idx, const float* weight, int64_t B, int64_t C, int64_t m, int64_t n,
+                          float* out, void* stream);
+/* Adjoints, deterministic: every source point's readers are listed in ascending output position (stable radix sort of the index
+ * tensor) and summed in that order in fp64; grad_features is written in full (zeros where nothing reads).  ws: pcb_points_grad_ws_bytes(B,
+ * N, L) with L = readers per scene (M, M * S; 3 * n for three_interpolate, whose source count is m). */
+size_t pcb_points_grad_ws_bytes(int64_t B, int64_t N, int64_t L);
+int pcb_gather_points_grad(const float* grad_out, const int32_t* idx, int64_t B, int64_t C, int64_t N, int64_t L, float* grad_features,
+                           void* ws, size_t ws_bytes, void* stream);
+int pcb_three_interpolate_grad(const float* grad_out, const int32_t* idx, const float* weight, int64_t B, int64_t C, int64_t n, int64_t m,
+                               float* grad_features, void* ws, size_t ws_bytes, void* stream);
+
 /* ----------------------------------------------------------------------------------------------- optimiser */
 /* torch.optim.SGD semantics on a flat buffer:  d = g*grad_scale + wd*p;  buf = first ? d : momentum*buf + (1-dampening)*d;  p -= lr*buf
  * (pretraining: dampening 0, `lib/ddp_trainer.py:107-111`; semseg finetuning: 0.1, `downstream/semseg/lib/solvers.py:50-57`) */

@@ -75,6 +75,15 @@ _SIGS = {
     "pcb_unit_ws_bytes": (_sz, [_i, _l, _l, _i, _i]),
     "pcb_unit_forward": (_i, [_p, _p]),
     "pcb_unit_backward": (_i, [_p, _p]),
+    "pcb_furthest_point_sampling_ws_bytes": (_sz, [_l, _l]),
+    "pcb_furthest_point_sampling": (_i, [_p, _l, _l, _l, _p, _p, _sz, _p]),
+    "pcb_ball_query": (_i, [_p, _p, _l, _l, _l, _f, _i, _p, _p]),
+    "pcb_three_nn": (_i, [_p, _p, _l, _l, _l, _p, _p, _p]),
+    "pcb_gather_points": (_i, [_p, _p, _l, _l, _l, _l, _p, _p]),
+    "pcb_three_interpolate": (_i, [_p, _p, _p, _l, _l, _l, _l, _p, _p]),
+    "pcb_points_grad_ws_bytes": (_sz, [_l, _l, _l]),
+    "pcb_gather_points_grad": (_i, [_p, _p, _l, _l, _l, _l, _p, _p, _sz, _p]),
+    "pcb_three_interpolate_grad": (_i, [_p, _p, _p, _l, _l, _l, _l, _p, _p, _sz, _p]),
 }
 
 
