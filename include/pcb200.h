@@ -8,7 +8,7 @@
  *   pcb_coords_* / pcb_hash_* / pcb_kernel_map*   ME CoordsManager (CPU hash map): initialize, stride, getKernelMap.
  *        Reached implicitly from every `ME.SparseTensor(F, coords=C)` (pretrain/pointcontrast/lib/ddp_trainer.py:290-297,392-398)
  *        and every strided / 3x3x3 convolution (pretrain/pointcontrast/model/res16unet.py:47-190).
- *   pcb_conv_forward / pcb_conv_wgrad / pcb_weight_prep
+ *   pcb_conv_forward[_split] / pcb_conv_wgrad[_split] / pcb_weight_tile
  *        ME ConvolutionForwardGPU / ConvolutionBackwardGPU (and the Transpose variants), bound in ME's python as
  *        MinkowskiConvolutionFunction.apply(input_features, kernel, tensor_stride, stride, kernel_size, dilation,
  *        region_type, region_offset, in_coords_key, out_coords_key, coords_manager) -- signature evidenced by
@@ -103,30 +103,19 @@ int pcb_radius_pairs(const float* src, int64_t ns, const float* dst, int64_t nd,
                      int64_t* n_pairs, void* ws, size_t ws_bytes, void* stream);
 
 /* ----------------------------------------------------------------------------------------------- convolution */
-/* fp32 W[K][Cin][Cout] -> bf16 hi/lo split planes in the same layout (w_hi, w_lo) and per-offset transposed
- * [K][Cout][Cin] (wt_hi, wt_lo).  x ~= hi + lo with |x - hi - lo| <= 2^-17 |x|. */
-int pcb_weight_prep(const float* W, int K, int Cin, int Cout, uint16_t* w_hi, uint16_t* w_lo,
-                    uint16_t* wt_hi, uint16_t* wt_lo, void* stream);
-
-/* Y[j, :] = bias + sum_k X[tbl[kmap[k]][j], :] . W[k]      (j < n_out)      -- fp32 operands (the modular ME-style surface)
- *   X  : [*, Cin] row stride ldx (floats);  Y: [n_out, Cout] row stride ldy.
- *   wk_hi/wk_lo : the weights of THIS call's roles as bf16 hi/lo planes, K-major = [K][Cout][Cin] (pcb_weight_prep: the wt_* planes for
- *               the forward roles; the w_* planes with swapped channel counts for the data gradient).  Tensor-core path (wgmma, fp32 rows
- *               split to bf16 hi/lo in the producers' registers, fp32 accumulate in registers): Cin % 32 == 0, Cout % 32 == 0, K <= 27.
- *   w_f32     : fp32 weights [K][Cin][Cout] for the exact SIMT path (other widths, the 3-channel stem, PCB_CONV_FORCE_SIMT); may be NULL
- *               when the tensor-core path applies.
- *   kmap      : HOST int32 [K] table row used by weight k (NULL = identity). */
-#define PCB_CONV_FORCE_SIMT 1
-#define PCB_CONV_ACCUMULATE 4  /* Y += result (tensor-core paths) / dW += result (weight gradients) */
+/* Y[j, :] = bias + sum_k X[tbl[kmap[k]][j], :] . W[k]      (j < n_out)      -- EXACT fp32, any channel counts
+ *   X  : [*, Cin] row stride ldx (floats);  Y: [n_out, Cout] row stride ldy;  W: fp32 [K][Cin][Cout];  bias: [Cout] or NULL.
+ *   kmap : HOST int32 [K] table row used by weight k (NULL = identity).
+ * The 3 -> 32 stem layer runs a dedicated kernel, every other width a generic SIMT kernel.  The tensor-core forward / data gradient is
+ * pcb_conv_forward_split on split operands. */
+int pcb_conv_forward(const float* X, int ldx, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap, int K,
+                     int64_t n_out, int Cin, int Cout, const float* W, const float* bias, float* Y, int ldy, void* stream);
+#define PCB_CONV_FORCE_SIMT 1  /* pcb_conv_wgrad: the generic exact kernel also for the stem layer (a cross-check of the stem kernel) */
+#define PCB_CONV_ACCUMULATE 4  /* Y += result (pcb_conv_forward_split) / dW += result (weight gradients) */
 #define PCB_PLANES_A_FP16 8    /* split-operand calls: the GATHERED operand's planes are fp16 hi/lo (default: bf16 hi/lo) */
 #define PCB_PLANES_B_FP16 16   /* pcb_conv_forward_split: the weight tiles are fp16 x 2^10 (pcb_weight_tile with this flag);
                                   pcb_conv_wgrad_split: the ROW-ALIGNED operand's planes are fp16.  Both operands of a call must
                                   use the same format (wgmma takes one 16-bit format for both operands): set both flags or neither. */
-/* Small levels split the (offset, channel-chunk) loop over extra CTAs and reduce through `ws` (deterministic). */
-size_t pcb_conv_forward_ws_bytes(int K, int64_t n_out, int Cin, int Cout);
-int pcb_conv_forward(const float* X, int ldx, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap, int K,
-                     int64_t n_out, int Cin, int Cout, const uint16_t* wk_hi, const uint16_t* wk_lo, const float* w_f32,
-                     const float* bias, float* Y, int ldy, void* ws, size_t ws_bytes, int flags, void* stream);
 
 /* Y[j, :] = sum_k X[tbl[kmap[k]][j], :];  cnt[j] (optional) = number of neighbours present.  The sum / average pooling and unpooling
  * layers of the sibling models (MinkowskiSumPooling / AvgPooling / PoolingTranspose / AvgUnpooling, `model/modules/common.py:170-214`,
@@ -143,9 +132,10 @@ int pcb_conv_wgrad(const float* A, int lda, const float* B, int ldb, const int32
                    int64_t n_out, int Ca, int Cb, float* dW, int transpose_out, void* ws, size_t ws_bytes,
                    int flags, void* stream);
 
-/* Split-operand variants (tensor-core path only): the gathered / row-aligned operands are bf16 hi/lo planes (see pcb_split_rows),
- * row strides lds/lda/ldb in ELEMENTS (multiples of 8).  Same semantics as pcb_conv_forward / pcb_conv_wgrad; the kernels'
- * operand staging is then a pure asynchronous copy (cp.async, zero-filled where a neighbour is missing). */
+/* Split-operand variants (tensor-core path; Cin, Cout multiples of 32): the gathered / row-aligned operands are 16-bit hi/lo planes
+ * (see pcb_split_rows), row strides lds/lda/ldb in ELEMENTS (multiples of 8), and the convolution's weights are pre-tiled by
+ * pcb_weight_tile[_batch].  Same semantics as pcb_conv_forward / pcb_conv_wgrad; the kernels' operand staging is then a pure
+ * asynchronous copy (cp.async, zero-filled where a neighbour is missing, and one TMA bulk copy per weight tile). */
 /* pcb_weight_tile: fp32 W[K][Cin][Cout] -> split weights pre-tiled as the shared-memory images of the split conv kernel (one
  * contiguous blob per (offset, 32-channel chunk, column block), fetched by ONE TMA bulk copy per pipeline stage):
  * `fwd_tiles` for the forward roles, `dgrad_tiles` for the data-gradient roles (Cin/Cout swapped).  flags & PCB_PLANES_B_FP16:
@@ -161,6 +151,9 @@ typedef struct pcb_tile_desc {
 } pcb_tile_desc;
 int pcb_tile_desc_fill(pcb_tile_desc* d, const float* W, int K, int Cin, int Cout, void* fwd_tiles, void* dgrad_tiles, int flags, int64_t start);
 int pcb_weight_tile_batch(const pcb_tile_desc* descs_dev, int n, int64_t total, void* stream);
+/* Small levels split the (offset, channel-chunk) loop of pcb_conv_forward_split over extra CTAs and reduce through `ws`
+ * (deterministic). */
+size_t pcb_conv_forward_split_ws_bytes(int K, int64_t n_out, int Cin, int Cout);
 int pcb_conv_forward_split(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride,
                            const int32_t* kmap, int K, int64_t n_out, int Cin, int Cout, const void* w_tiles,
                            const float* bias, float* Y, int ldy, void* ws, size_t ws_bytes, int flags, void* stream);

@@ -40,9 +40,7 @@ _SIGS = {
     "pcb_radius_pairs": (_i, [_p, _l, _p, _l, _f, _p, _l, C.POINTER(C.c_int64), _p, _sz, _p]),
     "pcb_kernel_map": (_i, [_p, _l, _p, _p, _l, _p, _i, _p, _p]),
     "pcb_kernel_map_count": (_i, [_p, _i, _l, _p, _p]),
-    "pcb_weight_prep": (_i, [_p, _i, _i, _i, _p, _p, _p, _p, _p]),
-    "pcb_conv_forward_ws_bytes": (_sz, [_i, _l, _i, _i]),
-    "pcb_conv_forward": (_i, [_p, _i, _p, _l, _p, _i, _l, _i, _i, _p, _p, _p, _p, _p, _i, _p, _sz, _i, _p]),
+    "pcb_conv_forward": (_i, [_p, _i, _p, _l, _p, _i, _l, _i, _i, _p, _p, _p, _i, _p]),
     "pcb_gather_sum": (_i, [_p, _i, _p, _l, _p, _i, _l, _i, _p, _i, _p, _p]),
     "pcb_conv_wgrad_ws_bytes": (_sz, [_i, _l, _i, _i]),
     "pcb_conv_wgrad": (_i, [_p, _i, _p, _i, _p, _l, _i, _l, _i, _i, _p, _i, _p, _sz, _i, _p]),
@@ -50,6 +48,7 @@ _SIGS = {
     "pcb_weight_tile": (_i, [_p, _i, _i, _i, _p, _p, _i, _p]),
     "pcb_tile_desc_fill": (_i, [_p, _p, _i, _i, _i, _p, _p, _i, _l]),
     "pcb_weight_tile_batch": (_i, [_p, _i, _l, _p]),
+    "pcb_conv_forward_split_ws_bytes": (_sz, [_i, _l, _i, _i]),
     "pcb_conv_forward_split": (_i, [_p, _p, _i, _p, _l, _p, _i, _l, _i, _i, _p, _p, _p, _i, _p, _sz, _i, _p]),
     "pcb_conv_wgrad_split_ws_bytes": (_sz, [_i, _l, _i, _i]),
     "pcb_conv_wgrad_split": (_i, [_p, _p, _i, _p, _p, _i, _p, _l, _i, _l, _i, _i, _p, _i, _p, _sz, _i, _p]),

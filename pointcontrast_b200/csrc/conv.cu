@@ -6,11 +6,12 @@
 // Replaces MinkowskiEngine 0.4.3 ConvolutionForwardGPU / ConvolutionBackwardGPU (+Transpose): per-offset
 // gather -> SIMT matmul -> atomicAdd scatter, K launches per layer (reference call sites in include/pcb200.h).
 //
-// Numerics: the contraction runs on the tensor cores as a 3-term bf16 split (x = hi + lo):
+// Numerics: the tensor-core entry points (pcb_conv_forward_split / pcb_conv_wgrad_split, kernels in conv_wgmma.cu) take their
+// operands as 16-bit hi/lo planes (x = hi + lo) and run the contraction as a 3-term split:
 //   x.w ~= hi.hi + lo.hi + hi.lo,  fp32 accumulate  ->  per-product relative error <= ~2^-16, i.e. fp32-class
-// parity (tests: 1e-3 relative against the fp64 oracle after 63 layers).  An exact fp32 SIMT kernel with the
-// same interface covers channel counts the tensor-core tiling does not (Cin = 3) and is the in-library
-// cross-check (PCB_CONV_FORCE_SIMT).
+// parity (tests: 1e-3 relative against the fp64 oracle after 63 layers).  The exact fp32 entry points (pcb_conv_forward /
+// pcb_conv_wgrad) cover the channel counts the tensor-core tiling does not (Cin = 3, odd widths) and are the in-library
+// cross-check of the tensor-core ones.
 #include <stdlib.h>
 #include <cuda_fp16.h>
 #include "common.cuh"
@@ -217,25 +218,6 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int split
   dW[i] = accumulate ? dW[i] + s : s;
 }
 
-// --------------------------------------------------------------------------------------------- weight preparation
-__global__ void weight_prep_kernel(const float* __restrict__ W, int K, int Cin, int Cout, __nv_bfloat16* __restrict__ hi,
-                                   __nv_bfloat16* __restrict__ lo, __nv_bfloat16* __restrict__ thi,
-                                   __nv_bfloat16* __restrict__ tlo) {
-  int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  int64_t n = (int64_t)K * Cin * Cout;
-  if (e >= n) return;
-  float w = W[e];
-  __nv_bfloat16 h = __float2bfloat16_rn(w);
-  __nv_bfloat16 l = __float2bfloat16_rn(w - __bfloat162float(h));
-  hi[e] = h; lo[e] = l;
-  int co = (int)(e % Cout);
-  int64_t r = e / Cout;
-  int ci = (int)(r % Cin);
-  int64_t k = r / Cin;
-  int64_t te = (k * Cout + co) * Cin + ci;
-  thi[te] = h; tlo[te] = l;
-}
-
 int pick_tile(int C) {      // largest of {128, 96, 64, 32} dividing C
   if (C % 128 == 0) return 128;
   if (C % 96 == 0) return 96;
@@ -273,69 +255,34 @@ int wgrad_splits(int K, int64_t n_out, int Ca, int Cb, int tm, int tn) {
 
 }  // namespace
 
-extern "C" int pcb_weight_prep(const float* W, int K, int Cin, int Cout, uint16_t* w_hi, uint16_t* w_lo,
-                               uint16_t* wt_hi, uint16_t* wt_lo, void* stream) {
-  PCB_ARG(W && w_hi && w_lo && wt_hi && wt_lo && K >= 1 && Cin >= 1 && Cout >= 1);
-  int64_t n = (int64_t)K * Cin * Cout;
-  weight_prep_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      W, K, Cin, Cout, (__nv_bfloat16*)w_hi, (__nv_bfloat16*)w_lo, (__nv_bfloat16*)wt_hi, (__nv_bfloat16*)wt_lo);
-  return check_launch("weight_prep_kernel");
-}
-
 namespace pcb {
 int wgrad_group();
 int launch_wgrad_wgmma(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
                          const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int Ca, int Cb, int rows_per_split, int splits,
                          float* partial, int transpose_out, int tn, cudaStream_t st, int a_fp16 = 0, int b_fp16 = 0);
-int launch_conv_wgmma(const float* X, int ldx, const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl,
-                        int64_t tbl_stride, const int* kmap, int K, int64_t n_out,
-                        int Cin, int Cout, const uint16_t* wk_hi, const uint16_t* wk_lo, const float* bias, float* Y, int ldy,
-                        float* partial, int nsplit, int bn, int accumulate, cudaStream_t st, int x_fp16 = 0, int w_fp16 = 0);
+int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl, int64_t tbl_stride,
+                      const int* kmap, int K, int64_t n_out, int Cin, int Cout, const float* bias, float* Y, int ldy,
+                      float* partial, int nsplit, int bn, int accumulate, cudaStream_t st, int x_fp16, int w_fp16);
 }
 
-extern "C" size_t pcb_conv_forward_ws_bytes(int K, int64_t n_out, int Cin, int Cout) {
-  if (Cin % 32 || Cout % 32 || n_out <= 0) return 256;
-  int s = conv_splits(K, n_out, Cin, Cout);
-  return s > 1 ? (size_t)s * n_out * Cout * sizeof(float) + 256 : 256;
-}
-
+// Exact fp32 forward / data gradient: the stem kernel for the 3 -> 32 layer, the generic SIMT kernel for every other width.
 extern "C" int pcb_conv_forward(const float* X, int ldx, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap, int K,
-                                int64_t n_out, int Cin, int Cout,
-                                const uint16_t* wk_hi, const uint16_t* wk_lo, const float* w_f32, const float* bias, float* Y,
-                                int ldy, void* ws, size_t ws_bytes, int flags, void* stream) {
+                                int64_t n_out, int Cin, int Cout, const float* W, const float* bias, float* Y, int ldy, void* stream) {
   PCB_ARG(K >= 1 && K <= PCB_MAX_KERNEL_VOLUME && n_out >= 0 && Cin >= 1 && Cout >= 1 && ldx >= Cin && ldy >= Cout);
   if (n_out == 0) return PCB_OK;
-  PCB_ARG(X && tbl && Y && tbl_stride >= n_out);
+  PCB_ARG(X && tbl && W && Y && tbl_stride >= n_out);
   cudaStream_t st = (cudaStream_t)stream;
   ProfScope prof(st, 0);
   KMap km;
   for (int k = 0; k < K; ++k) { km.v[k] = kmap ? kmap[k] : k; PCB_ARG(km.v[k] >= 0 && km.v[k] < PCB_MAX_KERNEL_VOLUME); }
-  const bool tc_ok = (Cin % 32 == 0) && (Cout % 32 == 0) && (ldx % 4 == 0) && wk_hi && wk_lo && !(flags & PCB_CONV_FORCE_SIMT);
-  if (!tc_ok) {
-    if (flags & PCB_CONV_ACCUMULATE) { set_error("PCB_CONV_ACCUMULATE needs the tensor-core path"); return PCB_ERR_ARG; }
-    if (!w_f32) { set_error("pcb_conv_forward: SIMT path needs w_f32 (Cin=%d Cout=%d)", Cin, Cout); return PCB_ERR_ARG; }
-    if (Cin == 3 && Cout == 32) {         // the stem layer
-      launch_kernel(conv_stem_kernel<3>, (unsigned)((n_out + 127) / 128), 128, 0, st, X, ldx, tbl, tbl_stride, km, K, n_out, w_f32, bias, Y, ldy);
-      return check_launch("conv_stem_kernel");
-    }
-    int64_t total = n_out * Cout;
-    launch_kernel(conv_simt_kernel, (unsigned)((total + 255) / 256), 256, 0, st, X, ldx, tbl, tbl_stride, km, K, n_out, Cin, Cout,
-                                                                      w_f32, bias, Y, ldy);
-    return check_launch("conv_simt_kernel");
+  if (Cin == 3 && Cout == 32) {         // the stem layer
+    launch_kernel(conv_stem_kernel<3>, (unsigned)((n_out + 127) / 128), 128, 0, st, X, ldx, tbl, tbl_stride, km, K, n_out, W, bias, Y, ldy);
+    return check_launch("conv_stem_kernel");
   }
-  // tensor-core path: the wgmma kernel on fp32 inputs (split to bf16 hi/lo in the producers' registers), K-major weight planes
-  if (!(wk_hi && wk_lo && ldy % 4 == 0)) { set_error("pcb_conv_forward: the tensor-core path needs the K-major planes wk_hi / wk_lo"); return PCB_ERR_ARG; }
-  const int nsplit = conv_splits(K, n_out, Cin, Cout);
-  if (nsplit > 1) PCB_ARG(ws && ws_bytes >= (size_t)nsplit * n_out * Cout * sizeof(float));
-  const int accumulate = (flags & PCB_CONV_ACCUMULATE) ? 1 : 0;
-  if (int e = launch_conv_wgmma(X, ldx, nullptr, nullptr, 0, nullptr, tbl, tbl_stride, km.v, K, n_out, Cin, Cout, wk_hi, wk_lo, bias, Y, ldy,
-                                nsplit > 1 ? (float*)ws : nullptr, nsplit, pick_tile(Cout), accumulate, st)) return e;
-  if (nsplit > 1) {
-    int64_t n4 = n_out * (Cout / 4);
-    launch_kernel(conv_split_reduce_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, (const float*)ws, nsplit, n_out, Cout, bias, Y, ldy, accumulate);
-    return check_launch("conv_split_reduce_kernel");
-  }
-  return PCB_OK;
+  int64_t total = n_out * Cout;
+  launch_kernel(conv_simt_kernel, (unsigned)((total + 255) / 256), 256, 0, st, X, ldx, tbl, tbl_stride, km, K, n_out, Cin, Cout,
+                                                                    W, bias, Y, ldy);
+  return check_launch("conv_simt_kernel");
 }
 
 extern "C" int pcb_gather_sum(const float* X, int ldx, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap, int K, int64_t n_out, int C,
@@ -583,7 +530,7 @@ int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, c
   const int nsplit = conv_splits(K, n_out, Cin, Cout);
   if (nsplit > 1) PCB_ARG(ws && ws_bytes >= (size_t)nsplit * n_out * Cout * sizeof(float));
   if (bn) PCB_ARG(!bias && !accumulate && bn->n0 >= 1 && bn->n0 <= n_out && bn_done);
-  if (int e = launch_conv_wgmma(nullptr, 0, Xhi, Xlo, lds, w_tiles, tbl, tbl_stride, km, K, n_out, Cin, Cout, nullptr, nullptr, bias, Y, ldy,
+  if (int e = launch_conv_wgmma(Xhi, Xlo, lds, w_tiles, tbl, tbl_stride, km, K, n_out, Cin, Cout, bias, Y, ldy,
                                 nsplit > 1 ? (float*)ws : nullptr, nsplit, pick_tile(Cout), accumulate, st,
                                 (flags & PCB_PLANES_A_FP16) ? 1 : 0, (flags & PCB_PLANES_B_FP16) ? 1 : 0)) return e;
   if (nsplit > 1) {
@@ -599,6 +546,12 @@ int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, c
   return PCB_OK;
 }
 }  // namespace pcb
+
+extern "C" size_t pcb_conv_forward_split_ws_bytes(int K, int64_t n_out, int Cin, int Cout) {
+  if (Cin % 32 || Cout % 32 || n_out <= 0) return 256;
+  int s = conv_splits(K, n_out, Cin, Cout);
+  return s > 1 ? (size_t)s * n_out * Cout * sizeof(float) + 256 : 256;
+}
 
 extern "C" int pcb_conv_forward_split(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride,
                                       const int32_t* kmap, int K, int64_t n_out, int Cin, int Cout, const void* w_tiles,

@@ -1,9 +1,8 @@
 // Hopper sparse convolution: the output-stationary gather-GEMM of conv.cu with the per-offset Cin x Cout contraction issued as
-// wgmma.mma_async, fp32 accumulators in registers.  CTA = 128 output rows x BN channels = two warpgroups of M64.  Every thread
-// gathers the neighbour rows of the current offset as 16-bit hi/lo planes in the K-major no-swizzle core-matrix layout; per
-// 32-channel step each warpgroup issues 2 k16-steps x 3 products (lo.hi + hi.lo + hi.hi).  SPLIT = false takes fp32 rows (split in
-// registers) and K-major weight planes (modular surface); SPLIT = true takes 16-bit planes (cp.async gathers, zero-filled where there
-// is no neighbour) and pre-tiled weight images (one TMA bulk copy per stage on an mbarrier).  Offsets without a neighbour in the
+// wgmma.mma_async, fp32 accumulators in registers.  CTA = 128 output rows x BN channels = two warpgroups of M64.  The input arrives as
+// 16-bit hi/lo planes, gathered per offset by cp.async (zero-filled where there is no neighbour) into the K-major no-swizzle
+// core-matrix layout; the weights arrive pre-tiled as shared-memory images, one TMA bulk copy per stage on an mbarrier.  Per
+// 32-channel step each warpgroup issues 2 k16-steps x 3 products (lo.hi + hi.lo + hi.hi).  Offsets without a neighbour in the
 // tile are skipped; small levels split the steps over gridDim.z (partial planes + fixed-order reduce).
 #include "common.cuh"
 #include "wgmma_ptx.cuh"
@@ -13,16 +12,6 @@ using namespace pcb;
 namespace pcb {
 
 namespace hw {
-
-__device__ __forceinline__ void split4(const float4& v, uint2& hi, uint2& lo) {
-  __nv_bfloat162 h0 = __floats2bfloat162_rn(v.x, v.y);
-  __nv_bfloat162 h1 = __floats2bfloat162_rn(v.z, v.w);
-  float2 f0 = __bfloat1622float2(h0), f1 = __bfloat1622float2(h1);
-  __nv_bfloat162 l0 = __floats2bfloat162_rn(v.x - f0.x, v.y - f0.y);
-  __nv_bfloat162 l1 = __floats2bfloat162_rn(v.z - f1.x, v.w - f1.y);
-  hi.x = *reinterpret_cast<uint32_t*>(&h0); hi.y = *reinterpret_cast<uint32_t*>(&h1);
-  lo.x = *reinterpret_cast<uint32_t*>(&l0); lo.y = *reinterpret_cast<uint32_t*>(&l1);
-}
 
 // NS-slot ring, loads PF = NS - 2 steps ahead: the slot written at step i was last read by the MMAs of step i - 2, which every
 // warpgroup has waited for (wgmma.wait_group 1) before the barrier of step i - 1.
@@ -34,13 +23,11 @@ constexpr int A_LBO = (BM / 8) * 128 + 32;
 constexpr int A_PLANE = (BK / 8) * A_LBO;
 
 struct Args {
-  const float* X; int ldx;
-  const __nv_bfloat16* Xhi; const __nv_bfloat16* Xlo; int lds;      // SPLIT kernel: the input as 16-bit hi/lo planes
+  const __nv_bfloat16* Xhi; const __nv_bfloat16* Xlo; int lds;      // the input as 16-bit hi/lo planes
   const int32_t* tbl; int64_t tbl_stride;
   int kmap[PCB_MAX_KERNEL_VOLUME]; int K;
   int64_t n_out; int Cin; int Cout;
-  const __nv_bfloat16* wk_hi; const __nv_bfloat16* wk_lo;      // K-major weights: [K][Cout][Cin]
-  const unsigned char* wt;                                      // SPLIT kernel: weights pre-tiled as shared-memory images
+  const unsigned char* wt;                                      // weights pre-tiled as shared-memory images
   const float* bias;
   float* Y; int ldy;
   float* partial;
@@ -60,7 +47,7 @@ struct Smem {
   static constexpr int TOTAL = BAR_OFF + NS * 8 + 16;
 };
 
-template <int BN, bool SPLIT, bool F16>
+template <int BN, bool F16>
 __global__ void __launch_bounds__(NTHR, 1) conv_wgmma_kernel(const Args p) {
   using S = Smem<BN>;
   extern __shared__ __align__(128) unsigned char smem[];
@@ -72,9 +59,9 @@ __global__ void __launch_bounds__(NTHR, 1) conv_wgmma_kernel(const Args p) {
   int* s_klist = s_flag + 32;
   int* s_nk = s_klist + 32;
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full_bar = smem_base + S::BAR_OFF;          // SPLIT: "weight tile of slot s landed"
+  const uint32_t full_bar = smem_base + S::BAR_OFF;          // "weight tile of slot s landed"
 
-  if (SPLIT && tid == 0) {
+  if (tid == 0) {
     for (int i = 0; i < NS; ++i) mbar_init(full_bar + 8 * i, 1);
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
@@ -126,61 +113,25 @@ __global__ void __launch_bounds__(NTHR, 1) conv_wgmma_kernel(const Args p) {
   constexpr uint32_t BLOB = 2 * S::B_PLANE;
 
   // ---- pipeline step i (relative to it0) uses slot i % NS
-  const int a_chunk = tid & 7, a_row = tid >> 3;         // fp32 path: (row, 4-float chunk) of the 32-channel slice
-  float4 v[4];
-  // fp32 path: the gathered rows of step i -> registers
-  auto load_regs = [&](int i) {
-    const int it = it0 + i;
-    const int k = s_klist[it / nkc], kc = it % nkc;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int idx = s_idx[k * BM + a_row + 32 * j];
-      if (idx >= 0) v[j] = __ldg(reinterpret_cast<const float4*>(p.X + (int64_t)idx * p.ldx + kc * BK) + a_chunk);
-      else v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-  };
-  // fp32 path: the registers of step i -> bf16 hi/lo planes
-  auto store_A = [&](int i) {
-    unsigned char* base = smem + (i % NS) * S::STAGE + (a_chunk >> 1) * A_LBO + (a_chunk & 1) * 8;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int r = a_row + 32 * j;
-      uint2 hi, lo;
-      split4(v[j], hi, lo);
-      const int off = (r >> 3) * A_SBO + (r & 7) * 16;
-      *reinterpret_cast<uint2*>(base + off) = hi;
-      *reinterpret_cast<uint2*>(base + A_PLANE + off) = lo;
-    }
-  };
   // asynchronous copies of step i: one cp.async group per call (possibly empty)
   auto load_async = [&](int i) {
     if (i < n_it) {
       const int it = it0 + i, s = i % NS;
       const int k = s_klist[it / nkc], kc = it % nkc;
       const uint32_t sb = smem_base + s * S::STAGE;
-      if (SPLIT) {
-        // A: 128 rows x 4 k8-chunks x 2 planes of 16 bytes, zero-filled where there is no neighbour
+      // A: 128 rows x 4 k8-chunks x 2 planes of 16 bytes, zero-filled where there is no neighbour
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int c = tid + j * NTHR;
-          const int plane = c >> 9, rem = c & 511, r = rem >> 2, k8 = rem & 3;
-          const int idx = s_idx[k * BM + r];
-          const __nv_bfloat16* src = (plane ? p.Xlo : p.Xhi) + (int64_t)(idx >= 0 ? idx : 0) * p.lds + kc * BK + k8 * 8;
-          cp_async16_zfill(sb + plane * A_PLANE + k8 * A_LBO + (r >> 3) * A_SBO + (r & 7) * 16, src, idx >= 0 ? 16u : 0u);
-        }
-        // B: the stage's weight tile is one TMA bulk copy of the pre-tiled image
-        if (tid == 0) {
-          mbar_arrive_expect_tx(full_bar + 8 * s, BLOB);
-          tma_bulk_load(sb + 2 * A_PLANE, p.wt + ((int64_t)(k * nkc + kc) * nblk + blockIdx.y) * BLOB, BLOB, full_bar + 8 * s);
-        }
-      } else {
-        constexpr int PER_PLANE = BN * (BK / 8);             // 16-byte chunks: BN rows x 4 k-chunks
-        for (int c = tid; c < 2 * PER_PLANE; c += NTHR) {
-          const int plane = c / PER_PLANE, rem = c - plane * PER_PLANE;
-          const int n = rem >> 2, k8 = rem & 3;
-          const __nv_bfloat16* src = (plane ? p.wk_lo : p.wk_hi) + ((int64_t)k * p.Cout + n0 + n) * p.Cin + kc * BK + k8 * 8;
-          cp_async16(sb + 2 * A_PLANE + plane * S::B_PLANE + k8 * S::B_LBO + (n >> 3) * S::B_SBO + (n & 7) * 16, src);
-        }
+      for (int j = 0; j < 4; ++j) {
+        const int c = tid + j * NTHR;
+        const int plane = c >> 9, rem = c & 511, r = rem >> 2, k8 = rem & 3;
+        const int idx = s_idx[k * BM + r];
+        const __nv_bfloat16* src = (plane ? p.Xlo : p.Xhi) + (int64_t)(idx >= 0 ? idx : 0) * p.lds + kc * BK + k8 * 8;
+        cp_async16_zfill(sb + plane * A_PLANE + k8 * A_LBO + (r >> 3) * A_SBO + (r & 7) * 16, src, idx >= 0 ? 16u : 0u);
+      }
+      // B: the stage's weight tile is one TMA bulk copy of the pre-tiled image
+      if (tid == 0) {
+        mbar_arrive_expect_tx(full_bar + 8 * s, BLOB);
+        tma_bulk_load(sb + 2 * A_PLANE, p.wt + ((int64_t)(k * nkc + kc) * nblk + blockIdx.y) * BLOB, BLOB, full_bar + 8 * s);
       }
     }
     cp_async_commit();
@@ -190,17 +141,12 @@ __global__ void __launch_bounds__(NTHR, 1) conv_wgmma_kernel(const Args p) {
 #pragma unroll
   for (int e = 0; e < BN / 2; ++e) acc[e] = 0.f;
   if (n_it > 0) {
-    if (!SPLIT) load_regs(0);
 #pragma unroll 1
     for (int i = 0; i < PF; ++i) load_async(i);
     for (int i = 0; i < n_it; ++i) {
       const int s = i % NS;
-      if (!SPLIT) {                                    // fp32 path: A goes through registers one step ahead
-        store_A(i);
-        if (i + 1 < n_it) load_regs(i + 1);
-      }
       cp_async_wait<PF - 1>();                         // this thread's copies of step i have landed
-      if (SPLIT) mbar_wait(full_bar + 8 * s, (uint32_t)((i / NS) & 1));
+      mbar_wait(full_bar + 8 * s, (uint32_t)((i / NS) & 1));
       fence_proxy_async();                             // generic-proxy smem writes -> visible to the tensor cores (async proxy)
       __syncthreads();
       const uint32_t a_hi = smem_base + s * S::STAGE + wg * 8 * A_SBO, a_lo = a_hi + A_PLANE;
@@ -248,32 +194,30 @@ __global__ void __launch_bounds__(NTHR, 1) conv_wgmma_kernel(const Args p) {
   }
 }
 
-template <int BN, bool SPLIT, bool F16>
+template <int BN, bool F16>
 int launch_cfg(const Args& a, int nsplit, cudaStream_t st) {
   using S = Smem<BN>;
   static bool attr_set[64] = {};          // per device: the opt-in is a per-device function attribute
   const int dev_ = current_device();
   if (!attr_set[dev_]) {
-    PCB_CUDA(cudaFuncSetAttribute(conv_wgmma_kernel<BN, SPLIT, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+    PCB_CUDA(cudaFuncSetAttribute(conv_wgmma_kernel<BN, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     attr_set[dev_] = true;
   }
   dim3 grid((unsigned)((a.n_out + BM - 1) / BM), a.Cout / BN, nsplit);
-  launch_kernel(conv_wgmma_kernel<BN, SPLIT, F16>, grid, NTHR, S::TOTAL, st, a);
-  return check_launch(SPLIT ? "conv_wgmma_kernel<split>" : "conv_wgmma_kernel");
+  launch_kernel(conv_wgmma_kernel<BN, F16>, grid, NTHR, S::TOTAL, st, a);
+  return check_launch("conv_wgmma_kernel");
 }
 
 template <int BN>
 int launch(const Args& a, int nsplit, cudaStream_t st, int f16) {
-  if (!a.Xhi) return launch_cfg<BN, false, false>(a, nsplit, st);
-  return f16 ? launch_cfg<BN, true, true>(a, nsplit, st) : launch_cfg<BN, true, false>(a, nsplit, st);
+  return f16 ? launch_cfg<BN, true>(a, nsplit, st) : launch_cfg<BN, false>(a, nsplit, st);
 }
 
 }  // namespace hw
 
-// Called by pcb_conv_forward / conv_forward_split_impl (conv.cu).  wk_*: K-major split weights [K][Cout][Cin] for this call's roles.
-int launch_conv_wgmma(const float* X, int ldx, const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl,
-                      int64_t tbl_stride, const int* kmap, int K, int64_t n_out,
-                      int Cin, int Cout, const uint16_t* wk_hi, const uint16_t* wk_lo, const float* bias, float* Y, int ldy,
+// Called by conv_forward_split_impl (conv.cu).  wt: the weights of this call's roles pre-tiled by pcb_weight_tile[_batch].
+int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl, int64_t tbl_stride,
+                      const int* kmap, int K, int64_t n_out, int Cin, int Cout, const float* bias, float* Y, int ldy,
                       float* partial, int nsplit, int bn, int accumulate, cudaStream_t st, int x_fp16, int w_fp16) {
   // wgmma takes ONE 16-bit format for both operands
   if (x_fp16 != w_fp16) { set_error("conv: fp16 and bf16 operand planes cannot be mixed"); return PCB_ERR_ARG; }
@@ -282,9 +226,9 @@ int launch_conv_wgmma(const float* X, int ldx, const uint16_t* Xhi, const uint16
   a.out_scale = w_fp16 ? 1.0f / 1024.0f : 1.0f;
   a.Xhi = (const __nv_bfloat16*)Xhi; a.Xlo = (const __nv_bfloat16*)Xlo; a.lds = lds;
   a.wt = (const unsigned char*)wt;
-  a.X = X; a.ldx = ldx; a.tbl = tbl; a.tbl_stride = tbl_stride; a.K = K; a.n_out = n_out; a.Cin = Cin; a.Cout = Cout;
+  a.tbl = tbl; a.tbl_stride = tbl_stride; a.K = K; a.n_out = n_out; a.Cin = Cin; a.Cout = Cout;
   for (int k = 0; k < K; ++k) a.kmap[k] = kmap[k];
-  a.wk_hi = (const __nv_bfloat16*)wk_hi; a.wk_lo = (const __nv_bfloat16*)wk_lo; a.bias = bias; a.Y = Y; a.ldy = ldy;
+  a.bias = bias; a.Y = Y; a.ldy = ldy;
   a.partial = partial;
   switch (bn) {
     case 128: return hw::launch<128>(a, nsplit, st, x_fp16);

@@ -86,7 +86,7 @@ inline bool tensor_core_shape(int Cin, int Cout) { return Cin % 32 == 0 && Cout 
 
 // scratch layout: [convolution scratch (largest of forward / data gradient / weight gradient) | BatchNorm partial sums]
 size_t conv_part_bytes(int K, int64_t n_in, int64_t n_out, int Cin, int Cout) {
-  size_t a = pcb_conv_forward_ws_bytes(K, n_out, Cin, Cout), b = pcb_conv_forward_ws_bytes(K, n_in, Cout, Cin);
+  size_t a = pcb_conv_forward_split_ws_bytes(K, n_out, Cin, Cout), b = pcb_conv_forward_split_ws_bytes(K, n_in, Cout, Cin);
   size_t c = tensor_core_shape(Cin, Cout) ? pcb_conv_wgrad_split_ws_bytes(K, n_out > n_in ? n_out : n_in, Cin, Cout)
                                           : pcb_conv_wgrad_ws_bytes(K, n_out > n_in ? n_out : n_in, Cin, Cout);
   size_t d = tensor_core_shape(Cin, Cout) ? pcb_conv_wgrad_split_ws_bytes(K, n_out > n_in ? n_out : n_in, Cout, Cin) : 0;
@@ -121,8 +121,8 @@ extern "C" int pcb_unit_forward(const pcb_unit* u, void* stream) {
                                         st, fuse ? &bn : nullptr, &have_stats)) return e;
   } else {
     PCB_ARG(u->x_p && u->W);
-    if (int e = pcb_conv_forward(u->x_p, u->x_ld, u->fwd_tbl, u->fwd_stride, u->fwd_kmap, u->K, u->n_out, u->Cin, u->Cout,
-                                 nullptr, nullptr, u->W, nullptr, u->z_p, u->z_ld, nullptr, 0, 0, stream)) return e;
+    if (int e = pcb_conv_forward(u->x_p, u->x_ld, u->fwd_tbl, u->fwd_stride, u->fwd_kmap, u->K, u->n_out, u->Cin, u->Cout, u->W,
+                                 nullptr, u->z_p, u->z_ld, stream)) return e;
   }
   ProfScope prof(st, 2);                     // BatchNorm forward: statistics (unless fused into the split reduction) + normalise / residual / ReLU / planes
   if (u->flags & PCB_UNIT_EVAL) {            // eval-mode BatchNorm (`downstream/semseg/lib/test.py:95-117`): normalise with the running statistics

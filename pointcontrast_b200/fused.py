@@ -250,15 +250,6 @@ def _plane_i16(p, n, C, ld, device):
         return torch.as_tensor(_Plane(p, n, C, ld), device=device)
 
 
-def _kmap(plan, which):
-    """HOST int32 array of a plan's kernel-offset permutation (cached on the plan) or None."""
-    cache = plan._c_kmaps
-    if which not in cache:
-        vals = getattr(plan, which)
-        cache[which] = me._c_int_array(vals) if vals is not None else None
-    return cache[which]
-
-
 class _Tape:
     __slots__ = ("units", "arena", "x_last", "p_final", "stats", "geom", "ws")
 
@@ -271,57 +262,32 @@ class Runner:
         self._bwd_hint = 0
 
     # ------------------------------------------------------------------------------------------ single launches (final layer)
-    def _conv(self, x, tbl, kmap, conv, transposed_roles, n_out, out, accumulate, bias=None, plan=None):
+    def _conv(self, kind, plan, conv, x, out, bias=None):
+        """The final layer's forward ("fwd") or data gradient ("dgrad") into `out`."""
         kern = conv.kernel
-        K, Cin, Cout = kern.shape
-        if plan is not None and me.PROFILE is not None:
-            me.PROFILE.append(dict(kind="dgrad" if transposed_roles else "fwd", K=K, Cin=Cin, Cout=Cout, n_in=plan.n_in, n_out=plan.n_out,
-                                   plan=plan, tc=Cin % 32 == 0 and Cout % 32 == 0))
-        if transposed_roles:
-            Cin, Cout = Cout, Cin
-        st = stream()
+        Cin, Cout = kern.shape[1:]
         if Cin % 32 == 0 and Cout % 32 == 0:
-            wt = conv._prepared.tiles(kern)[1 if transposed_roles else 0]          # pre-tiled split weights for these roles
-            flags = 4 if accumulate else 0
-            if me.FWD_FP16 and not transposed_roles:          # forward roles: fp16 activation planes x fp16 weight tiles
-                flags |= me.PLANES_A_FP16 | me.PLANES_B_FP16
-            wsb = lib.pcb_conv_forward_ws_bytes(K, n_out, Cin, Cout)
-            ws = me.workspace(wsb, self.device, slot=2)
             assert x.hi, "tensor-core conv needs the split planes of its input"
-            check(lib.pcb_conv_forward_split(x.hi, x.lo, x.ld, ptr(tbl), tbl.shape[1], kmap, K, n_out, Cin, Cout, ptr(wt),
-                                             ptr(bias), out.p, out.ld, ptr(ws), wsb, flags, st))
+            tiles = conv._prepared.tiles(kern, me.FWD_FP16)[0 if kind == "fwd" else 1]
+            fp16 = me.FWD_FP16 and kind == "fwd"          # forward roles: fp16 activation planes x fp16 weight tiles
+            me.conv(kind, plan, Cin, Cout, (x.hi, x.lo), x.ld, out.p, out.ld, tiles=ptr(tiles), bias=ptr(bias), fp16=fp16)
         else:
-            # exact fp32 SIMT kernel: output widths the tensor-core tiling does not cover (13 / 20 semantic classes); as a
-            # data gradient it runs on the per-offset transposed weights
-            assert not accumulate and x.p, "the fp32 SIMT conv writes (never accumulates) and reads the fp32 plane"
-            w = kern.detach().transpose(1, 2).contiguous() if transposed_roles else kern.detach()
-            check(lib.pcb_conv_forward(x.p, x.ld, ptr(tbl), tbl.shape[1], kmap, K, n_out, Cin, Cout, None, None,
-                                       ptr(w), ptr(bias), out.p, out.ld, None, 0, 0, st))
+            # exact fp32 kernel: output widths the tensor-core tiling does not cover (13 / 20 semantic classes); as a data gradient it
+            # runs on the per-offset transposed weights
+            assert x.p, "the exact fp32 conv reads the fp32 plane"
+            w = kern.detach() if kind == "fwd" else kern.detach().transpose(1, 2).contiguous()
+            me.conv(kind, plan, Cin, Cout, x.p, x.ld, out.p, out.ld, w=ptr(w), bias=ptr(bias))
 
     def _wgrad(self, conv, plan, a_in, dz):
         kern = conv.kernel
-        K, Cin, Cout = kern.shape
+        Cin, Cout = kern.shape[1:]
         if kern.grad is None:
             kern.grad = torch.zeros_like(kern)
-        if plan.wg_gather_x:
-            A, B, Ca, Cb, tr, rows = a_in, dz, Cin, Cout, 0, plan.n_out
-        else:
-            A, B, Ca, Cb, tr, rows = dz, a_in, Cout, Cin, 1, plan.n_in
-        tc = Ca % 32 == 0 and Cb % 32 == 0
-        if me.PROFILE is not None:
-            me.PROFILE.append(dict(kind="wgrad", K=K, Cin=Cin, Cout=Cout, n_in=plan.n_in, n_out=plan.n_out, plan=plan, tc=tc))
-        if tc:
-            wsb = lib.pcb_conv_wgrad_split_ws_bytes(K, rows, Ca, Cb)
-            ws = me.workspace(wsb, self.device, slot=0)
+        if Cin % 32 == 0 and Cout % 32 == 0:
             pl = lambda b: (b.bh, b.bl) if b.bh else (b.hi, b.lo)          # activations: their bf16 planes (gradients only have those)
-            (ah, al), (bh, bl) = pl(A), pl(B)
-            check(lib.pcb_conv_wgrad_split(ah, al, A.ld, bh, bl, B.ld, ptr(plan.wg_tbl), plan.wg_tbl.shape[1], K, rows, Ca, Cb,
-                                           kern.grad.data_ptr(), tr, ptr(ws), wsb, 4, stream()))
+            me.wgrad(plan, Cin, Cout, pl(a_in), a_in.ld, pl(dz), dz.ld, kern.grad.data_ptr(), True, accumulate=True)
         else:
-            wsb = lib.pcb_conv_wgrad_ws_bytes(K, rows, Ca, Cb)
-            ws = me.workspace(wsb, self.device, slot=0)
-            check(lib.pcb_conv_wgrad(A.p, A.ld, B.p, B.ld, ptr(plan.wg_tbl), plan.wg_tbl.shape[1], K, rows, Ca, Cb, kern.grad.data_ptr(),
-                                     tr, ptr(ws), wsb, 4, stream()))
+            me.wgrad(plan, Cin, Cout, a_in.p, a_in.ld, dz.p, dz.ld, kern.grad.data_ptr(), False, accumulate=True)
 
     # ------------------------------------------------------------------------------------------ forward
     def _unit(self, conv, bnm, a_in, plan, relu, residual=None, out=None, need_f32=False):
@@ -341,11 +307,11 @@ class Runner:
         u.n_in, u.n_out, u.n0 = plan.n_in, n, n0
         u.K, u.Cin, u.Cout, u.relu = K, Cin, Cout, 1 if relu else 0
         u.fwd_tbl, u.fwd_stride = plan.fwd_tbl.data_ptr(), plan.fwd_tbl.shape[1]
-        km = _kmap(plan, "fwd_kmap")
+        km = plan.c_kmap("fwd_kmap")
         u.fwd_kmap = ctypes.cast(km, ctypes.c_void_p) if km is not None else None
         u.W = kern.data_ptr()
         if tc:
-            tiles = conv._prepared.tiles(kern)
+            tiles = conv._prepared.tiles(kern, me.FWD_FP16)
             u.wt_fwd, u.wt_dg = tiles[0].data_ptr(), tiles[1].data_ptr()
             u.x_hi, u.x_lo, u.x_lds = a_in.hi, a_in.lo, a_in.ld
             if a_in.bh:
@@ -370,8 +336,7 @@ class Runner:
             u.res_p, u.res_ld = residual.p, residual.ld
         u.ws, u.ws_bytes = self.ws.data_ptr(), self.ws.numel()
         u.flags = (1 if SEPARATE_STATS else 0) | (2 if me.FWD_FP16 else 0) | (4 if self.eval_mode else 0)
-        if me.PROFILE is not None:
-            me.PROFILE.append(dict(kind="fwd", K=K, Cin=Cin, Cout=Cout, n_in=plan.n_in, n_out=plan.n_out, plan=plan, tc=tc))
+        me.record_profile("fwd", plan, K, Cin, Cout, tc)
         check(lib.pcb_unit_forward(ctypes.byref(u), self.st))
         if CAPTURE_RELU is not None and relu:
             CAPTURE_RELU.append((n0, _plane_i16(out.hi, n, Cout, out.ld, self.device) > 0))
@@ -385,7 +350,7 @@ class Runner:
         step) and hand the results to the per-layer caches (`me._PreparedWeights`), instead of one small launch per layer."""
         m = self.model
         convs = [c for c in m.modules() if isinstance(c, me._ConvolutionBase) and c.in_channels % 32 == 0 and c.out_channels % 32 == 0]
-        tags = [(c.kernel.data_ptr(), c.kernel._version, tuple(c.kernel.shape), me._WEIGHTS_EPOCH[0], me.FWD_FP16) for c in convs]
+        tags = [me._PreparedWeights.tag(c.kernel, me.FWD_FP16) for c in convs]
         if all(c._prepared.tile_tag == t for c, t in zip(convs, tags)):
             return
         cache = self.__dict__.get("_tile_batch")
@@ -516,8 +481,7 @@ class Runner:
             x = self._stage(m.block8, cat8, p3[0], p1[0], need_f32=not fin_tc)
             out_t = torch.empty(n[0], fin.out_channels, dtype=torch.float32, device=dev)
             out = Buf(out_t, out_t.data_ptr(), n[0], fin.out_channels, fin.out_channels, dev)
-            self._conv(x, p1[0].fwd_tbl, None, fin, False, n[0], out, False,
-                       bias=fin.bias.detach().reshape(-1) if fin.bias is not None else None, plan=p1[0])
+            self._conv("fwd", p1[0], fin, x, out, bias=fin.bias.detach().reshape(-1) if fin.bias is not None else None)
             if self.bns:
                 torch._foreach_add_([bn.num_batches_tracked for bn in self.bns], g.calls)       # one multi-tensor launch, not 62
         self._fwd_hint = _grow_hint(self._fwd_hint, arena.total)
@@ -551,7 +515,7 @@ class Runner:
                 fin.bias.grad += d_out.sum(0, keepdim=True)
             self._wgrad(fin, p_final, x_last, dfin)
             gx = x_last.grad(arena)
-            self._conv(dfin, p_final.dg_tbl, _kmap(p_final, "dg_kmap"), fin, True, p_final.n_in, gx, False, plan=p_final)
+            self._conv("dgrad", p_final, fin, dfin, gx)
             x_last.slot[0] = True
             after_unit = m.__dict__.get("_fused_after_unit")       # trainer hook: gradient all-reduce of the chunk this unit completes
             for (u, conv, bn, a_in, out, plan, residual) in reversed(tape.units):
@@ -580,12 +544,11 @@ class Runner:
                     u.gin_p, u.gin_ld, u.gin_mode = ga.p, ga.ld, 2 if a_in.slot[0] else 1
                     a_in.slot[0] = True
                     u.dg_tbl, u.dg_stride = plan.dg_tbl.data_ptr(), plan.dg_tbl.shape[1]
-                    km = _kmap(plan, "dg_kmap")
+                    km = plan.c_kmap("dg_kmap")
                     u.dg_kmap = ctypes.cast(km, ctypes.c_void_p) if km is not None else None
-                if me.PROFILE is not None:
-                    me.PROFILE.append(dict(kind="wgrad", K=u.K, Cin=u.Cin, Cout=u.Cout, n_in=plan.n_in, n_out=plan.n_out, plan=plan, tc=tc))
-                    if u.gin_mode:
-                        me.PROFILE.append(dict(kind="dgrad", K=u.K, Cin=u.Cin, Cout=u.Cout, n_in=plan.n_in, n_out=plan.n_out, plan=plan, tc=tc))
+                me.record_profile("wgrad", plan, u.K, u.Cin, u.Cout, tc)
+                if u.gin_mode:
+                    me.record_profile("dgrad", plan, u.K, u.Cin, u.Cout, tc)
                 check(lib.pcb_unit_backward(ctypes.byref(u), st))
                 if after_unit is not None:
                     after_unit(conv)

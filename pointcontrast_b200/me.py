@@ -151,6 +151,13 @@ class ConvPlan:
             self._counts = cnt.cpu().tolist()
         return self._counts
 
+    def c_kmap(self, which):
+        """HOST int32 array of the kernel-offset permutation `which` ("fwd_kmap" / "dg_kmap"), cached on the plan, or None."""
+        if which not in self._c_kmaps:
+            vals = getattr(self, which)
+            self._c_kmaps[which] = _c_int_array(vals) if vals is not None else None
+        return self._c_kmaps[which]
+
 
 def _c_int_array(vals):
     return (ctypes.c_int32 * len(vals))(*[int(v) for v in vals])
@@ -386,23 +393,71 @@ import os as _os
 
 FORCE_SIMT = False      # tests flip this to run the exact fp32 kernels
 SIMT_OPS = set()        # diagnostics: subset of {"fwd", "dgrad", "wgrad"} forced onto the exact fp32 kernels (modular path)
-CONV_IMPL = "wgmma"     # the only tensor-core implementation; kept as a name for callers
 # bench.py sets this to a list: every convolution / weight-gradient entry-point call then appends its description here, in
 # issue order -- the same order in which the library (pcb_profile_enable) brackets those calls with CUDA events.
 PROFILE = None
 # Fused executor: activations travel as fp16 hi/lo planes and the forward weight tiles are fp16 (22 mantissa bits per operand instead of
 # bf16 hi/lo's 16): the forward pass is what sets the whole-network gradient error.  0: bf16 everywhere.
 FWD_FP16 = _os.environ.get("PCB_FWD_FP16", "1") == "1"
-PLANES_A_FP16, PLANES_B_FP16 = 8, 16
+CONV_FORCE_SIMT, CONV_ACCUMULATE, PLANES_A_FP16, PLANES_B_FP16 = 1, 4, 8, 16
 
 
-def _prof_begin():
-    return PROFILE is not None
-
-
-def _prof_end(on, kind, plan, K, Cin, Cout, tc):
-    if on:
+def record_profile(kind, plan, K, Cin, Cout, tc):
+    """The PROFILE record of one library call ("fwd" / "dgrad" / "wgrad" of the convolution [K][Cin][Cout] on `plan`)."""
+    if PROFILE is not None:
         PROFILE.append(dict(kind=kind, K=K, Cin=Cin, Cout=Cout, n_in=plan.n_in, n_out=plan.n_out, plan=plan, tc=tc))
+
+
+def _device():
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def conv(kind, plan, Cin, Cout, x, ldx, y, ldy, tiles=None, w=None, bias=None, accumulate=False, fp16=False):
+    """y (+)= one convolution of `plan` with the kernel [K][Cin][Cout]: kind "fwd" maps x [n_in, Cin] to y [n_out, Cout], kind "dgrad"
+    (the data gradient: opposite roles) maps x [n_out, Cout] to y [n_in, Cin].  Arguments are device pointers, row strides in elements.
+      tiles: this call's pre-tiled weights (`_PreparedWeights.tiles`) -> the split-operand tensor-core kernel; x = (hi, lo) plane
+             pointers, bf16 unless `fp16` (fp16 planes and forward tiles);
+      else : the exact fp32 kernel on x = fp32 rows and w = the fp32 weights in this call's [K][Cin][Cout] roles; it cannot accumulate."""
+    K = plan.K
+    record_profile(kind, plan, K, Cin, Cout, tiles is not None)
+    if kind == "fwd":
+        tbl, kmap, n_out = plan.fwd_tbl, plan.c_kmap("fwd_kmap"), plan.n_out
+    else:
+        tbl, kmap, n_out, Cin, Cout = plan.dg_tbl, plan.c_kmap("dg_kmap"), plan.n_in, Cout, Cin
+    if tiles is not None:
+        flags = (CONV_ACCUMULATE if accumulate else 0) | ((PLANES_A_FP16 | PLANES_B_FP16) if fp16 else 0)
+        wsb = lib.pcb_conv_forward_split_ws_bytes(K, n_out, Cin, Cout)
+        ws = workspace(wsb, _device(), slot=2)
+        check(lib.pcb_conv_forward_split(x[0], x[1], ldx, ptr(tbl), tbl.shape[1], kmap, K, n_out, Cin, Cout, tiles, bias, y, ldy,
+                                         ptr(ws), wsb, flags, stream()))
+    else:
+        if accumulate:
+            raise _lib.PcbError("the exact fp32 convolution writes its output, it does not accumulate")
+        check(lib.pcb_conv_forward(x, ldx, ptr(tbl), tbl.shape[1], kmap, K, n_out, Cin, Cout, w, bias, y, ldy, stream()))
+
+
+def wgrad(plan, Cin, Cout, x, ldx, dy, lddy, dw, split, accumulate=False, force_simt=False):
+    """dw (+)= the weight gradient [K][Cin][Cout] of `plan` from its input x [n_in, Cin] and output gradient dy [n_out, Cout] (device
+    pointers, row strides in elements).  split: x, dy = (hi, lo) bf16 plane pointers -> the tensor-core kernel; else fp32 rows -> the
+    exact kernel (force_simt: its generic kernel also for the stem layer)."""
+    K = plan.K
+    record_profile("wgrad", plan, K, Cin, Cout, split)
+    if plan.wg_gather_x:
+        A, lda, B, ldb, Ca, Cb, tr, rows = x, ldx, dy, lddy, Cin, Cout, 0, plan.n_out
+    else:
+        A, lda, B, ldb, Ca, Cb, tr, rows = dy, lddy, x, ldx, Cout, Cin, 1, plan.n_in
+    flags = CONV_ACCUMULATE if accumulate else 0
+    tbl = plan.wg_tbl
+    if split:
+        wsb = lib.pcb_conv_wgrad_split_ws_bytes(K, rows, Ca, Cb)
+        ws = workspace(wsb, _device())
+        check(lib.pcb_conv_wgrad_split(A[0], A[1], lda, B[0], B[1], ldb, ptr(tbl), tbl.shape[1], K, rows, Ca, Cb, dw, tr, ptr(ws), wsb,
+                                       flags, stream()))
+    else:
+        wsb = lib.pcb_conv_wgrad_ws_bytes(K, rows, Ca, Cb)
+        ws = workspace(wsb, _device())
+        check(lib.pcb_conv_wgrad(A, lda, B, ldb, ptr(tbl), tbl.shape[1], K, rows, Ca, Cb, dw, tr, ptr(ws), wsb,
+                                 flags | (CONV_FORCE_SIMT if force_simt else 0), stream()))
 
 
 _WEIGHTS_EPOCH = [0]
@@ -415,34 +470,27 @@ def bump_weights_epoch():
 
 
 class _PreparedWeights:
-    """bf16 hi/lo split planes of a kernel (+ per-offset transposes), refreshed when the parameter changes."""
+    """A kernel's weights pre-tiled for the split-operand conv kernel, refreshed when the parameter or the wanted format changes."""
 
     def __init__(self):
-        self.tag = None
-        self.planes = None
         self.tile_tag = None
         self._tiles = None
 
-    def tiles(self, kernel):
-        """(forward, data-gradient) weights pre-tiled as shared-memory images for the split wgmma kernel (TMA bulk loads)."""
-        tag = (kernel.data_ptr(), kernel._version, tuple(kernel.shape), _WEIGHTS_EPOCH[0], FWD_FP16)
+    @staticmethod
+    def tag(kernel, fp16):
+        return (kernel.data_ptr(), kernel._version, tuple(kernel.shape), _WEIGHTS_EPOCH[0], fp16)
+
+    def tiles(self, kernel, fp16):
+        """(forward, data-gradient) weights pre-tiled as shared-memory images for the split wgmma kernel (TMA bulk loads); the
+        forward tiles are fp16 x 2^10 if `fp16`, else bf16 like the data-gradient ones."""
+        tag = self.tag(kernel, fp16)
         if tag != self.tile_tag:
             K, Cin, Cout = kernel.shape
             f = torch.empty(lib.pcb_weight_tile_bytes(K, Cin, Cout, 0), dtype=torch.uint8, device=kernel.device)
             d = torch.empty(lib.pcb_weight_tile_bytes(K, Cin, Cout, 1), dtype=torch.uint8, device=kernel.device)
-            check(lib.pcb_weight_tile(ptr(kernel.detach()), K, Cin, Cout, ptr(f), ptr(d), PLANES_B_FP16 if FWD_FP16 else 0, stream()))
+            check(lib.pcb_weight_tile(ptr(kernel.detach()), K, Cin, Cout, ptr(f), ptr(d), PLANES_B_FP16 if fp16 else 0, stream()))
             self._tiles, self.tile_tag = (f, d), tag
         return self._tiles
-
-    def get(self, kernel):
-        tag = (kernel.data_ptr(), kernel._version, tuple(kernel.shape), _WEIGHTS_EPOCH[0])
-        if tag != self.tag:
-            K, Cin, Cout = kernel.shape
-            planes = torch.empty(4, K * Cin * Cout, dtype=torch.int16, device=kernel.device)
-            check(lib.pcb_weight_prep(ptr(kernel.detach()), K, Cin, Cout, ptr(planes[0]), ptr(planes[1]), ptr(planes[2]),
-                                      ptr(planes[3]), stream()))
-            self.planes, self.tag = planes, tag
-        return self.planes
 
 
 def _simt(op):
@@ -453,36 +501,35 @@ def _use_tc(Cin, Cout, op="fwd"):
     return (not _simt(op)) and Cin % 32 == 0 and Cout % 32 == 0
 
 
-def _conv_forward_raw(x, tbl, kmap, K, n_out, Cin, Cout, w_f32, bias, kmajor_hi=None, kmajor_lo=None, op="fwd"):
-    """Y = conv(x) on a neighbour table.  kmajor_*: the bf16 hi/lo weight planes laid out [K][Cout][Cin] for THIS call's roles (tensor-
-    core path); w_f32: fp32 [K][Cin][Cout] (exact SIMT path)."""
-    y = torch.empty(n_out, Cout, dtype=torch.float32, device=x.device)
-    km = _c_int_array(kmap) if kmap is not None else None
-    flags = 1 if _simt(op) else 0
-    wsb = lib.pcb_conv_forward_ws_bytes(K, n_out, Cin, Cout)
-    ws = workspace(wsb, x.device, slot=2)
-    check(lib.pcb_conv_forward(ptr(x), x.stride(0), ptr(tbl), tbl.shape[1], km, K, n_out, Cin, Cout, ptr(kmajor_hi), ptr(kmajor_lo),
-                               ptr(w_f32), ptr(bias), ptr(y), Cout, ptr(ws), wsb, flags, stream()))
-    return y
+def _split_rows(t):
+    """bf16 hi/lo planes of a contiguous fp32 matrix (the operand format of the tensor-core kernels): (storage, (hi, lo) pointers)."""
+    n = t.shape[0] * t.shape[1]
+    pl = torch.empty(2 * n, dtype=torch.bfloat16, device=t.device)
+    hi = pl.data_ptr()
+    check(lib.pcb_split_rows(ptr(t), t.shape[1], t.shape[0], t.shape[1], hi, hi + 2 * n, t.shape[1], 0, stream()))
+    return pl, (hi, hi + 2 * n)
 
 
 class _SparseConvFunction(torch.autograd.Function):
+    """The modular surface's convolution: tensor-core shapes run the split-operand kernel on bf16 hi/lo planes and bf16 weight
+    tiles; the 3-channel stem, widths that are not multiples of 32 and FORCE_SIMT / SIMT_OPS run the exact fp32 kernels."""
+
     @staticmethod
     def forward(ctx, x, kernel, bias, plan, prepared):
         _lib.require_cuda(x)
         x = x.contiguous()
         if x.dtype != torch.float32:
             raise _lib.PcbError("features must be float32")
-        K, Cin, Cout = kernel.shape
+        Cin, Cout = kernel.shape[1:]
         with torch.cuda.device(x.device):
-            khi = klo = None
+            y = torch.empty(plan.n_out, Cout, dtype=torch.float32, device=x.device)
+            b = bias.detach().reshape(-1) if bias is not None else None
             if _use_tc(Cin, Cout):
-                pl = prepared.get(kernel)
-                khi, klo = pl[2], pl[3]                    # [K][Cout][Cin]: K-major for the forward roles
-            ev = _prof_begin()
-            y = _conv_forward_raw(x, plan.fwd_tbl, plan.fwd_kmap, K, plan.n_out, Cin, Cout,
-                                  kernel.detach().contiguous(), bias.detach().reshape(-1) if bias is not None else None, khi, klo)
-            _prof_end(ev, "fwd", plan, K, Cin, Cout, khi is not None)
+                xs, xp = _split_rows(x)
+                conv("fwd", plan, Cin, Cout, xp, Cin, ptr(y), Cout, tiles=ptr(prepared.tiles(kernel, False)[0]), bias=ptr(b))
+            else:
+                w = kernel.detach().contiguous()
+                conv("fwd", plan, Cin, Cout, ptr(x), Cin, ptr(y), Cout, w=ptr(w), bias=ptr(b))
         ctx.save_for_backward(x, kernel)
         ctx.plan, ctx.prepared, ctx.has_bias = plan, prepared, bias is not None
         return y
@@ -491,44 +538,27 @@ class _SparseConvFunction(torch.autograd.Function):
     def backward(ctx, dy):
         x, kernel = ctx.saved_tensors
         plan = ctx.plan
-        K, Cin, Cout = kernel.shape
+        Cin, Cout = kernel.shape[1:]
         dy = dy.contiguous()
         dx = dw = db = None
         with torch.cuda.device(dy.device):
+            dgrad_tc = ctx.needs_input_grad[0] and _use_tc(Cin, Cout, "dgrad")
+            wgrad_tc = ctx.needs_input_grad[1] and _use_tc(Cin, Cout, "wgrad")
+            dys, dyp = _split_rows(dy) if dgrad_tc or wgrad_tc else (None, None)      # one split of dy serves both tensor-core calls
             if ctx.needs_input_grad[0]:
-                khi = klo = wt = None
-                if _use_tc(Cout, Cin, "dgrad"):
-                    pl = ctx.prepared.get(kernel)
-                    khi, klo = pl[0], pl[1]                # [K][Cin][Cout]: K-major for the data-gradient roles (N = Cin, contraction = Cout)
+                dx = torch.empty(plan.n_in, Cin, dtype=torch.float32, device=dy.device)
+                if dgrad_tc:
+                    conv("dgrad", plan, Cin, Cout, dyp, Cout, ptr(dx), Cin, tiles=ptr(ctx.prepared.tiles(kernel, False)[1]))
                 else:
-                    wt = kernel.detach().transpose(1, 2).contiguous()
-                ev = _prof_begin()
-                dx = _conv_forward_raw(dy, plan.dg_tbl, plan.dg_kmap, K, plan.n_in, Cout, Cin, wt, None, khi, klo, op="dgrad")
-                _prof_end(ev, "dgrad", plan, K, Cin, Cout, khi is not None)
+                    wt = kernel.detach().transpose(1, 2).contiguous()      # the data-gradient roles' [K][Cout][Cin]
+                    conv("dgrad", plan, Cin, Cout, ptr(dy), Cout, ptr(dx), Cin, w=ptr(wt))
             if ctx.needs_input_grad[1]:
                 dw = torch.empty_like(kernel)
-                if plan.wg_gather_x:
-                    A, B, Ca, Cb, tr, rows = x, dy, Cin, Cout, 0, plan.n_out
-                else:
-                    A, B, Ca, Cb, tr, rows = dy, x, Cout, Cin, 1, plan.n_in
-                tc = Ca % 32 == 0 and Cb % 32 == 0 and not _simt("wgrad")
-                ev = _prof_begin()
-                if tc:      # tensor-core weight gradient on split (bf16 hi/lo) operands
-                    def planes(t):
-                        pl = torch.empty(2, t.shape[0] * t.shape[1], dtype=torch.bfloat16, device=t.device)
-                        check(lib.pcb_split_rows(ptr(t), t.shape[1], t.shape[0], t.shape[1], pl[0].data_ptr(), pl[1].data_ptr(), t.shape[1], 0, stream()))
-                        return pl
-                    Ap, Bp = planes(A), planes(B)
-                    wsb = lib.pcb_conv_wgrad_split_ws_bytes(K, rows, Ca, Cb)
-                    ws = workspace(wsb, dy.device)
-                    check(lib.pcb_conv_wgrad_split(Ap[0].data_ptr(), Ap[1].data_ptr(), Ca, Bp[0].data_ptr(), Bp[1].data_ptr(), Cb, ptr(plan.wg_tbl),
-                                                   plan.wg_tbl.shape[1], K, rows, Ca, Cb, ptr(dw), tr, ptr(ws), wsb, 0, stream()))
+                if wgrad_tc:
+                    xs, xp = _split_rows(x)
+                    wgrad(plan, Cin, Cout, xp, Cin, dyp, Cout, ptr(dw), True)
                 else:       # exact fp32 (stem layer, odd widths, FORCE_SIMT)
-                    wsb = lib.pcb_conv_wgrad_ws_bytes(K, rows, Ca, Cb)
-                    ws = workspace(wsb, dy.device)
-                    check(lib.pcb_conv_wgrad(ptr(A), A.stride(0), ptr(B), B.stride(0), ptr(plan.wg_tbl), plan.wg_tbl.shape[1], K,
-                                             rows, Ca, Cb, ptr(dw), tr, ptr(ws), wsb, 1 if _simt("wgrad") else 0, stream()))
-                _prof_end(ev, "wgrad", plan, K, Cin, Cout, tc)
+                    wgrad(plan, Cin, Cout, ptr(x), Cin, ptr(dy), Cout, ptr(dw), False, force_simt=_simt("wgrad"))
             if ctx.has_bias and ctx.needs_input_grad[2]:
                 db = dy.sum(0, keepdim=True)
         return dx, dw, db, None, None

@@ -245,7 +245,8 @@ def test_split_operand_wgrad_tcgen05_matches_exact_fp32_kernel(Ca, Cb, tr):
 
 
 @pytest.mark.parametrize("cin,cout", [(96, 96), (128, 96), (32, 64), (256, 256), (384, 256)])
-def test_split_operand_conv_forward_matches_fp32_input_kernel(cin, cout):
+def test_split_operand_conv_forward_matches_exact_fp32_kernel(cin, cout):
+    """Tensor-core forward / data gradient on bf16 hi/lo planes and pre-tiled weights vs the exact fp32 SIMT kernel of the library."""
     from pointcontrast_b200 import me
     from pointcontrast_b200._lib import check, lib, ptr, stream
     rng = np.random.default_rng(cin + cout)
@@ -255,30 +256,43 @@ def test_split_operand_conv_forward_matches_fp32_input_kernel(cin, cout):
     plan = st.coords_man.conv_plan(st.coords_key, st.coords_key, kg, False)
     n = plan.n_out
     X = torch.randn(n, cin, device="cuda"); W = torch.randn(27, cin, cout, device="cuda") * 0.05
-    planes = torch.empty(4, 27 * cin * cout, dtype=torch.int16, device="cuda")
-    check(lib.pcb_weight_prep(ptr(W), 27, cin, cout, ptr(planes[0]), ptr(planes[1]), ptr(planes[2]), ptr(planes[3]), stream()))
-    ref = me._conv_forward_raw(X, plan.fwd_tbl, None, 27, n, cin, cout, W, None, planes[2], planes[3])
+    ref = torch.empty(n, cout, device="cuda")
+    check(lib.pcb_conv_forward(ptr(X), cin, ptr(plan.fwd_tbl), plan.fwd_tbl.shape[1], None, 27, n, cin, cout, ptr(W), None, ptr(ref), cout,
+                               stream()))
     Xs = _split(X)
     got = torch.full((n, cout), 0.25, device="cuda")
-    wsb = lib.pcb_conv_forward_ws_bytes(27, n, cin, cout); ws = torch.empty(max(wsb, 256), dtype=torch.uint8, device="cuda")
+    wsb = lib.pcb_conv_forward_split_ws_bytes(27, n, cin, cout); ws = torch.empty(max(wsb, 256), dtype=torch.uint8, device="cuda")
     ft = torch.empty(lib.pcb_weight_tile_bytes(27, cin, cout, 0), dtype=torch.uint8, device="cuda")
     dt = torch.empty(lib.pcb_weight_tile_bytes(27, cin, cout, 1), dtype=torch.uint8, device="cuda")
     check(lib.pcb_weight_tile(ptr(W), 27, cin, cout, ptr(ft), ptr(dt), 0, stream()))
     check(lib.pcb_conv_forward_split(Xs[0].data_ptr(), Xs[1].data_ptr(), cin, ptr(plan.fwd_tbl), plan.fwd_tbl.shape[1], None, 27, n, cin,
-                                     cout, ptr(ft), None, ptr(got), cout, ptr(ws), wsb, 4, stream()))
+                                     cout, ptr(ft), None, ptr(got), cout, ptr(ws), wsb, 4, stream()))      # accumulate onto 0.25
     torch.cuda.synchronize()
-    assert max_rel_err(got - 0.25, ref) < 1e-5
-    # data-gradient roles: dX = sum_k dY[tbl[opp k]] W[k]^T through the dgrad tiles vs the fp32-input kernel
+    assert max_rel_err(got - 0.25, ref) < 1e-4          # bf16 hi/lo products (2^-17) vs exact fp32
+    # and against fp64, offset by offset
+    def fp64(tbl, kmap, A, Wk):
+        out = torch.zeros(n, Wk.shape[2], dtype=torch.float64, device="cuda")
+        for k in range(27):
+            t = tbl[kmap[k] if kmap is not None else k].long()
+            ok = t >= 0
+            out[ok] += A.double()[t[ok]] @ Wk[k].double()
+        return out
+    assert max_rel_err(got - 0.25, fp64(plan.fwd_tbl, None, X, W)) < 1e-4
+    # data-gradient roles: dX = sum_k dY[tbl[opp k]] W[k]^T through the dgrad tiles vs the exact kernel on the transposed weights
     dY = torch.randn(n, cout, device="cuda")
     opp = plan.dg_kmap
-    ref_dx = me._conv_forward_raw(dY, plan.dg_tbl, opp, 27, n, cout, cin, None, None, planes[0], planes[1])
+    Wt = W.transpose(1, 2).contiguous()
+    ref_dx = torch.empty(n, cin, device="cuda")
+    check(lib.pcb_conv_forward(ptr(dY), cout, ptr(plan.dg_tbl), plan.dg_tbl.shape[1], me._c_int_array(opp), 27, n, cout, cin, ptr(Wt), None,
+                               ptr(ref_dx), cin, stream()))
     dYs = _split(dY)
     got_dx = torch.empty(n, cin, device="cuda")
-    wsb = lib.pcb_conv_forward_ws_bytes(27, n, cout, cin); ws = torch.empty(max(wsb, 256), dtype=torch.uint8, device="cuda")
+    wsb = lib.pcb_conv_forward_split_ws_bytes(27, n, cout, cin); ws = torch.empty(max(wsb, 256), dtype=torch.uint8, device="cuda")
     check(lib.pcb_conv_forward_split(dYs[0].data_ptr(), dYs[1].data_ptr(), cout, ptr(plan.dg_tbl), plan.dg_tbl.shape[1],
                                      me._c_int_array(opp), 27, n, cout, cin, ptr(dt), None, ptr(got_dx), cin, ptr(ws), wsb, 0, stream()))
     torch.cuda.synchronize()
-    assert max_rel_err(got_dx, ref_dx) < 1e-5
+    assert max_rel_err(got_dx, ref_dx) < 1e-4
+    assert max_rel_err(got_dx, fp64(plan.dg_tbl, opp, dY, Wt)) < 1e-4
 
 
 @pytest.mark.parametrize("n0,n1,C", [(5000, 3777, 32), (130, 1, 96), (128, 128, 64), (1, 300, 256)])
