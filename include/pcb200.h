@@ -102,6 +102,43 @@ size_t pcb_radius_pairs_ws_bytes(int64_t ns, int64_t nd);
 int pcb_radius_pairs(const float* src, int64_t ns, const float* dst, int64_t nd, float radius, int32_t* pairs, int64_t cap,
                      int64_t* n_pairs, void* ws, size_t ws_bytes, void* stream);
 
+/* ----------------------------------------------------------------------------------------------- semseg training data (8f-6) */
+/* Label-aware voxelisation of integer coordinates (int32 [N,3], |c| < 2^20): the M occupied voxels in ascending (x,y,z) order
+ * (out_coords int32 [M,3]), sel[M] = the smallest index of a point in the voxel, out_labels[M] = the label all of the voxel's points
+ * share, else ignore_label -- `ME.utils.sparse_quantize(coords, feats, labels=, ignore_label=)` (ME 0.4.3 `quantize_label`) of
+ * `downstream/semseg/lib/voxelizer.py:145-146`.  Outputs hold up to n rows.  SYNCHRONISES once to return *m_out. */
+size_t pcb_voxelize_labels_ws_bytes(int64_t n);
+int pcb_voxelize_labels(const int32_t* coords, const int32_t* labels, int64_t n, int32_t ignore_label, int32_t* out_coords, int32_t* sel,
+                        int32_t* out_labels, int64_t* m_out, void* ws, size_t ws_bytes, void* stream);
+/* Per-axis minimum (lo[3]) and maximum (hi[3]) of fp32 points [N,3], N >= 1; lo / hi are host pointers.  SYNCHRONISES. */
+size_t pcb_point_bounds_ws_bytes(void);
+int pcb_point_bounds(const float* xyz, int64_t n, float* lo, float* hi, void* ws, size_t ws_bytes, void* stream);
+/* Elastic distortion (`downstream/semseg/lib/transforms.py:187-217`).  noise: the drawn fp32 grid [gx,gy,gz,3] (device, in place: on
+ * return it holds the grid after two rounds of the x, y, z 3-tap box filters, scipy.ndimage.convolve's float64 accumulation, zero
+ * outside).  axes: device fp64 [gx + gy + gz], the grid positions per axis (strictly ascending).  Then per point, in place:
+ * xyz += RegularGridInterpolator(axes, grid, fill_value=0)(xyz) * magnitude, in fp64, rounded to fp32.  Bit-exact vs scipy. */
+size_t pcb_elastic_distort_ws_bytes(int gx, int gy, int gz);
+int pcb_elastic_distort(float* xyz, int64_t n, float* noise, int gx, int gy, int gz, const double* axes, double magnitude, void* ws,
+                        size_t ws_bytes, void* stream);
+/* out[i] = floor(homo(xyz_i) @ T[:3,:].T) - min_i(...) per axis (int32 [N,3]), min_out[3] (host) = that minimum
+ * (`downstream/semseg/lib/voxelizer.py:134-142`).  T: host fp64 row-major 4x4 (rows 0-2 read); each value is
+ * ((x T[j,0] + y T[j,1]) + z T[j,2]) + T[j,3] in fp64.  PCB_ERR_RANGE if a floor lies outside +-2^20.  SYNCHRONISES. */
+size_t pcb_affine_floor_ws_bytes(void);
+int pcb_affine_floor(const float* xyz, int64_t n, const double* T, int32_t* out, int32_t* min_out, void* ws, size_t ws_bytes, void* stream);
+/* The semseg input transforms after dropout, in place on voxels coords int32 [N,3] / colours fp32 [N,3], in the loader's order
+ * (`downstream/semseg/lib/dataset.py:344-350`, `lib/transforms.py:23-179`), with the per-scene draws as arguments (coords may be
+ * NULL when flip_mask == 0):
+ *   RandomHorizontalFlip    bit k of flip_mask: coords[:,k] = max(coords[:,k]) - coords[:,k]
+ *   ChromaticAutoContrast   contrast != 0: fp32 (lo, hi, scale = 255 / (hi - lo)), blended with the fp64 factor `blend`;
+ *                           PCB_ERR_RANGE if the largest colour is <= 1 (the reference's assert) -- SYNCHRONISES in that case
+ *   ChromaticTranslation    translation (host fp64 [3]) or NULL: clip(translation + colour, 0, 255) in fp64, stored fp32
+ *   ChromaticJitter         jitter_noise (device fp64 [N,3], standard normal) or NULL: clip(noise * jitter_scale + colour, 0, 255)
+ *   normalize != 0          colour / 255 - 0.5 in fp32 (`downstream/semseg/lib/train.py:114`) */
+size_t pcb_semseg_input_transform_ws_bytes(void);
+int pcb_semseg_input_transform(int32_t* coords, float* feats, int64_t n, int flip_mask, int contrast, double blend,
+                               const double* translation, const double* jitter_noise, double jitter_scale, int normalize, void* ws,
+                               size_t ws_bytes, void* stream);
+
 /* ----------------------------------------------------------------------------------------------- convolution */
 /* Y[j, :] = bias + sum_k X[tbl[kmap[k]][j], :] . W[k]      (j < n_out)      -- EXACT fp32, any channel counts
  *   X  : [*, Cin] row stride ldx (floats);  Y: [n_out, Cout] row stride ldy;  W: fp32 [K][Cin][Cout];  bias: [Cout] or NULL.

@@ -23,7 +23,7 @@ def _load():
 
 lib = _load()
 
-_p, _i, _l, _f, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
+_p, _i, _l, _f, _d, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double, C.c_size_t
 _SIGS = {
     "pcb_last_error": (C.c_char_p, []),
     "pcb_version": (C.c_char_p, []),
@@ -38,6 +38,16 @@ _SIGS = {
     "pcb_voxelize": (_i, [_p, _l, _f, _p, _p, C.POINTER(C.c_int64), _p, _sz, _p]),
     "pcb_radius_pairs_ws_bytes": (_sz, [_l, _l]),
     "pcb_radius_pairs": (_i, [_p, _l, _p, _l, _f, _p, _l, C.POINTER(C.c_int64), _p, _sz, _p]),
+    "pcb_voxelize_labels_ws_bytes": (_sz, [_l]),
+    "pcb_voxelize_labels": (_i, [_p, _p, _l, C.c_int32, _p, _p, _p, C.POINTER(C.c_int64), _p, _sz, _p]),
+    "pcb_point_bounds_ws_bytes": (_sz, []),
+    "pcb_point_bounds": (_i, [_p, _l, _p, _p, _p, _sz, _p]),
+    "pcb_elastic_distort_ws_bytes": (_sz, [_i, _i, _i]),
+    "pcb_elastic_distort": (_i, [_p, _l, _p, _i, _i, _i, _p, _d, _p, _sz, _p]),
+    "pcb_affine_floor_ws_bytes": (_sz, []),
+    "pcb_affine_floor": (_i, [_p, _l, _p, _p, _p, _p, _sz, _p]),
+    "pcb_semseg_input_transform_ws_bytes": (_sz, []),
+    "pcb_semseg_input_transform": (_i, [_p, _p, _l, _i, _i, _d, _p, _p, _d, _i, _p, _sz, _p]),
     "pcb_kernel_map": (_i, [_p, _l, _p, _p, _l, _p, _i, _p, _p]),
     "pcb_kernel_map_count": (_i, [_p, _i, _l, _p, _p]),
     "pcb_conv_forward": (_i, [_p, _i, _p, _l, _p, _i, _l, _i, _i, _p, _p, _p, _i, _p]),

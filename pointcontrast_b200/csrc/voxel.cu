@@ -2,6 +2,8 @@
 // (`pretrain/pointcontrast/lib/ddp_data_loaders.py:196-265`), which today runs on CPU workers:
 //   * `ME.utils.sparse_quantize(xyz / voxel_size, return_index=True)` (`:228-241`; semseg: `lib/voxelizer.py:113-148`):
 //     one point per occupied voxel                                                          -> pcb_voxelize
+//   * its label variant on integer coordinates (semseg `lib/voxelizer.py:145-146`): a voxel keeps the label its points share,
+//     else ignore_label                                                                     -> pcb_voxelize_labels
 //   * `get_matching_indices` (`:36-49`): an open3d KD-tree radius search PER POINT, radius 1.5 voxels   -> pcb_radius_pairs
 // Both are integer / hashing work on the same primitives as the coordinate manager (radix sort + head flags + scan, the
 // open-addressing hash table of common.cuh); results are exact (tests/test_gpu_voxel.py: vs numpy / scipy cKDTree).
@@ -150,11 +152,8 @@ SortWs carve(void* ws, int64_t n) {
 }
 size_t carve_bytes(int64_t n) { return 2 * align_up(n * 8) + 4 * align_up(n * 4) + 512 + align_up(sort_scan_bytes(n)) + 256; }
 
-// keys of the points' cells -> stable sort -> head flags -> inclusive scan (rank)
-int sort_cells(const float* xyz, int64_t n, float size, SortWs& w, cudaStream_t st) {
-  PCB_CUDA(cudaMemsetAsync(w.status, 0, sizeof(int32_t), st));
-  point_key_kernel<<<blocks_for(n, 256), 256, 0, st>>>(xyz, n, size, w.k, w.idx, w.status);
-  if (int e = check_launch("point_key_kernel")) return e;
+// keys w.k / indices w.idx -> stable sort -> head flags -> inclusive scan (rank)
+int sort_runs(int64_t n, SortWs& w, cudaStream_t st) {
   size_t cb = w.cub_bytes;
   PCB_CUDA(cub::DeviceRadixSort::SortPairs(w.cub, cb, w.k, w.sk, w.idx, w.sidx, (int)n, 0, 63, st));
   head_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, n, w.flag);
@@ -163,6 +162,44 @@ int sort_cells(const float* xyz, int64_t n, float size, SortWs& w, cudaStream_t 
   PCB_CUDA(cub::DeviceScan::InclusiveSum(w.cub, cb, w.flag, w.rank, (int)n, st));
   g_launches.fetch_add(10);
   return PCB_OK;
+}
+
+// keys of the points' cells -> sort_runs
+int sort_cells(const float* xyz, int64_t n, float size, SortWs& w, cudaStream_t st) {
+  PCB_CUDA(cudaMemsetAsync(w.status, 0, sizeof(int32_t), st));
+  point_key_kernel<<<blocks_for(n, 256), 256, 0, st>>>(xyz, n, size, w.k, w.idx, w.status);
+  if (int e = check_launch("point_key_kernel")) return e;
+  return sort_runs(n, w, st);
+}
+
+__global__ void int_key_kernel(const int32_t* __restrict__ c, int64_t n, uint64_t* __restrict__ keys, int32_t* __restrict__ idx, int32_t* status) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int x = c[3 * i], y = c[3 * i + 1], z = c[3 * i + 2];
+  if (x <= -VB || x >= VB || y <= -VB || y >= VB || z <= -VB || z >= VB) { atomicOr(status, PCB_ERR_RANGE); x = y = z = 0; }
+  keys[i] = cell_key(x, y, z);
+  idx[i] = (int32_t)i;
+}
+
+// label-aware voxelisation output: one thread per run head writes the voxel and scans its run (the stable sort keeps the points of a
+// voxel in ascending index order) for the smallest and largest label; the voxel keeps its label only if the two agree
+__global__ void voxel_label_write_kernel(const uint64_t* __restrict__ sk, const int32_t* __restrict__ sidx, const int32_t* __restrict__ rank,
+                                         const int32_t* __restrict__ labels, int64_t n, int32_t ignore_label, int32_t* __restrict__ coords,
+                                         int32_t* __restrict__ sel, int32_t* __restrict__ out_labels, int64_t* m_out) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (i == n - 1) *m_out = rank[i];
+  const uint64_t k = sk[i];
+  if (i > 0 && sk[i - 1] == k) return;
+  const int r = rank[i] - 1;
+  coords[3 * r] = (int)(k >> 42) - VB; coords[3 * r + 1] = (int)((k >> 21) & 0x1FFFFF) - VB; coords[3 * r + 2] = (int)(k & 0x1FFFFF) - VB;
+  sel[r] = sidx[i];
+  int32_t lo = labels[sidx[i]], hi = lo;
+  for (int64_t j = i + 1; j < n && sk[j] == k; ++j) {
+    const int32_t l = labels[sidx[j]];
+    lo = min(lo, l); hi = max(hi, l);
+  }
+  out_labels[r] = lo == hi ? lo : ignore_label;
 }
 
 }  // namespace
@@ -185,6 +222,31 @@ extern "C" int pcb_voxelize(const float* xyz, int64_t n, float voxel_size, int32
   PCB_CUDA(cudaMemcpyAsync(&status, w.status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   PCB_CUDA(cudaStreamSynchronize(st));
   if (status) { set_error("pcb_voxelize: a point lies outside +-2^20 voxels"); return PCB_ERR_RANGE; }
+  return PCB_OK;
+}
+
+extern "C" size_t pcb_voxelize_labels_ws_bytes(int64_t n) { return carve_bytes(n < 1 ? 1 : n); }
+
+extern "C" int pcb_voxelize_labels(const int32_t* coords, const int32_t* labels, int64_t n, int32_t ignore_label, int32_t* out_coords,
+                                   int32_t* sel, int32_t* out_labels, int64_t* m_out, void* ws, size_t ws_bytes, void* stream) {
+  PCB_ARG(n >= 0 && n < (1ll << 31) && m_out);
+  *m_out = 0;
+  if (n == 0) return PCB_OK;
+  PCB_ARG(coords && labels && out_coords && sel && out_labels && ws && ws_bytes >= pcb_voxelize_labels_ws_bytes(n));
+  cudaStream_t st = (cudaStream_t)stream;
+  SortWs w = carve(ws, n);
+  PCB_CUDA(cudaMemsetAsync(w.status, 0, sizeof(int32_t), st));
+  int_key_kernel<<<blocks_for(n, 256), 256, 0, st>>>(coords, n, w.k, w.idx, w.status);
+  if (int e = check_launch("int_key_kernel")) return e;
+  if (int e = sort_runs(n, w, st)) return e;
+  voxel_label_write_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, w.sidx, w.rank, labels, n, ignore_label, out_coords, sel, out_labels,
+                                                               w.count);
+  if (int e = check_launch("voxel_label_write_kernel")) return e;
+  int32_t status = 0;
+  PCB_CUDA(cudaMemcpyAsync(m_out, w.count, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  PCB_CUDA(cudaMemcpyAsync(&status, w.status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  PCB_CUDA(cudaStreamSynchronize(st));
+  if (status) { set_error("pcb_voxelize_labels: a coordinate lies outside +-2^20"); return PCB_ERR_RANGE; }
   return PCB_OK;
 }
 

@@ -41,6 +41,42 @@ def synth_room(seed, scale=0.751, n_raw=300_000):
     return pts
 
 
+def synth_labelled_room(seed, n_raw, scale=1.0, labels=(1, 2, 3, 4, 5, 6, 7, 8, 9), label_noise=0.1, num_labels=41):
+    """A labelled, coloured room as the semseg `.ply` files hold it: float32 xyz [n_raw, 3], uint8 rgb [n_raw, 3], uint8 labels [n_raw].
+    Each surface of `synth_room` has one label of `labels` and a base colour; a `label_noise` share of the points gets a uniformly random
+    label in [0, num_labels), so voxels on surface boundaries and noisy points mix labels."""
+    rng = np.random.default_rng(seed)
+    rects = _rects()
+    areas = np.array([np.linalg.norm(np.cross(u, v)) for _, u, v in rects])
+    which = rng.choice(len(rects), size=n_raw, p=areas / areas.sum())
+    a, b = rng.random(n_raw)[:, None], rng.random(n_raw)[:, None]
+    o, u, v = (np.stack([r[k] for r in rects])[which] for k in range(3))
+    pts = (o + a * u + b * v) * scale + rng.normal(0.0, 0.005, size=(n_raw, 3))
+    base = rng.integers(30, 226, size=(len(rects), 3))
+    rgb = np.clip(base[which] + rng.normal(0, 12, size=(n_raw, 3)), 0, 255).astype(np.uint8)
+    lab = np.asarray(labels, np.int64)[which % len(labels)]
+    noisy = rng.random(n_raw) < label_noise
+    lab[noisy] = rng.integers(0, num_labels, noisy.sum())
+    return pts.astype(np.float32), rgb, lab.astype(np.uint8)
+
+
+def write_ply(path, xyz, rgb, labels=None):
+    """A binary little-endian PLY with the vertex layout of the semseg preprocessing (`downstream/semseg/lib/pc_utils.py:41-70`)."""
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"), ("blue", "u1")]
+    if labels is not None:
+        fields.append(("label", "u1"))
+    v = np.empty(len(xyz), dtype=fields)
+    v["x"], v["y"], v["z"] = xyz[:, 0], xyz[:, 1], xyz[:, 2]
+    v["red"], v["green"], v["blue"] = rgb[:, 0], rgb[:, 1], rgb[:, 2]
+    if labels is not None:
+        v["label"] = labels
+    types = {"<f4": "float", "u1": "uchar"}
+    head = ["ply", "format binary_little_endian 1.0", f"element vertex {len(v)}"] + [f"property {types[t]} {n}" for n, t in fields]
+    with open(path, "wb") as f:
+        f.write(("\n".join(head + ["end_header"]) + "\n").encode("ascii"))
+        f.write(v.tobytes())
+
+
 def _rot(rng):
     """Random rotation, same law as `sample_random_trans` (`ddp_data_loaders.py:137-142`)."""
     axis = rng.random(3) - 0.5
