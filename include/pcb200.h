@@ -352,6 +352,31 @@ int pcb_gather_points_grad(const float* grad_out, const int32_t* idx, int64_t B,
 int pcb_three_interpolate_grad(const float* grad_out, const int32_t* idx, const float* weight, int64_t B, int64_t C, int64_t n, int64_t m,
                                float* grad_features, void* ws, size_t ws_bytes, void* stream);
 
+/* ----------------------------------------------------------------------------------------------- sparse-conv detection backbone (8f-7) */
+/* Batched voxelisation of a collated VoteNet batch, xyz fp32 [B, N, 3] (`downstream/votenet_det_new/models/backbone/sparseconv/
+ * voxelized_dataset.py:33-65`: per scene floor(xyz / voxel_size) in fp32, `ME.utils.sparse_quantize(coords, return_index=True)`).
+ * One row per occupied (scene, voxel), scene-major, ascending first index within a scene: out_coords int32 [M, 4] = (b, x, y, z),
+ * inds int32 [M] = the scene-local index of the voxel's first (smallest-index) point, offsets int64 [B + 1] (device): scene b is rows
+ * [offsets[b], offsets[b+1]).  out_coords / inds hold up to B * N rows.  SYNCHRONISES once: offsets_host (host, B + 1 entries) receives
+ * the offsets, M = offsets_host[B].  A cell index outside +-2^20 returns PCB_ERR_RANGE.  B < 1, N < 1, voxel_size <= 0, NULL pointers
+ * and a short workspace return PCB_ERR_ARG. */
+size_t pcb_voxelize_scenes_ws_bytes(int64_t B, int64_t N);
+int pcb_voxelize_scenes(const float* xyz, int64_t B, int64_t N, float voxel_size, int32_t* out_coords, int32_t* inds, int64_t* offsets,
+                        int64_t* offsets_host, void* ws, size_t ws_bytes, void* stream);
+/* Furthest-point sampling of B scenes of different sizes in one launch: points fp32 [M, 3] grouped by scene, device offsets [B + 1]
+ * (scene b is rows [offsets[b], offsets[b+1])), max_n an upper bound on every scene's size (sizes the clusters and the workspace; a
+ * bound above M counts as M).  idx [B, npoint] of scene-local indices, for every scene identical to pcb_furthest_point_sampling on that
+ * scene alone.  A scene that is empty, larger than max_n or outside [0, M) gets -1 in every slot.  B < 1, M < B, max_n < 1 and NULL
+ * pointers return PCB_ERR_ARG.  ws: pcb_furthest_point_sampling_ragged_ws_bytes (0 unless max_n exceeds what a cluster holds on chip). */
+size_t pcb_furthest_point_sampling_ragged_ws_bytes(int64_t B, int64_t M, int64_t max_n);
+int pcb_furthest_point_sampling_ragged(const float* xyz, const int64_t* offsets, int64_t B, int64_t M, int64_t max_n, int64_t npoint,
+                                       int32_t* idx, void* ws, size_t ws_bytes, void* stream);
+/* Adjoint of the row gather out[p, :] = rows[idx[p], :], p < L, over rows fp32 [M, C] (row-major): grad_rows [M, C] written in full,
+ * each row the fp64 sum of its readers' gradients in ascending p (deterministic; an index outside [0, M) is read by nobody).
+ * ws: pcb_points_grad_ws_bytes(1, M, L). */
+int pcb_gather_rows_grad(const float* grad_out, const int32_t* idx, int64_t L, int64_t C, int64_t M, float* grad_rows, void* ws,
+                         size_t ws_bytes, void* stream);
+
 /* ----------------------------------------------------------------------------------------------- optimiser */
 /* torch.optim.SGD semantics on a flat buffer:  d = g*grad_scale + wd*p;  buf = first ? d : momentum*buf + (1-dampening)*d;  p -= lr*buf
  * (pretraining: dampening 0, `lib/ddp_trainer.py:107-111`; semseg finetuning: 0.1, `downstream/semseg/lib/solvers.py:50-57`) */

@@ -93,6 +93,11 @@ _SIGS = {
     "pcb_points_grad_ws_bytes": (_sz, [_l, _l, _l]),
     "pcb_gather_points_grad": (_i, [_p, _p, _l, _l, _l, _l, _p, _p, _sz, _p]),
     "pcb_three_interpolate_grad": (_i, [_p, _p, _p, _l, _l, _l, _l, _p, _p, _sz, _p]),
+    "pcb_voxelize_scenes_ws_bytes": (_sz, [_l, _l]),
+    "pcb_voxelize_scenes": (_i, [_p, _l, _l, _f, _p, _p, _p, _p, _p, _sz, _p]),
+    "pcb_furthest_point_sampling_ragged_ws_bytes": (_sz, [_l, _l, _l]),
+    "pcb_furthest_point_sampling_ragged": (_i, [_p, _p, _l, _l, _l, _l, _p, _p, _sz, _p]),
+    "pcb_gather_rows_grad": (_i, [_p, _p, _l, _l, _l, _p, _p, _sz, _p]),
 }
 
 

@@ -51,18 +51,33 @@ __device__ __forceinline__ unsigned long long fps_key(float d, int64_t k) {
   return ((unsigned long long)__float_as_uint(d) << 32) | (0xFFFFFFFFu - (uint32_t)k);
 }
 
-__global__ void __launch_bounds__(FPS_THREADS, 1) fps_kernel(const float* __restrict__ xyz, int64_t N, int64_t npoint, int cs, int64_t per_cta,
-                                                             float* __restrict__ temp, int32_t* __restrict__ out) {
+// Scene b is rows [offsets[b], offsets[b+1]) of xyz (ragged batches) or, with offsets == NULL, rows [b*N, (b+1)*N).  Indices are
+// scene-local.  The selection does not depend on the cluster shape (per-point running distances, index-unique keys), so a ragged
+// launch sized for its largest scene returns, for every scene, what a launch for that scene alone returns.  A ragged scene that is
+// empty, ends past `total` rows or exceeds the cluster's capacity cs * per_cta gets -1 in every slot.
+__global__ void __launch_bounds__(FPS_THREADS, 1) fps_kernel(const float* __restrict__ xyz, const int64_t* __restrict__ offsets, int64_t N,
+                                                             int64_t total, int64_t npoint, int cs, int64_t per_cta, float* __restrict__ temp,
+                                                             int32_t* __restrict__ out) {
   extern __shared__ float4 sp[];
   __shared__ FpsSlot slots[2][FPS_MAX_CLUSTER];
   __shared__ unsigned long long wbest[FPS_THREADS / 32];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t rank = cluster_rank();
   const int64_t b = blockIdx.x / cs;
-  xyz += b * N * 3;
   out += b * npoint;
+  int64_t begin = b * N;
+  if (offsets) {                                   // uniform over the cluster: either every CTA returns here or none does
+    begin = offsets[b];
+    N = offsets[b + 1] - begin;
+    if (begin < 0 || N < 1 || begin + N > total || N > cs * per_cta) {
+      if (rank == 0)
+        for (int64_t j = tid; j < npoint; j += FPS_THREADS) out[j] = -1;
+      return;
+    }
+  }
+  xyz += begin * 3;
   const int64_t lo = rank * per_cta, n_loc = max((int64_t)0, min(N, lo + per_cta) - lo), n_sm = min(n_loc, (int64_t)FPS_SMEM_PTS);
-  float* tg = temp ? temp + b * N + lo : nullptr;
+  float* tg = temp ? temp + begin + lo : nullptr;
   for (int64_t i = tid; i < n_loc; i += FPS_THREADS) {
     const float x = xyz[3 * (lo + i)], y = xyz[3 * (lo + i) + 1], z = xyz[3 * (lo + i) + 2];
     const float mag = __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z));
@@ -304,15 +319,15 @@ dim3 gather_grid(int64_t cols, int64_t C, int64_t B) {
   return dim3((unsigned)((cols + G_THREADS - 1) / G_THREADS), (unsigned)((C + G_CH - 1) / G_CH), (unsigned)std::min<int64_t>(B, 65535));
 }
 
-int points_grad(const float* g, const int32_t* idx, const float* w, int R, int64_t B, int64_t C, int64_t N, int64_t L, float* grad, void* ws,
-                size_t ws_bytes, cudaStream_t st) {
+// readers of every source point: off [B*N + 1], svals (reader positions, ascending within a source point), carved from ws
+int csr_build(const int32_t* idx, int64_t B, int64_t N, int64_t L, void* ws, int32_t*& off, int32_t*& svals, cudaStream_t st) {
   const int64_t total = B * L, rows = B * N;
   char* p = (char*)ws;
   uint32_t* keys = (uint32_t*)p; p += align_up(total * 4);
   uint32_t* skeys = (uint32_t*)p; p += align_up(total * 4);
   int32_t* vals = (int32_t*)p; p += align_up(total * 4);
-  int32_t* svals = (int32_t*)p; p += align_up(total * 4);
-  int32_t* off = (int32_t*)p; p += align_up((rows + 1) * 4);
+  svals = (int32_t*)p; p += align_up(total * 4);
+  off = (int32_t*)p; p += align_up((rows + 1) * 4);
   size_t cb = cub_sort_bytes(total);
   int end_bit = 1;
   while (end_bit < 32 && ((uint64_t)1 << end_bit) <= (uint64_t)rows) ++end_bit;     // keys are <= rows (the sentinel)
@@ -323,7 +338,24 @@ int points_grad(const float* g, const int32_t* idx, const float* w, int R, int64
     g_launches.fetch_add(4);
   }
   csr_offsets_kernel<<<(unsigned)((rows + 1 + 255) / 256), 256, 0, st>>>(skeys, total, rows, off);
-  if (int e = check_launch("csr_offsets_kernel")) return e;
+  return check_launch("csr_offsets_kernel");
+}
+
+// row-major adjoint of a row gather: grad[a, c] = sum over the readers p of row a, ascending p, of g[p, c], in fp64
+__global__ void __launch_bounds__(G_THREADS) rows_sum_kernel(const float* __restrict__ g, const int32_t* __restrict__ off,
+                                                             const int32_t* __restrict__ svals, int64_t C, int64_t M, float* __restrict__ grad) {
+  const int64_t t = blockIdx.x * (int64_t)G_THREADS + threadIdx.x;
+  if (t >= M * C) return;
+  const int64_t a = t / C, c = t - a * C;
+  double acc = 0.0;
+  for (int32_t r = off[a]; r < off[a + 1]; ++r) acc += (double)g[(int64_t)svals[r] * C + c];
+  grad[t] = (float)acc;
+}
+
+int points_grad(const float* g, const int32_t* idx, const float* w, int R, int64_t B, int64_t C, int64_t N, int64_t L, float* grad, void* ws,
+                size_t ws_bytes, cudaStream_t st) {
+  int32_t *off = nullptr, *svals = nullptr;
+  if (int e = csr_build(idx, B, N, L, ws, off, svals, st)) return e;
   if (R == 1) csr_sum_kernel<1><<<gather_grid(N, C, B), G_THREADS, 0, st>>>(g, w, off, svals, B, C, N, L, grad);
   else csr_sum_kernel<3><<<gather_grid(N, C, B), G_THREADS, 0, st>>>(g, w, off, svals, B, C, N, L, grad);
   return check_launch("csr_sum_kernel");
@@ -335,13 +367,11 @@ extern "C" size_t pcb_furthest_point_sampling_ws_bytes(int64_t B, int64_t N) {
   return (B > 0 && N > 0 && fps_overflows(N)) ? (size_t)(B * N * 4) : 0;
 }
 
-extern "C" int pcb_furthest_point_sampling(const float* xyz, int64_t B, int64_t N, int64_t npoint, int32_t* idx, void* ws, size_t ws_bytes,
-                                           void* stream) {
-  PCB_ARG(B >= 0 && B < LIM && N >= 1 && N < LIM && npoint >= 1 && npoint < LIM && B * N < LIM && B * npoint < LIM);
-  if (B == 0) return PCB_OK;
-  PCB_ARG(xyz && idx && ws_bytes >= pcb_furthest_point_sampling_ws_bytes(B, N) && (ws || !fps_overflows(N)));
-  const int cs = fps_cluster(N);
-  const int64_t per_cta = (N + cs - 1) / cs;
+// one cluster per scene, its size chosen from max_n (the scene size, or an upper bound on it for ragged batches)
+int fps_launch(const float* xyz, const int64_t* offsets, int64_t B, int64_t N, int64_t total, int64_t max_n, int64_t npoint, int32_t* idx,
+               void* ws, cudaStream_t st) {
+  const int cs = fps_cluster(max_n);
+  const int64_t per_cta = (max_n + cs - 1) / cs;
   const size_t smem = (size_t)std::min<int64_t>(per_cta, FPS_SMEM_PTS) * sizeof(float4);
   PCB_ARG(B * cs < LIM);
   static bool attr_set[64] = {};
@@ -351,13 +381,34 @@ extern "C" int pcb_furthest_point_sampling(const float* xyz, int64_t B, int64_t 
     attr_set[dev] = true;
   }
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(B * cs)); cfg.blockDim = dim3(FPS_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = (cudaStream_t)stream;
+  cfg.gridDim = dim3((unsigned)(B * cs)); cfg.blockDim = dim3(FPS_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  cudaLaunchKernelEx(&cfg, fps_kernel, xyz, N, npoint, cs, per_cta, fps_overflows(N) ? (float*)ws : (float*)nullptr, idx);
+  cudaLaunchKernelEx(&cfg, fps_kernel, xyz, offsets, N, total, npoint, cs, per_cta, fps_overflows(max_n) ? (float*)ws : (float*)nullptr, idx);
   return check_launch("fps_kernel");
+}
+
+extern "C" int pcb_furthest_point_sampling(const float* xyz, int64_t B, int64_t N, int64_t npoint, int32_t* idx, void* ws, size_t ws_bytes,
+                                           void* stream) {
+  PCB_ARG(B >= 0 && B < LIM && N >= 1 && N < LIM && npoint >= 1 && npoint < LIM && B * N < LIM && B * npoint < LIM);
+  if (B == 0) return PCB_OK;
+  PCB_ARG(xyz && idx && ws_bytes >= pcb_furthest_point_sampling_ws_bytes(B, N) && (ws || !fps_overflows(N)));
+  return fps_launch(xyz, nullptr, B, N, B * N, N, npoint, idx, ws, (cudaStream_t)stream);
+}
+
+// max_n: an upper bound on every scene's size; no scene is larger than M, so a larger bound counts as M
+extern "C" size_t pcb_furthest_point_sampling_ragged_ws_bytes(int64_t B, int64_t M, int64_t max_n) {
+  return (B > 0 && M > 0 && max_n > 0 && M < LIM && fps_overflows(std::min(max_n, M))) ? (size_t)(M * 4) : 0;
+}
+
+extern "C" int pcb_furthest_point_sampling_ragged(const float* xyz, const int64_t* offsets, int64_t B, int64_t M, int64_t max_n, int64_t npoint,
+                                                  int32_t* idx, void* ws, size_t ws_bytes, void* stream) {
+  PCB_ARG(B >= 1 && B < LIM && M >= B && M < LIM && max_n >= 1 && npoint >= 1 && npoint < LIM && B * npoint < LIM);
+  max_n = std::min(max_n, M);
+  PCB_ARG(xyz && offsets && idx && ws_bytes >= pcb_furthest_point_sampling_ragged_ws_bytes(B, M, max_n) && (ws || !fps_overflows(max_n)));
+  return fps_launch(xyz, offsets, B, 0, M, max_n, npoint, idx, ws, (cudaStream_t)stream);
 }
 
 extern "C" int pcb_ball_query(const float* new_xyz, const float* xyz, int64_t B, int64_t M, int64_t N, float radius, int nsample, int32_t* idx,
@@ -410,6 +461,18 @@ extern "C" int pcb_gather_points_grad(const float* grad_out, const int32_t* idx,
   if (B == 0 || C == 0 || N == 0) return PCB_OK;
   PCB_ARG(grad_features && ws && ws_bytes >= pcb_points_grad_ws_bytes(B, N, L) && ((grad_out && idx) || L == 0));
   return points_grad(grad_out, idx, nullptr, 1, B, C, N, L, grad_features, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int pcb_gather_rows_grad(const float* grad_out, const int32_t* idx, int64_t L, int64_t C, int64_t M, float* grad_rows, void* ws,
+                                    size_t ws_bytes, void* stream) {
+  PCB_ARG(L >= 0 && C >= 0 && M >= 0 && L < LIM && C < LIM && M < LIM && M * C < (1ll << 40));
+  if (C == 0 || M == 0) return PCB_OK;
+  PCB_ARG(grad_rows && ws && ws_bytes >= pcb_points_grad_ws_bytes(1, M, L) && ((grad_out && idx) || L == 0));
+  cudaStream_t st = (cudaStream_t)stream;
+  int32_t *off = nullptr, *svals = nullptr;
+  if (int e = csr_build(idx, 1, M, L, ws, off, svals, st)) return e;
+  rows_sum_kernel<<<(unsigned)((M * C + G_THREADS - 1) / G_THREADS), G_THREADS, 0, st>>>(grad_out, off, svals, C, M, grad_rows);
+  return check_launch("rows_sum_kernel");
 }
 
 extern "C" int pcb_three_interpolate_grad(const float* grad_out, const int32_t* idx, const float* weight, int64_t B, int64_t C, int64_t n, int64_t m,

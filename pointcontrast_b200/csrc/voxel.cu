@@ -2,11 +2,15 @@
 // (`pretrain/pointcontrast/lib/ddp_data_loaders.py:196-265`), which today runs on CPU workers:
 //   * `ME.utils.sparse_quantize(xyz / voxel_size, return_index=True)` (`:228-241`; semseg: `lib/voxelizer.py:113-148`):
 //     one point per occupied voxel                                                          -> pcb_voxelize
+//   * the same per scene of a collated VoteNet batch, the scene index in the key (`downstream/votenet_det_new/models/backbone/
+//     sparseconv/voxelized_dataset.py:33-65`): rows scene-major, ascending first index        -> pcb_voxelize_scenes
 //   * its label variant on integer coordinates (semseg `lib/voxelizer.py:145-146`): a voxel keeps the label its points share,
 //     else ignore_label                                                                     -> pcb_voxelize_labels
 //   * `get_matching_indices` (`:36-49`): an open3d KD-tree radius search PER POINT, radius 1.5 voxels   -> pcb_radius_pairs
 // Both are integer / hashing work on the same primitives as the coordinate manager (radix sort + head flags + scan, the
 // open-addressing hash table of common.cuh); results are exact (tests/test_gpu_voxel.py: vs numpy / scipy cKDTree).
+#include <algorithm>
+#include <vector>
 #include <cub/cub.cuh>
 #include "common.cuh"
 
@@ -152,24 +156,63 @@ SortWs carve(void* ws, int64_t n) {
 }
 size_t carve_bytes(int64_t n) { return 2 * align_up(n * 8) + 4 * align_up(n * 4) + 512 + align_up(sort_scan_bytes(n)) + 256; }
 
-// keys w.k / indices w.idx -> stable sort -> head flags -> inclusive scan (rank)
-int sort_runs(int64_t n, SortWs& w, cudaStream_t st) {
+// keys w.k / indices w.idx -> stable sort (w.sk / w.sidx); w.k keeps each point's key at its original position
+int sort_keys(int64_t n, SortWs& w, cudaStream_t st) {
   size_t cb = w.cub_bytes;
   PCB_CUDA(cub::DeviceRadixSort::SortPairs(w.cub, cb, w.k, w.sk, w.idx, w.sidx, (int)n, 0, 63, st));
+  g_launches.fetch_add(8);
+  return PCB_OK;
+}
+
+// stable sort -> head flags -> inclusive scan (rank)
+int sort_runs(int64_t n, SortWs& w, cudaStream_t st) {
+  if (int e = sort_keys(n, w, st)) return e;
   head_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, n, w.flag);
   if (int e = check_launch("head_kernel")) return e;
-  cb = w.cub_bytes;
+  size_t cb = w.cub_bytes;
   PCB_CUDA(cub::DeviceScan::InclusiveSum(w.cub, cb, w.flag, w.rank, (int)n, st));
-  g_launches.fetch_add(10);
+  g_launches.fetch_add(2);
   return PCB_OK;
+}
+
+int point_keys(const float* xyz, int64_t n, float size, SortWs& w, cudaStream_t st) {
+  PCB_CUDA(cudaMemsetAsync(w.status, 0, sizeof(int32_t), st));
+  point_key_kernel<<<blocks_for(n, 256), 256, 0, st>>>(xyz, n, size, w.k, w.idx, w.status);
+  return check_launch("point_key_kernel");
 }
 
 // keys of the points' cells -> sort_runs
 int sort_cells(const float* xyz, int64_t n, float size, SortWs& w, cudaStream_t st) {
-  PCB_CUDA(cudaMemsetAsync(w.status, 0, sizeof(int32_t), st));
-  point_key_kernel<<<blocks_for(n, 256), 256, 0, st>>>(xyz, n, size, w.k, w.idx, w.status);
-  if (int e = check_launch("point_key_kernel")) return e;
+  if (int e = point_keys(xyz, n, size, w, st)) return e;
   return sort_runs(n, w, st);
+}
+
+// Batched voxelisation.  After the stable sort by cell key alone, a run of equal keys lists its points in ascending GLOBAL index, i.e.
+// grouped by scene (scenes are contiguous in the input) and ascending within each scene; so a (scene, cell) voxel starts where the key
+// or the scene changes, and its first element is the scene's smallest index in that cell.  The flag goes back to the head's ORIGINAL
+// position, so one exclusive scan over the input order numbers the voxels scene-major, ascending first index within a scene.
+__global__ void scene_head_kernel(const uint64_t* __restrict__ sk, const int32_t* __restrict__ sidx, int64_t n, int64_t N,
+                                  int32_t* __restrict__ flag) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  flag[sidx[i]] = (i == 0 || sk[i] != sk[i - 1] || sidx[i] / N != sidx[i - 1] / N) ? 1 : 0;
+}
+
+// row = exclusive scan of the flags at the head's position; offsets[b] = the scan at b * N, offsets[B] = M (also into stage[])
+__global__ void scene_write_kernel(const uint64_t* __restrict__ k, const int32_t* __restrict__ flag, const int64_t* __restrict__ row,
+                                   int64_t n, int64_t N, int32_t* __restrict__ coords, int32_t* __restrict__ inds, int64_t* __restrict__ offsets,
+                                   int64_t* __restrict__ stage) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t b = i / N;
+  if (i - b * N == 0) { offsets[b] = row[i]; stage[b] = row[i]; }
+  if (i == n - 1) { offsets[b + 1] = row[i] + flag[i]; stage[b + 1] = row[i] + flag[i]; }
+  if (!flag[i]) return;
+  const int64_t r = row[i];
+  const uint64_t key = k[i];
+  coords[4 * r] = (int32_t)b;
+  coords[4 * r + 1] = (int)(key >> 42) - VB; coords[4 * r + 2] = (int)((key >> 21) & 0x1FFFFF) - VB; coords[4 * r + 3] = (int)(key & 0x1FFFFF) - VB;
+  inds[r] = (int32_t)(i - b * N);
 }
 
 __global__ void int_key_kernel(const int32_t* __restrict__ c, int64_t n, uint64_t* __restrict__ keys, int32_t* __restrict__ idx, int32_t* status) {
@@ -222,6 +265,39 @@ extern "C" int pcb_voxelize(const float* xyz, int64_t n, float voxel_size, int32
   PCB_CUDA(cudaMemcpyAsync(&status, w.status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   PCB_CUDA(cudaStreamSynchronize(st));
   if (status) { set_error("pcb_voxelize: a point lies outside +-2^20 voxels"); return PCB_ERR_RANGE; }
+  return PCB_OK;
+}
+
+extern "C" size_t pcb_voxelize_scenes_ws_bytes(int64_t B, int64_t N) {
+  if (B < 1 || N < 1 || B * N >= (1ll << 31)) return 0;
+  return carve_bytes(B * N) + align_up((B + 2) * 8);
+}
+
+extern "C" int pcb_voxelize_scenes(const float* xyz, int64_t B, int64_t N, float voxel_size, int32_t* out_coords, int32_t* inds, int64_t* offsets,
+                                   int64_t* offsets_host, void* ws, size_t ws_bytes, void* stream) {
+  PCB_ARG(B >= 1 && N >= 1 && B * N < (1ll << 31) && voxel_size > 0.f);
+  PCB_ARG(xyz && out_coords && inds && offsets && offsets_host && ws && ws_bytes >= pcb_voxelize_scenes_ws_bytes(B, N));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t n = B * N;
+  SortWs w = carve(ws, n);
+  int64_t* stage = (int64_t*)w.end;                // offsets[0..B], then the range status: one copy back to the host
+  w.status = (int32_t*)(stage + B + 1);
+  PCB_CUDA(cudaMemsetAsync(stage + B + 1, 0, sizeof(int64_t), st));
+  if (int e = point_keys(xyz, n, voxel_size, w, st)) return e;
+  if (int e = sort_keys(n, w, st)) return e;
+  scene_head_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, w.sidx, n, N, w.flag);
+  if (int e = check_launch("scene_head_kernel")) return e;
+  int64_t* row = (int64_t*)w.sk;                   // the sorted keys are dead after the head flags
+  size_t cb = w.cub_bytes;
+  PCB_CUDA(cub::DeviceScan::ExclusiveSum(w.cub, cb, w.flag, row, (int)n, st));
+  g_launches.fetch_add(2);
+  scene_write_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.k, w.flag, row, n, N, out_coords, inds, offsets, stage);
+  if (int e = check_launch("scene_write_kernel")) return e;
+  std::vector<int64_t> host((size_t)B + 2);
+  PCB_CUDA(cudaMemcpyAsync(host.data(), stage, (B + 2) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  PCB_CUDA(cudaStreamSynchronize(st));
+  if ((int32_t)host[B + 1]) { set_error("pcb_voxelize_scenes: a point lies outside +-2^20 voxels"); return PCB_ERR_RANGE; }
+  std::copy(host.begin(), host.begin() + B + 1, offsets_host);
   return PCB_OK;
 }
 

@@ -886,6 +886,38 @@ def cat(*tensors):
     return SparseTensor(torch.cat([t.F for t in tensors], dim=1), coords_key=key, coords_manager=tensors[0].coords_man)
 
 
+def convert_to_int_tensor(arg, expand_dimension):
+    """ME 0.4.3 `MinkowskiCommon.convert_to_int_tensor`: an IntTensor of `expand_dimension` entries from a scalar or a sequence."""
+    if isinstance(arg, torch.IntTensor):
+        assert arg.numel() == expand_dimension
+        return arg
+    if isinstance(arg, (list, tuple, np.ndarray)):
+        tmp = torch.IntTensor([i for i in arg])
+        assert tmp.numel() == expand_dimension
+    elif np.isscalar(arg):
+        tmp = torch.IntTensor([int(arg) for _ in range(expand_dimension)])
+    else:
+        raise ValueError("Input must be a scalar or a sequence")
+    return tmp
+
+
+_CRF_ONLY = ("{} is used only by the CRF wrappers of the sparse-conv model package (`models/conditional_random_fields.py`: "
+             "BilateralCRF / TrilateralCRF), which this library does not provide; it exists so that the package imports")
+
+
+def convert_region_type(*args, **kwargs):
+    raise NotImplementedError(_CRF_ONLY.format("convert_region_type"))
+
+
+class MinkowskiConvolutionFunction:
+    def __init__(self, *args, **kwargs):
+        raise NotImplementedError(_CRF_ONLY.format("MinkowskiConvolutionFunction"))
+
+    @staticmethod
+    def apply(*args, **kwargs):
+        raise NotImplementedError(_CRF_ONLY.format("MinkowskiConvolutionFunction"))
+
+
 def install(name="MinkowskiEngine"):
     """Register this module as `MinkowskiEngine` (and `MinkowskiEngine.MinkowskiOps`)."""
     me = sys.modules[__name__]

@@ -53,6 +53,38 @@ def furthest_point_sampling(points, nsamples):
     return out
 
 
+def furthest_point_sampling_ragged(points, offsets, max_n, nsamples):
+    """points fp32 [M, 3] grouped by scene, offsets int64 [B + 1] on the same device (scene b is rows [offsets[b], offsets[b+1])),
+    max_n an upper bound on every scene's size -> int32 [B, nsamples] of scene-local indices: for every scene what
+    `furthest_point_sampling` returns for that scene alone, all scenes in one launch."""
+    _check(points, torch.float32, "points"); _check(offsets, torch.int64, "offsets", points.device)
+    _dims(points, 2, "points", last=3); _dims(offsets, 1, "offsets")
+    M, B = points.shape[0], offsets.shape[0] - 1
+    out = torch.empty(B, int(nsamples), dtype=torch.int32, device=points.device)
+    with torch.cuda.device(points.device):
+        wsb = lib.pcb_furthest_point_sampling_ragged_ws_bytes(B, M, int(max_n))
+        ws = workspace(wsb, points.device, slot=_WS_SLOT) if wsb else None
+        check(lib.pcb_furthest_point_sampling_ragged(ptr(points), ptr(offsets), B, M, int(max_n), int(nsamples), ptr(out), ptr(ws), wsb,
+                                                     stream()))
+    return out
+
+
+def gather_rows_grad(grad_out, idx, m):
+    """Adjoint of rows[idx] for rows [m, C]: grad_out fp32 [L, C], idx int32 [L] -> [m, C], each row the sum of its readers'
+    gradients in ascending reader order (fp64, deterministic)."""
+    _check(grad_out, torch.float32, "grad_out"); _check(idx, torch.int32, "idx", grad_out.device)
+    _dims(grad_out, 2, "grad_out"); _dims(idx, 1, "idx")
+    L, C = grad_out.shape
+    if idx.shape[0] != L:
+        raise PcbError(f"idx has {idx.shape[0]} entries, grad_out {L} rows")
+    out = torch.empty(int(m), C, dtype=torch.float32, device=grad_out.device)
+    with torch.cuda.device(grad_out.device):
+        wsb = lib.pcb_points_grad_ws_bytes(1, int(m), L)
+        ws = workspace(wsb, grad_out.device, slot=_WS_SLOT)
+        check(lib.pcb_gather_rows_grad(ptr(grad_out), ptr(idx), L, C, int(m), ptr(out), ptr(ws), wsb, stream()))
+    return out
+
+
 def gather_points(points, idx):
     """points fp32 [B, C, N], idx int32 [B, M] -> [B, C, M]."""
     _check(points, torch.float32, "points"); _check(idx, torch.int32, "idx", points.device)

@@ -172,6 +172,17 @@ def synth_batch(step, batch_size, scale=0.9, voxel=0.025, n_raw=300_000):
     return collate_pairs([synth_pair(1000 * step + p, scale, voxel, n_raw) for p in range(batch_size)])
 
 
+def synth_votenet_batch(seed, batch_size, num_points, scale=1.5):
+    """VoteNet's collated `point_clouds` (`no_height=True`, `use_color=False`): float32 [batch_size, num_points, 3], scene b a room of
+    about 4.8 m x 4.5 m x 3.6 m (at scale 1.5) sampled with seed 1000 * seed + b, centred in x and y, floor at z = 0."""
+    out = np.empty((batch_size, num_points, 3), np.float32)
+    for b in range(batch_size):
+        pts = synth_room(1000 * seed + b, scale, num_points)
+        pts[:, :2] -= pts[:, :2].mean(0)
+        out[b] = pts
+    return out
+
+
 def synth_scene(seed, scale=2.5, voxel=0.05, n_raw=1_500_000):
     """S3DIS-shaped single room for the forward-only config (C4): coords [N,4], RGB/255-0.5 features."""
     rng = np.random.default_rng(seed + 99)

@@ -31,6 +31,27 @@ def voxelize(xyz, voxel_size):
     return coords[:m.value], sel[:m.value].long()
 
 
+def voxelize_scenes(xyz, voxel_size):
+    """xyz: float32 CUDA [B,N,3], one scene per row.  Returns (coords int32 [M,4] = (b, x, y, z), inds int32 [M]: the scene-local
+    index of each voxel's first point, offsets int64 [B+1] on the device, offsets as a host list).  Rows are scene-major and, within a
+    scene, in ascending `inds`.  Synchronises once."""
+    _lib.require_cuda(xyz)
+    if xyz.dim() != 3 or xyz.shape[2] != 3:
+        raise _lib.PcbError(f"xyz must be [B, N, 3], got {tuple(xyz.shape)}")
+    xyz = xyz.contiguous().float()
+    B, N, _ = xyz.shape
+    coords = torch.empty(B * N, 4, dtype=torch.int32, device=xyz.device)
+    inds = torch.empty(B * N, dtype=torch.int32, device=xyz.device)
+    offsets = torch.empty(B + 1, dtype=torch.int64, device=xyz.device)
+    host = (ctypes.c_int64 * (B + 1))()
+    with torch.cuda.device(xyz.device):
+        wsb = lib.pcb_voxelize_scenes_ws_bytes(B, N)
+        ws = workspace(wsb, xyz.device, slot=6)
+        check(lib.pcb_voxelize_scenes(ptr(xyz), B, N, float(voxel_size), ptr(coords), ptr(inds), ptr(offsets), host, ptr(ws), wsb, stream()))
+    m = host[B]
+    return coords[:m], inds[:m], offsets, list(host)
+
+
 def radius_pairs(src, dst, radius):
     """src [Ns,3], dst [Nd,3] float32 CUDA.  Returns int32 [P,2]: every (i, j) with |src_i - dst_j| < radius, sorted by (i, j)."""
     _lib.require_cuda(src); _lib.require_cuda(dst)
