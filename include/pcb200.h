@@ -150,9 +150,9 @@ int pcb_conv_forward(const float* X, int ldx, const int32_t* tbl, int64_t tbl_st
 #define PCB_CONV_FORCE_SIMT 1  /* pcb_conv_wgrad: the generic exact kernel also for the stem layer (a cross-check of the stem kernel) */
 #define PCB_CONV_ACCUMULATE 4  /* Y += result (pcb_conv_forward_split) / dW += result (weight gradients) */
 #define PCB_PLANES_A_FP16 8    /* split-operand calls: the GATHERED operand's planes are fp16 hi/lo (default: bf16 hi/lo) */
-#define PCB_PLANES_B_FP16 16   /* pcb_conv_forward_split: the weight tiles are fp16 x 2^10 (pcb_weight_tile with this flag);
-                                  pcb_conv_wgrad_split: the ROW-ALIGNED operand's planes are fp16.  Both operands of a call must
-                                  use the same format (wgmma takes one 16-bit format for both operands): set both flags or neither. */
+#define PCB_PLANES_B_FP16 16   /* pcb_conv_forward_split: the weight tiles are fp16 x 2^10 (pcb_weight_tile with this flag).  Both
+                                  operands of a call must use the same format (wgmma takes one 16-bit format for both operands): set
+                                  both flags or neither.  pcb_conv_wgrad_split reads bf16 planes only and rejects either flag. */
 
 /* Y[j, :] = sum_k X[tbl[kmap[k]][j], :];  cnt[j] (optional) = number of neighbours present.  The sum / average pooling and unpooling
  * layers of the sibling models (MinkowskiSumPooling / AvgPooling / PoolingTranspose / AvgUnpooling, `model/modules/common.py:170-214`,
@@ -194,38 +194,29 @@ size_t pcb_conv_forward_split_ws_bytes(int K, int64_t n_out, int Cin, int Cout);
 int pcb_conv_forward_split(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride,
                            const int32_t* kmap, int K, int64_t n_out, int Cin, int Cout, const void* w_tiles,
                            const float* bias, float* Y, int ldy, void* ws, size_t ws_bytes, int flags, void* stream);
+/* pcb_conv_wgrad_split: both operands as bf16 hi/lo planes; flags: PCB_CONV_ACCUMULATE only (PCB_ERR_ARG if a PCB_PLANES_* flag
+ * is set). */
 size_t pcb_conv_wgrad_split_ws_bytes(int K, int64_t n_out, int Ca, int Cb);
 int pcb_conv_wgrad_split(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
                          const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int Ca, int Cb, float* dW,
                          int transpose_out, void* ws, size_t ws_bytes, int flags, void* stream);
 
 /* ----------------------------------------------------------------------------------------------- batch norm */
-/* Training-mode statistics over n rows: mean[C], invstd[C] = 1/sqrt(var_biased + eps); if running_* non-NULL:
- * running = (1-momentum)*running + momentum*{mean, var_unbiased}.  ws: pcb_bn_ws_bytes(n, C). */
-size_t pcb_bn_ws_bytes(int64_t n, int C);
-int pcb_bn_stats(const float* X, int64_t n, int C, float eps, float momentum, float* mean, float* invstd,
-                 float* running_mean, float* running_var, void* ws, size_t ws_bytes, void* stream);
-/* Y = (X - mean) * invstd * gamma + beta  [+ residual] [relu].   Y may alias X. */
-int pcb_bn_apply(const float* X, int64_t n, int C, const float* mean, const float* invstd, const float* gamma,
-                 const float* beta, const float* residual, int relu, float* Y, void* stream);
-/* Backward of the affine-normalise (no relu): given dY and X, writes dX, dgamma[C], dbeta[C]. */
-int pcb_bn_backward(const float* dY, const float* X, int64_t n, int C, const float* mean, const float* invstd,
-                    const float* gamma, float* dX, float* dgamma, float* dbeta, void* ws, size_t ws_bytes,
-                    void* stream);
-
-/* Strided / row-segmented variants used by the fused network executor (pointcontrast_b200/fused.py).  All ld* are row strides
+/* Training-mode BatchNorm on row-segmented matrices: rows [0, n0) and [n0, n) are two independent BatchNorm batches -- the two views
+ * of a scene pair stacked in one feature matrix, each normalised with its own statistics exactly as the reference's two forward calls
+ * do (`lib/ddp_trainer.py:290-297,392-398`); n0 == n is one batch (MinkowskiBatchNorm on the modular surface).  All ld* are row strides
  * in floats (>= C, multiples of 4), so inputs/outputs may be column slices of wider (concatenated) buffers.
+ *   stats   : mean[seg][C], invstd[seg][C] = 1/sqrt(var_biased + eps); if running_* non-NULL:
+ *             running = (1-momentum)*running + momentum*{mean, var_unbiased}, with segment 0 and then with segment 1.
+ *             ws: pcb_bn_ws_bytes(n, C).
  *   apply   : Y = [relu]( (X-mean)*invstd*gamma+beta [+ residual] ), as fp32 (Y, may be NULL) and/or split planes (Yhi/Ylo);
  *             flags: PCB_BN_RELU, PCB_PLANES_A_FP16 (Yhi/Ylo are fp16 hi/lo instead of bf16 hi/lo; Ybhi/Yblo, if non-NULL, then
  *             receive the bf16 hi/lo planes as well)
- *   backward: g = dY * (relu_out > 0) if relu_out else dY;   dgamma/dbeta (+)= sum(g*xhat) / sum(g);
+ *   backward: g = dY * (relu_out > 0) if relu_out else dY;   dgamma/dbeta (+)= sum(g*xhat) / sum(g), summed over both segments;
  *             dX = gamma*invstd*(g - mean(g) - xhat*mean(g*xhat));   gout (=|+=) g  (gout_mode 0 none, 1 write, 2 add)
  *             -- gout is the gradient of the residual input of the forward unit; it may alias dY. */
 #define PCB_BN_RELU 1
-/* Row-segmented variants: rows [0, n0) and [n0, n) are two independent BatchNorm batches -- the two views of a scene pair
- * stacked in one feature matrix, each normalised with its own statistics exactly as the reference's two forward calls do
- * (`lib/ddp_trainer.py:290-297,392-398`).  mean / invstd are [2][C]; the running statistics are updated with segment 0 and
- * then with segment 1; dgamma / dbeta sum over both segments.  n0 == n degenerates to the single-batch functions above. */
+size_t pcb_bn_ws_bytes(int64_t n, int C);
 int pcb_bn_stats_seg(const float* X, int ldx, int64_t n, int64_t n0, int C, float eps, float momentum, float* mean, float* invstd,
                      float* running_mean, float* running_var, void* ws, size_t ws_bytes, void* stream);
 int pcb_bn_apply_seg(const float* X, int ldx, int64_t n, int64_t n0, int C, const float* mean, const float* invstd,
@@ -302,7 +293,7 @@ int pcb_unit_backward(const pcb_unit* u, void* stream);
  * Writes loss (device float), dq, dk (= d loss / d q, d k).  ws: pcb_nce_ws_bytes(n).
  * D = 32 or 64: fused wgmma kernels (nce_wgmma.cu) -- q k^T tiles on the tensor cores from fp16 hi/lo operands (|q|,|k| <= ~1: the
  * L2-normalised features), softmax statistics and both gradients straight from the tiles, the n x n logits never stored.
- * Other widths (or PCB_NCE_SIMT=1): exact fp32 SIMT kernels that materialise the logits in ws. */
+ * Other widths: exact fp32 SIMT kernels that materialise the logits in ws. */
 size_t pcb_nce_ws_bytes(int64_t n);
 int pcb_nce_forward_backward(const float* q, const float* k, int64_t n, int D, float inv_T, float* loss, float* dq,
                              float* dk, void* ws, size_t ws_bytes, void* stream);

@@ -63,9 +63,6 @@ _SIGS = {
     "pcb_conv_wgrad_split_ws_bytes": (_sz, [_i, _l, _i, _i]),
     "pcb_conv_wgrad_split": (_i, [_p, _p, _i, _p, _p, _i, _p, _l, _i, _l, _i, _i, _p, _i, _p, _sz, _i, _p]),
     "pcb_bn_ws_bytes": (_sz, [_l, _i]),
-    "pcb_bn_stats": (_i, [_p, _l, _i, _f, _f, _p, _p, _p, _p, _p, _sz, _p]),
-    "pcb_bn_apply": (_i, [_p, _l, _i, _p, _p, _p, _p, _p, _i, _p, _p]),
-    "pcb_bn_backward": (_i, [_p, _p, _l, _i, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "pcb_bn_stats_seg": (_i, [_p, _i, _l, _l, _i, _f, _f, _p, _p, _p, _p, _p, _sz, _p]),
     "pcb_bn_apply_seg": (_i, [_p, _i, _l, _l, _i, _p, _p, _p, _p, _p, _i, _i, _p, _i, _p, _p, _i, _p, _p, _p]),
     "pcb_bn_backward_seg": (_i, [_p, _i, _p, _i, _p, _i, _l, _l, _i, _p, _p, _p, _p, _i, _p, _p, _i, _p, _i, _i, _p, _p, _i, _p, _sz,

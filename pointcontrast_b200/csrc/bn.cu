@@ -391,11 +391,6 @@ extern "C" int pcb_bn_stats_seg(const float* X, int ldx, int64_t n, int64_t n0, 
   return check_launch("bn_finalize_kernel");
 }
 
-extern "C" int pcb_bn_stats(const float* X, int64_t n, int C, float eps, float momentum, float* mean, float* invstd,
-                            float* running_mean, float* running_var, void* ws, size_t ws_bytes, void* stream) {
-  return pcb_bn_stats_seg(X, C, n, n, C, eps, momentum, mean, invstd, running_mean, running_var, ws, ws_bytes, stream);
-}
-
 extern "C" int pcb_split_rows(const float* X, int ldx, int64_t n, int C, uint16_t* hi, uint16_t* lo, int lds, int flags, void* stream) {
   PCB_ARG(n >= 0 && C >= 4 && C % 4 == 0 && ldx >= C && ldx % 4 == 0 && lds >= C && lds % 4 == 0);
   if (n == 0) return PCB_OK;
@@ -420,11 +415,6 @@ extern "C" int pcb_bn_apply_seg(const float* X, int ldx, int64_t n, int64_t n0, 
                 ldr, relu, Y, ldy, (__nv_bfloat16*)Yhi, (__nv_bfloat16*)Ylo, lds, n0, (flags & PCB_PLANES_A_FP16) ? 1 : 0,
                 (__nv_bfloat16*)Ybhi, (__nv_bfloat16*)Yblo);
   return check_launch("bn_apply_kernel");
-}
-
-extern "C" int pcb_bn_apply(const float* X, int64_t n, int C, const float* mean, const float* invstd, const float* gamma,
-                            const float* beta, const float* residual, int relu, float* Y, void* stream) {
-  return pcb_bn_apply_seg(X, C, n, n, C, mean, invstd, gamma, beta, residual, C, relu, Y, C, nullptr, nullptr, 0, nullptr, nullptr, stream);
 }
 
 namespace pcb {
@@ -494,11 +484,4 @@ extern "C" int pcb_bn_backward_seg(const float* dY, int lddy, const float* X, in
                                    uint16_t* dXhi, uint16_t* dXlo, int lds, void* ws, size_t ws_bytes, void* stream) {
   return pcb::bn_backward_impl(dY, lddy, X, ldx, relu_out, ldm, nullptr, 0, n, n0, C, mean, invstd, gamma, dX, lddx, dgamma, dbeta,
                                accumulate_param_grads, gout, ldg, gout_mode, dXhi, dXlo, lds, ws, ws_bytes, (cudaStream_t)stream);
-}
-
-extern "C" int pcb_bn_backward(const float* dY, const float* X, int64_t n, int C, const float* mean, const float* invstd,
-                               const float* gamma, float* dX, float* dgamma, float* dbeta, void* ws, size_t ws_bytes,
-                               void* stream) {
-  return pcb_bn_backward_seg(dY, C, X, C, nullptr, 0, n, n, C, mean, invstd, gamma, dX, C, dgamma, dbeta, 0, nullptr, 0, 0, nullptr,
-                             nullptr, 0, ws, ws_bytes, stream);
 }

@@ -50,13 +50,13 @@ struct ProfScope {
   ~ProfScope() { prof_end(st, kind); }
 };
 
-// Programmatic dependent launch (default; PCB_PDL=0 turns it off): every kernel below starts with pdl_wait() -- it blocks until the preceding kernel of
-// the stream has completed and its writes are visible -- followed by pdl_trigger(), which lets the NEXT kernel's CTAs be scheduled
-// as soon as all of this kernel's CTAs are running.  The launch latency and CTA ramp-up of a kernel then overlap the tail of its
-// predecessor; ordering is unchanged (nothing precedes the wait).  Launched without the attribute, both are no-ops.
+// Programmatic dependent launch: launch_kernel() launches every kernel with programmatic stream serialisation, and every kernel
+// below starts with pdl_wait() -- it blocks until the preceding kernel of the stream has completed and its writes are visible --
+// followed by pdl_trigger(), which lets the NEXT kernel's CTAs be scheduled as soon as all of this kernel's CTAs are running.  The
+// launch latency and CTA ramp-up of a kernel then overlap the tail of its predecessor; ordering is unchanged (nothing precedes the
+// wait).  In a kernel launched with <<<>>> (no attribute) both are no-ops.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-bool pdl_enabled();
 
 template <typename... Exp, typename... Act>
 inline void launch_kernel(void (*kernel)(Exp...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Act&&... args) {
@@ -65,7 +65,7 @@ inline void launch_kernel(void (*kernel)(Exp...), dim3 grid, dim3 block, size_t 
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   cudaLaunchKernelEx(&cfg, kernel, static_cast<Act&&>(args)...);       // errors surface through check_launch (cudaGetLastError)
 }
 

@@ -12,7 +12,6 @@
 // parity (tests: 1e-3 relative against the fp64 oracle after 63 layers).  The exact fp32 entry points (pcb_conv_forward /
 // pcb_conv_wgrad) cover the channel counts the tensor-core tiling does not (Cin = 3, odd widths) and are the in-library
 // cross-check of the tensor-core ones.
-#include <stdlib.h>
 #include <cuda_fp16.h>
 #include "common.cuh"
 
@@ -233,8 +232,7 @@ int conv_splits(int K, int64_t n_out, int Cin, int Cout) {
   int64_t base = ((n_out + BM - 1) / BM) * (Cout / bn);
   const int64_t one_wave = num_sms();          // the tensor-core kernel runs one CTA per SM
   if (base >= one_wave) return 1;
-  static double waves = 0.0;        // CTAs to aim for on a small level, in units of one resident wave
-  if (waves == 0.0) { const char* e = getenv("PCB_CONV_SPLIT_WAVES"); waves = e ? atof(e) : 0.5; if (waves < 0.05) waves = 0.05; }
+  const double waves = 0.5;         // CTAs to aim for on a small level, in units of one resident wave
   int64_t s = ((int64_t)(waves * one_wave) + base - 1) / base;
   int64_t T = (int64_t)K * (Cin / BK);
   if (s > T) s = T;
@@ -259,7 +257,7 @@ namespace pcb {
 int wgrad_group();
 int launch_wgrad_wgmma(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
                          const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int Ca, int Cb, int rows_per_split, int splits,
-                         float* partial, int transpose_out, int tn, cudaStream_t st, int a_fp16 = 0, int b_fp16 = 0);
+                         float* partial, int transpose_out, int tn, cudaStream_t st);
 int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl, int64_t tbl_stride,
                       const int* kmap, int K, int64_t n_out, int Cin, int Cout, const float* bias, float* Y, int ldy,
                       float* partial, int nsplit, int bn, int accumulate, cudaStream_t st, int x_fp16, int w_fp16);
@@ -351,53 +349,6 @@ extern "C" int pcb_conv_wgrad(const float* A, int lda, const float* B, int ldb, 
 namespace {
 __host__ __device__ inline int64_t tile_plane_bytes(int bn) { return 4ll * ((bn / 8) * 128 + 16); }
 
-__global__ void weight_tile_kernel(const float* __restrict__ W, int K, int Cin, int Cout, int bn_f, int bn_d,
-                                   unsigned char* __restrict__ fwd, unsigned char* __restrict__ dg, int fwd_fp16) {
-  pdl_wait(); pdl_trigger();
-  int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (e >= (int64_t)K * Cin * Cout) return;
-  const float w = W[e];
-  const __nv_bfloat16 h = __float2bfloat16_rn(w);
-  const __nv_bfloat16 l = __float2bfloat16_rn(w - __bfloat162float(h));
-  const int co = (int)(e % Cout);
-  const int64_t r = e / Cout;
-  const int ci = (int)(r % Cin);
-  const int k = (int)(r / Cin);
-  {   // forward roles: N = Cout, contraction = Cin
-    const int64_t plane = tile_plane_bytes(bn_f);
-    const int64_t blob = ((int64_t)(k * (Cin / 32) + ci / 32) * (Cout / bn_f) + co / bn_f) * 2 * plane;
-    const int n = co % bn_f, c = ci % 32;
-    const int64_t off = blob + (c / 8) * (plane / 4) + (n / 8) * 128 + (n % 8) * 16 + (c % 8) * 2;
-    if (fwd_fp16) {          // fp16 hi/lo of W * 2^10: the lo plane stays in fp16's normal range for every weight that matters
-      const float ws = fminf(fmaxf(w * 1024.0f, -65000.f), 65000.f);
-      const __half fh = __float2half_rn(ws);
-      const __half fl = __float2half_rn(ws - __half2float(fh));
-      *reinterpret_cast<__half*>(fwd + off) = fh;
-      *reinterpret_cast<__half*>(fwd + off + plane) = fl;
-    } else {
-      *reinterpret_cast<__nv_bfloat16*>(fwd + off) = h;
-      *reinterpret_cast<__nv_bfloat16*>(fwd + off + plane) = l;
-    }
-  }
-  {   // data-gradient roles: N = Cin, contraction = Cout
-    const int64_t plane = tile_plane_bytes(bn_d);
-    const int64_t blob = ((int64_t)(k * (Cout / 32) + co / 32) * (Cin / bn_d) + ci / bn_d) * 2 * plane;
-    const int n = ci % bn_d, c = co % 32;
-    const int64_t off = blob + (c / 8) * (plane / 4) + (n / 8) * 128 + (n % 8) * 16 + (c % 8) * 2;
-    *reinterpret_cast<__nv_bfloat16*>(dg + off) = h;
-    *reinterpret_cast<__nv_bfloat16*>(dg + off + plane) = l;
-  }
-}
-}  // namespace
-
-// All convolutions of a network in ONE launch (the fused executor re-tiles every kernel after each SGD step: 62 small launches
-// otherwise).  descs: DEVICE array; `start` = prefix sum of K*Cin*Cout; a thread finds its convolution by binary search.
-// A thread produces one 16-byte chunk (8 contraction-direction elements of one tile row) of BOTH planes for each role, so the tile
-// images are written with 128-bit stores that line up across a warp (the element-per-thread version, `weight_tile_kernel`, scatters
-// 2-byte stores: 0.53 ms per step for the 38 M parameters).  Forward roles: 8 consecutive input channels of one output channel
-// (threads along Cout: 8 coalesced 4-byte loads); data-gradient roles: 8 consecutive output channels of one input channel (threads along
-// Cin: two 128-bit loads).
-namespace {
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b, float& ra, float& rb) {
   const __nv_bfloat16 ha = __float2bfloat16_rn(a), hb = __float2bfloat16_rn(b);
   ra = a - __bfloat162float(ha); rb = b - __bfloat162float(hb);
@@ -423,17 +374,11 @@ __device__ __forceinline__ void split8(const float (&w)[8], uint4& hi, uint4& lo
   hi = make_uint4(h[0], h[1], h[2], h[3]); lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
-__global__ void weight_tile_batch_kernel(const pcb_tile_desc* __restrict__ descs, int n, int64_t total) {
-  pdl_wait(); pdl_trigger();
-  __shared__ int64_t s_start[257];
-  for (int i = threadIdx.x; i <= n; i += blockDim.x) s_start[i] = i < n ? descs[i].start : total;
-  __syncthreads();
-  const int64_t t8 = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;      // chunk index; every start is a multiple of 8 (channels % 32 == 0)
-  if (t8 * 8 >= total) return;
-  int lo_ = 0, hi_ = n - 1;
-  while (lo_ < hi_) { const int mid = (lo_ + hi_ + 1) >> 1; if (s_start[mid] <= t8 * 8) lo_ = mid; else hi_ = mid - 1; }
-  const pcb_tile_desc d = descs[lo_];
-  const int64_t t = t8 - d.start / 8;
+// Chunk t of convolution d: one 16-byte chunk (8 contraction-direction elements of one tile row) of BOTH planes for each role, so the
+// tile images are written with 128-bit stores that line up across a warp (an element per thread scatters 2-byte stores: 0.53 ms per
+// step for the 38 M parameters).  Forward roles: 8 consecutive input channels of one output channel (threads along Cout: 8 coalesced
+// 4-byte loads); data-gradient roles: 8 consecutive output channels of one input channel (threads along Cin: two 128-bit loads).
+__device__ __forceinline__ void weight_tile_chunk(const pcb_tile_desc& d, int64_t t) {
   const int Cin = d.Cin, Cout = d.Cout;
   const float* __restrict__ W = d.W;
   {   // forward roles: N = Cout, contraction = Cin; chunk = input channels ci0 .. ci0 + 7 of output channel co
@@ -473,6 +418,28 @@ __global__ void weight_tile_batch_kernel(const pcb_tile_desc* __restrict__ descs
     *reinterpret_cast<uint4*>(dst + plane) = l;
   }
 }
+
+// One convolution (pcb_weight_tile): d passed by value, `chunks` = K*Cin*Cout / 8.
+__global__ void weight_tile_single_kernel(const pcb_tile_desc d, int64_t chunks) {
+  pdl_wait(); pdl_trigger();
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (t < chunks) weight_tile_chunk(d, t);
+}
+
+// All convolutions of a network in ONE launch (the fused executor re-tiles every kernel after each SGD step: 62 small launches
+// otherwise).  descs: DEVICE array; `start` = prefix sum of K*Cin*Cout; a thread finds its convolution by binary search.
+__global__ void weight_tile_batch_kernel(const pcb_tile_desc* __restrict__ descs, int n, int64_t total) {
+  pdl_wait(); pdl_trigger();
+  __shared__ int64_t s_start[257];
+  for (int i = threadIdx.x; i <= n; i += blockDim.x) s_start[i] = i < n ? descs[i].start : total;
+  __syncthreads();
+  const int64_t t8 = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;      // chunk index; every start is a multiple of 8 (channels % 32 == 0)
+  if (t8 * 8 >= total) return;
+  int lo_ = 0, hi_ = n - 1;
+  while (lo_ < hi_) { const int mid = (lo_ + hi_ + 1) >> 1; if (s_start[mid] <= t8 * 8) lo_ = mid; else hi_ = mid - 1; }
+  const pcb_tile_desc d = descs[lo_];
+  weight_tile_chunk(d, t8 - d.start / 8);
+}
 }  // namespace
 
 extern "C" int pcb_tile_desc_fill(pcb_tile_desc* d, const float* W, int K, int Cin, int Cout, void* fwd_tiles, void* dgrad_tiles, int flags,
@@ -499,11 +466,11 @@ extern "C" size_t pcb_weight_tile_bytes(int K, int Cin, int Cout, int dgrad_role
 }
 
 extern "C" int pcb_weight_tile(const float* W, int K, int Cin, int Cout, void* fwd_tiles, void* dgrad_tiles, int flags, void* stream) {
-  PCB_ARG(W && fwd_tiles && dgrad_tiles && K >= 1 && Cin % 32 == 0 && Cout % 32 == 0 && Cin >= 32 && Cout >= 32);
-  int64_t n = (int64_t)K * Cin * Cout;
-  launch_kernel(weight_tile_kernel, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, W, K, Cin, Cout, pick_tile(Cout), pick_tile(Cin),
-                (unsigned char*)fwd_tiles, (unsigned char*)dgrad_tiles, (flags & PCB_PLANES_B_FP16) ? 1 : 0);
-  return check_launch("weight_tile_kernel");
+  pcb_tile_desc d;
+  if (int e = pcb_tile_desc_fill(&d, W, K, Cin, Cout, fwd_tiles, dgrad_tiles, flags, 0)) return e;
+  const int64_t chunks = (int64_t)K * Cin * Cout / 8;
+  launch_kernel(weight_tile_single_kernel, (unsigned)((chunks + 255) / 256), 256, 0, (cudaStream_t)stream, d, chunks);
+  return check_launch("weight_tile_single_kernel");
 }
 
 namespace pcb {
@@ -566,8 +533,7 @@ int wgrad_split_splits(int K, int64_t n_out, int Ca, int Cb) {
   int tn = pick_tile(Cb);
   const int gk = pcb::wgrad_group();          // offsets per CTA
   int64_t base = (int64_t)((K + gk - 1) / gk) * ((Ca + 127) / 128) * (Cb / tn);      // CTAs per split: offset groups x channel blocks
-  static double wwaves = 0.0;
-  if (wwaves == 0.0) { const char* e = getenv("PCB_WGRAD_SPLIT_WAVES"); wwaves = e ? atof(e) : 1.0; if (wwaves < 0.05) wwaves = 0.05; }
+  const double wwaves = 1.0;
   // heuristic, not tuned on H100: aim for 2 x num_sms CTAs (two waves of a kernel that fits once per SM), never a nearly-empty extra
   // wave; shorter row ranges per split also keep each fp32 accumulator's sum short
   int64_t s = (int64_t)(wwaves * 2 * num_sms()) / base;
@@ -589,6 +555,7 @@ extern "C" int pcb_conv_wgrad_split(const uint16_t* Ahi, const uint16_t* Alo, in
                                     int transpose_out, void* ws, size_t ws_bytes, int flags, void* stream) {
   PCB_ARG(K >= 1 && K <= PCB_MAX_KERNEL_VOLUME && n_out >= 0 && Ca % 32 == 0 && Cb % 32 == 0 && Ca >= 32 && Cb >= 32 && dW);
   PCB_ARG(lda >= Ca && ldb >= Cb && lda % 8 == 0 && ldb % 8 == 0);
+  PCB_ARG(!(flags & (PCB_PLANES_A_FP16 | PCB_PLANES_B_FP16)));       // the weight gradient reads bf16 hi/lo planes only
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t nW = (int64_t)K * Ca * Cb;
   if (n_out == 0) {
@@ -596,15 +563,13 @@ extern "C" int pcb_conv_wgrad_split(const uint16_t* Ahi, const uint16_t* Alo, in
     return PCB_OK;
   }
   PCB_ARG(Ahi && Alo && Bhi && Blo && tbl && ws && tbl_stride >= n_out);
-  // wgmma takes ONE 16-bit format for both operands
-  PCB_ARG(((flags & PCB_PLANES_A_FP16) != 0) == ((flags & PCB_PLANES_B_FP16) != 0));
   ProfScope prof(st, 1);
   const int splits = wgrad_split_splits(K, n_out, Ca, Cb);
   PCB_ARG(ws_bytes >= (size_t)splits * nW * sizeof(float));
   int64_t rps = (n_out + splits - 1) / splits;
   rps = (rps + 15) / 16 * 16;
   if (int e = launch_wgrad_wgmma(Ahi, Alo, lda, Bhi, Blo, ldb, tbl, tbl_stride, K, n_out, Ca, Cb, (int)rps, splits, (float*)ws,
-                                 transpose_out, pick_tile(Cb), st, (flags & PCB_PLANES_A_FP16) ? 1 : 0, (flags & PCB_PLANES_B_FP16) ? 1 : 0)) return e;
+                                 transpose_out, pick_tile(Cb), st)) return e;
   launch_kernel(wgrad_reduce_kernel, (unsigned)((nW + 255) / 256), 256, 0, st, (const float*)ws, splits, nW, dW,
                                                                     (flags & PCB_CONV_ACCUMULATE) ? 1 : 0);
   return check_launch("wgrad_reduce_kernel");

@@ -269,7 +269,7 @@ __host__ __device__ inline int a_lbo(int mrows) { return (mrows / 8) * SBO + 16;
 __host__ __device__ inline int b_lbo(int tn) { return (tn / 8) * SBO + 16; }
 __host__ __device__ inline int stage_bytes(int mrows, int tn) { return 4 * b_lbo(tn) + GK * 4 * a_lbo(mrows); }
 
-template <int TN, bool F16>
+template <int TN>
 __global__ void __launch_bounds__(NTHR, 1) wgrad_wgmma_kernel(const Args p) {
   using namespace hw;
   extern __shared__ __align__(128) unsigned char smem[];
@@ -367,9 +367,9 @@ __global__ void __launch_bounds__(NTHR, 1) wgrad_wgmma_kernel(const Args p) {
       for (int g = 0; g < GK; ++g) {
         const uint32_t ab = sb + 4 * B_LBO + g * 4 * A_LBO + wgi * 8 * SBO;
         const uint64_t dah = make_desc(ab, A_LBO, SBO), dal = make_desc(ab + 2 * A_LBO, A_LBO, SBO);
-        wgmma<TN, F16, 1, 1>(acc[g], dal, dbh, 1u);
-        wgmma<TN, F16, 1, 1>(acc[g], dah, dbl, 1u);
-        wgmma<TN, F16, 1, 1>(acc[g], dah, dbh, 1u);
+        wgmma<TN, false, 1, 1>(acc[g], dal, dbh, 1u);
+        wgmma<TN, false, 1, 1>(acc[g], dah, dbl, 1u);
+        wgmma<TN, false, 1, 1>(acc[g], dah, dbh, 1u);
       }
       wgmma_commit();
       wgmma_wait<1>();
@@ -406,8 +406,8 @@ __global__ void __launch_bounds__(NTHR, 1) wgrad_wgmma_kernel(const Args p) {
   }
 }
 
-template <int TN, bool F16>
-int launch_cfg(const Args& a, int splits, cudaStream_t st) {
+template <int TN>
+int launch(const Args& a, int splits, cudaStream_t st) {
   static bool attr_set[64] = {};          // per device: the opt-in is a per-device function attribute
   const int mrows_max = a.Ca < WM ? a.Ca : WM;
   // + 4 KB: the M = 64 descriptor of the upper warpgroup of a 96-channel block reads (and ignores) a few hundred bytes past the
@@ -415,37 +415,32 @@ int launch_cfg(const Args& a, int splits, cudaStream_t st) {
   const size_t smem = (size_t)NS * stage_bytes(mrows_max, TN) + 4096;
   const int dev_ = current_device();
   if (!attr_set[dev_]) {
-    PCB_CUDA(cudaFuncSetAttribute(wgrad_wgmma_kernel<TN, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    PCB_CUDA(cudaFuncSetAttribute(wgrad_wgmma_kernel<TN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   NS * stage_bytes(WM, 128) + 4096));
     attr_set[dev_] = true;
   }
   const int groups = (a.K + GK - 1) / GK;
   dim3 grid((unsigned)(groups * ((a.Ca + WM - 1) / WM) * (a.Cb / TN)), splits);
-  launch_kernel(wgrad_wgmma_kernel<TN, F16>, grid, NTHR, smem, st, a);
+  launch_kernel(wgrad_wgmma_kernel<TN>, grid, NTHR, smem, st, a);
   return check_launch("wgrad_wgmma_kernel");
-}
-
-template <int TN>
-int launch(const Args& a, int splits, cudaStream_t st, int f16) {
-  return f16 ? launch_cfg<TN, true>(a, splits, st) : launch_cfg<TN, false>(a, splits, st);
 }
 
 }  // namespace wg
 
+// Called by pcb_conv_wgrad_split (conv.cu): both operands as bf16 hi/lo planes.
 int launch_wgrad_wgmma(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
                        const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int Ca, int Cb, int rows_per_split, int splits,
-                       float* partial, int transpose_out, int tn, cudaStream_t st, int a_fp16, int b_fp16) {
-  if (a_fp16 != b_fp16) { set_error("wgrad: fp16 and bf16 operand planes cannot be mixed"); return PCB_ERR_ARG; }
+                       float* partial, int transpose_out, int tn, cudaStream_t st) {
   wg::Args a;
   a.Ahi = (const __nv_bfloat16*)Ahi; a.Alo = (const __nv_bfloat16*)Alo; a.lda = lda;
   a.Bhi = (const __nv_bfloat16*)Bhi; a.Blo = (const __nv_bfloat16*)Blo; a.ldb = ldb;
   a.tbl = tbl; a.tbl_stride = tbl_stride; a.K = K; a.n_out = n_out; a.Ca = Ca; a.Cb = Cb; a.rows_per_split = rows_per_split;
   a.partial = partial; a.transpose_out = transpose_out;
   switch (tn) {
-    case 128: return wg::launch<128>(a, splits, st, a_fp16);
-    case 96: return wg::launch<96>(a, splits, st, a_fp16);
-    case 64: return wg::launch<64>(a, splits, st, a_fp16);
-    default: return wg::launch<32>(a, splits, st, a_fp16);
+    case 128: return wg::launch<128>(a, splits, st);
+    case 96: return wg::launch<96>(a, splits, st);
+    case 64: return wg::launch<64>(a, splits, st);
+    default: return wg::launch<32>(a, splits, st);
   }
 }
 

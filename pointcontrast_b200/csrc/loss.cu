@@ -4,7 +4,6 @@
 //   Hardest-contrastive: fused pairwise distance + row min/argmin (replaces the 537 MB broadcast `pdist`
 //   + .min(1), lib/ddp_trainer.py:182-184,215-219).
 // These are < 1 % of a training step; they are exact-fp32 SIMT kernels.
-#include <stdlib.h>
 #include "common.cuh"
 
 using namespace pcb;
@@ -194,7 +193,7 @@ int nce_tc_forward_backward(const float* q, const float* k, int64_t n, int D, fl
 }
 
 // scratch: the tensor-core path needs O(n * D) (partial statistics / gradients); the exact-fp32 SIMT path (feature widths other
-// than 32 / 64, or PCB_NCE_SIMT=1) materialises the n x n logits
+// than 32 / 64) materialises the n x n logits
 extern "C" size_t pcb_nce_ws_bytes(int64_t n) {
   size_t simt = (size_t)n * n * sizeof(float) + (size_t)n * sizeof(float) + 512, tc = nce_tc_ws_bytes(n, 64);
   return simt > tc ? simt : tc;
@@ -205,10 +204,8 @@ extern "C" int pcb_nce_forward_backward(const float* q, const float* k, int64_t 
   PCB_ARG(q && k && loss && dq && dk && ws && n >= 1 && n <= 46000 && D >= 1);
   PCB_ARG(ws_bytes >= pcb_nce_ws_bytes(n) - 512);
   cudaStream_t st = (cudaStream_t)stream;
-  static int force_simt = -1;
-  if (force_simt < 0) { const char* e = getenv("PCB_NCE_SIMT"); force_simt = (e && atoi(e)) ? 1 : 0; }
   ProfScope prof(st, 4);
-  if (!force_simt && nce_tc_supported(n, D)) return nce_tc_forward_backward(q, k, n, D, inv_T, loss, dq, dk, ws, st);
+  if (nce_tc_supported(n, D)) return nce_tc_forward_backward(q, k, n, D, inv_T, loss, dq, dk, ws, st);
   float* L = (float*)ws;
   float* rowloss = L + n * n;
   if (int e = launch_sgemm<false, true>(q, D, k, D, L, (int)n, (int)n, (int)n, D, inv_T, st)) return e;

@@ -22,7 +22,6 @@ int bn_backward_impl(const float* dY, int lddy, const float* X, int ldx, const f
 using namespace pcb;
 
 // ------------------------------------------------------------------------------------------------ per-launch timing
-#include <stdlib.h>
 #include <vector>
 namespace {
 struct ProfRec { cudaEvent_t e0, e1; int kind; };
@@ -38,11 +37,6 @@ cudaEvent_t prof_event() {
 }
 }  // namespace
 namespace pcb {
-bool pdl_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("PCB_PDL"); on = (e && atoi(e) == 0) ? 0 : 1; }      // on by default; PCB_PDL=0 disables
-  return on == 1;
-}
 void prof_begin(cudaStream_t st) {
   if (!g_prof_on) return;
   g_prof_open = prof_event();

@@ -20,7 +20,6 @@ The executor reads the graph from the attribute names (`matches`), so it serves 
 reference's own, unmodified `model/res16unet.py` alike.
 """
 import ctypes
-import os
 
 import torch
 
@@ -29,15 +28,13 @@ from ._lib import PcbUnit, check, lib, ptr, stream
 
 ENABLED = True
 # Both views of a pair batch in ONE pass (see `stack_views`): half the launches, twice the rows per launch on the deep,
-# latency-bound levels.  BatchNorm keeps the reference's per-view statistics through the row-segmented kernels.
-PAIR = os.environ.get("PCB_PAIR", "1") == "1"
+# latency-bound levels.  BatchNorm keeps the reference's per-view statistics through the row-segmented kernels.  Test hook:
+# False runs the two forward calls of the reference (tests/test_gpu_model.py compares the two).
+PAIR = True
 VIEW1_BATCH_OFFSET = 1 << 14      # batch indices of view 1 in a stacked tensor (packed keys hold batch < 65535)
-# Coordinate-manager build on a side stream (0: on the current stream, as the modular `SparseTensor(...)` path always does).
-SIDE_STREAM = os.environ.get("PCB_COORDS_STREAM", "1") == "1"
-# CUDA stream priority of that stream (0 = default, -1 = high).
-SIDE_PRIORITY = int(os.environ.get("PCB_COORDS_PRIORITY", "0"))
-# Cross-check switch: BatchNorm statistics by a separate pass over z instead of the convolution epilogue.
-SEPARATE_STATS = os.environ.get("PCB_SEPARATE_STATS", "0") == "1"
+# Test hook: True takes the BatchNorm statistics by a separate pass over z instead of the convolution's reduction pass (the
+# cross-check of the fused reduce + statistics pass).
+SEPARATE_STATS = False
 # Test hook: a list to which every ReLU unit of a training forward pass appends (rows of view 0, bool [n, C] = the ReLU decision
 # its backward pass will use), in the order the model file calls its ReLUs.  tests/test_gpu_model.py replays these decisions in
 # the fp64 oracle: a pre-activation within rounding distance of zero is a coin flip in ANY finite precision, and one flipped
@@ -53,7 +50,7 @@ _READY = {}       # (data_ptr, version, numel) of a device-resident input -> eve
 def _side_stream(device):
     s = _SIDE.get(device.index)
     if s is None:
-        s = _SIDE[device.index] = torch.cuda.Stream(device=device, priority=SIDE_PRIORITY)
+        s = _SIDE[device.index] = torch.cuda.Stream(device=device)
     return s
 
 
@@ -101,10 +98,6 @@ def prepare_pair(model, feats0, coords0, feats1, coords1, device):
     batch i and none of it is on the critical path."""
     device = torch.device(device)
     p = Prepared()
-    if not SIDE_STREAM:
-        p.sinput, p.n0 = stack_views(feats0, coords0, feats1, coords1, device)
-        p.geom = Geometry(model, p.sinput, p.n0)
-        return p
     with torch.cuda.device(device):
         main = torch.cuda.current_stream()
         side = _side_stream(device)

@@ -389,16 +389,15 @@ class SparseTensor:
 
 
 # ------------------------------------------------------------------------------------------------ convolution
-import os as _os
-
 FORCE_SIMT = False      # tests flip this to run the exact fp32 kernels
 SIMT_OPS = set()        # diagnostics: subset of {"fwd", "dgrad", "wgrad"} forced onto the exact fp32 kernels (modular path)
 # bench.py sets this to a list: every convolution / weight-gradient entry-point call then appends its description here, in
 # issue order -- the same order in which the library (pcb_profile_enable) brackets those calls with CUDA events.
 PROFILE = None
 # Fused executor: activations travel as fp16 hi/lo planes and the forward weight tiles are fp16 (22 mantissa bits per operand instead of
-# bf16 hi/lo's 16): the forward pass is what sets the whole-network gradient error.  0: bf16 everywhere.
-FWD_FP16 = _os.environ.get("PCB_FWD_FP16", "1") == "1"
+# bf16 hi/lo's 16): the forward pass is what sets the whole-network gradient error.  Test hook: False runs bf16 everywhere (the
+# modular path's numerics), the reference side of tests/test_gpu_model.py and profiles/grad_precision_ab.py.
+FWD_FP16 = True
 CONV_FORCE_SIMT, CONV_ACCUMULATE, PLANES_A_FP16, PLANES_B_FP16 = 1, 4, 8, 16
 
 
@@ -663,12 +662,12 @@ class _BatchNormFunction(torch.autograd.Function):
                 invstd = torch.empty_like(mean)
                 wsb = lib.pcb_bn_ws_bytes(n, C)
                 ws = workspace(wsb, x.device)
-                check(lib.pcb_bn_stats(ptr(x), n, C, eps, momentum if momentum is not None else 0.0, ptr(mean), ptr(invstd),
-                                       ptr(running_mean), ptr(running_var), ptr(ws), wsb, stream()))
+                check(lib.pcb_bn_stats_seg(ptr(x), C, n, n, C, eps, momentum if momentum is not None else 0.0, ptr(mean),
+                                           ptr(invstd), ptr(running_mean), ptr(running_var), ptr(ws), wsb, stream()))
             else:
                 mean, invstd = running_mean, torch.rsqrt(running_var + eps)
-            check(lib.pcb_bn_apply(ptr(x), n, C, ptr(mean), ptr(invstd), ptr(gamma.detach()), ptr(beta.detach()), None, 0,
-                                   ptr(y), stream()))
+            check(lib.pcb_bn_apply_seg(ptr(x), C, n, n, C, ptr(mean), ptr(invstd), ptr(gamma.detach()), ptr(beta.detach()), None, C,
+                                       0, ptr(y), C, None, None, 0, None, None, stream()))
         ctx.save_for_backward(x, gamma, mean, invstd)
         ctx.training = training
         return y
@@ -688,8 +687,8 @@ class _BatchNormFunction(torch.autograd.Function):
         with torch.cuda.device(x.device):
             wsb = lib.pcb_bn_ws_bytes(n, C)
             ws = workspace(wsb, x.device)
-            check(lib.pcb_bn_backward(ptr(dy), ptr(x), n, C, ptr(mean), ptr(invstd), ptr(gamma.detach()), ptr(dx), ptr(dgamma),
-                                      ptr(dbeta), ptr(ws), wsb, stream()))
+            check(lib.pcb_bn_backward_seg(ptr(dy), C, ptr(x), C, None, 0, n, n, C, ptr(mean), ptr(invstd), ptr(gamma.detach()), ptr(dx),
+                                          C, ptr(dgamma), ptr(dbeta), 0, None, 0, 0, None, None, 0, ptr(ws), wsb, stream()))
         return dx, dgamma, dbeta, None, None, None, None, None
 
 

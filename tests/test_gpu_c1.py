@@ -96,7 +96,7 @@ def test_direct_epilogue_conv_at_c1_rows(cin, cout):
                                    plan.wg_tbl.shape[1], 27, n, cin, cout, ptr(dW), 0, ptr(wws), wsb, 4, stream()))
     torch.cuda.synchronize()
     assert max_rel_err(dW - 0.125, oconv.kernel.grad) < TOL and rel_err(dW - 0.125, oconv.kernel.grad) < TOL / 10
-    # fp16 hi/lo activation planes x fp16 weight tiles (the fused executor's forward format, PCB_FWD_FP16): 2^-22 products
+    # fp16 hi/lo activation planes x fp16 weight tiles (the fused executor's forward format, me.FWD_FP16): 2^-22 products
     ft16 = torch.zeros_like(ft); dt16 = torch.zeros_like(dt)
     check(lib.pcb_weight_tile(ptr(Wd), 27, cin, cout, ptr(ft16), ptr(dt16), 16, stream()))
     assert torch.equal(dt16, dt)                                   # the data-gradient tiles stay bf16

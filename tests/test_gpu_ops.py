@@ -368,7 +368,7 @@ def test_l2_normalize_matches_torch(n, C):
 @pytest.mark.parametrize("n,D,T", [(2000, 64, 0.4), (300, 32, 0.07)])
 def test_point_nce_tensor_core_and_simt_paths_agree(n, D, T, monkeypatch):
     """The fused tensor-core PointInfoNCE (D = 32 / 64) against the oracle AND against the exact-fp32 SIMT kernels of the same
-    library (`PCB_NCE_SIMT` is read once per process, so the SIMT side is reached through a width the tiling does not cover)."""
+    library (the SIMT side is reached through a width the tiling does not cover)."""
     from pointcontrast_b200 import losses
     g = torch.Generator().manual_seed(n + D)
     F0 = torch.nn.functional.normalize(torch.randn(n, D, generator=g, dtype=torch.float64), dim=1)
@@ -487,32 +487,51 @@ def test_global_pooling_broadcast_and_instance_norm():
     assert max_rel_err(y, refn) < 1e-4
 
 
+def _host_tile_image(w, fp16):
+    """Host restatement of a weight-tile image of the split conv kernel, as int16 words.  w: fp32 [K][Kc][N] (contraction channels x
+    tile columns: [K][Cin][Cout] for the forward roles, [K][Cout][Cin] for the data-gradient roles)."""
+    w = w.contiguous()
+    K, Kc, N = w.shape
+    bn = next(b for b in (128, 96, 64, 32) if N % b == 0)
+    plane = 4 * ((bn // 8) * 128 + 16)
+    k, c, n = np.meshgrid(np.arange(K), np.arange(Kc), np.arange(N), indexing="ij")
+    blob = ((k * (Kc // 32) + c // 32) * (N // bn) + n // bn) * 2 * plane
+    off = blob + (c % 32 // 8) * (plane // 4) + (n % bn // 8) * 128 + (n % 8) * 16 + (c % 8) * 2
+    v, dt = ((w * 1024.0).clamp(-65000.0, 65000.0), torch.float16) if fp16 else (w, torch.bfloat16)
+    hi = v.to(dt)
+    lo = (v - hi.float()).to(dt)
+    img = np.zeros(K * (Kc // 32) * (N // bn) * plane, np.int16)        # 2 * plane bytes per blob; the 16-byte pads stay zero
+    img[off // 2] = hi.view(torch.int16).numpy()
+    img[(off + plane) // 2] = lo.view(torch.int16).numpy()
+    return img
+
+
 @pytest.mark.parametrize("fp16", [False, True])
-def test_batched_weight_tiling_equals_per_convolution_tiling(fp16):
-    """`pcb_weight_tile_batch` (all convolutions of a network in one launch, 16-byte chunk per thread) writes bit for bit the tile images
-    of `pcb_weight_tile` (one convolution, element per thread): forward roles (fp16 of W * 2^10 or bf16) and data-gradient roles (bf16)."""
+def test_weight_tiling_matches_host_layout(fp16):
+    """`pcb_weight_tile` (one convolution) and `pcb_weight_tile_batch` (all convolutions of a network in one launch) write bit for bit the
+    tile images restated on the host: forward roles (fp16 hi/lo of W * 2^10, or bf16 hi/lo) and data-gradient roles (bf16 hi/lo)."""
     import ctypes
     from pointcontrast_b200._lib import PcbTileDesc, check, lib, ptr, stream
     g = torch.Generator().manual_seed(3)
     shapes = [(27, 96, 96), (8, 32, 64), (1, 128, 256), (27, 384, 256), (27, 32, 32)]
-    Ws = [(torch.randn(K, ci, co, generator=g) * (0.3 if i else 1e-3)).cuda() for i, (K, ci, co) in enumerate(shapes)]
+    Ws = [torch.randn(K, ci, co, generator=g) * (0.3 if i else 1e-3) for i, (K, ci, co) in enumerate(shapes)]
+    Wd = [W.cuda() for W in Ws]
     flag = 16 if fp16 else 0
-    ref = []
-    for W, (K, ci, co) in zip(Ws, shapes):
-        f = torch.zeros(lib.pcb_weight_tile_bytes(K, ci, co, 0), dtype=torch.uint8, device="cuda")
-        d = torch.zeros(lib.pcb_weight_tile_bytes(K, ci, co, 1), dtype=torch.uint8, device="cuda")
-        check(lib.pcb_weight_tile(ptr(W), K, ci, co, ptr(f), ptr(d), flag, stream()))
-        ref.append((f, d))
     descs = (PcbTileDesc * len(shapes))()
-    outs, start = [], 0
-    for i, (W, (K, ci, co)) in enumerate(zip(Ws, shapes)):
-        f = torch.zeros_like(ref[i][0]); d = torch.zeros_like(ref[i][1])
-        check(lib.pcb_tile_desc_fill(ctypes.byref(descs[i]), W.data_ptr(), K, ci, co, f.data_ptr(), d.data_ptr(), flag, start))
+    single, batch, start = [], [], 0
+    for i, (W, (K, ci, co)) in enumerate(zip(Wd, shapes)):
+        f, d, fb, db = (torch.zeros(lib.pcb_weight_tile_bytes(K, ci, co, r), dtype=torch.uint8, device="cuda") for r in (0, 1, 0, 1))
+        check(lib.pcb_weight_tile(ptr(W), K, ci, co, ptr(f), ptr(d), flag, stream()))
+        check(lib.pcb_tile_desc_fill(ctypes.byref(descs[i]), ptr(W), K, ci, co, ptr(fb), ptr(db), flag, start))
         start += K * ci * co
-        outs.append((f, d))
+        single.append((f, d))
+        batch.append((fb, db))
     dev = torch.frombuffer(bytearray(bytes(descs)), dtype=torch.uint8).cuda()
     check(lib.pcb_weight_tile_batch(dev.data_ptr(), len(shapes), start, stream()))
     torch.cuda.synchronize()
-    for (f, d), (rf, rd), sh in zip(outs, ref, shapes):
-        assert torch.equal(f, rf), (sh, "forward tiles", int((f != rf).sum()), f.numel(), (f != rf).nonzero()[:8].flatten().tolist())
-        assert torch.equal(d, rd), (sh, "data-gradient tiles", int((d != rd).sum()), d.numel(), (d != rd).nonzero()[:8].flatten().tolist())
+    for W, sh, s, b in zip(Ws, shapes, single, batch):
+        want = (_host_tile_image(W, fp16), _host_tile_image(W.transpose(1, 2), False))
+        for role, ref in zip(("forward", "data-gradient"), want):
+            for entry, out in (("pcb_weight_tile", s), ("pcb_weight_tile_batch", b)):
+                got = out[role != "forward"].cpu().numpy().view(np.int16)
+                assert got.shape == ref.shape and np.array_equal(got, ref), (sh, entry, role, int((got != ref).sum()), ref.size)

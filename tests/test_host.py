@@ -52,6 +52,18 @@ def test_argument_errors_do_not_need_a_gpu():
     assert _lib.lib.pcb_nce_ws_bytes(4096) >= 4096 * 4096 * 4
 
 
+def test_split_weight_gradient_rejects_fp16_planes():
+    """pcb_conv_wgrad_split reads bf16 hi/lo planes only: a PCB_PLANES_* flag is an argument error, checked before the early return for
+    n_out = 0 (which, with PCB_CONV_ACCUMULATE set, makes no CUDA call)."""
+    from pointcontrast_b200 import _lib
+    fake = 256                                   # never dereferenced
+    def wgrad(flags):
+        return _lib.lib.pcb_conv_wgrad_split(fake, fake, 32, fake, fake, 32, fake, 0, 27, 0, 32, 32, fake, 0, fake, 256, flags, None)
+    assert wgrad(4) == 0
+    for flags in (4 | 8, 4 | 16, 4 | 8 | 16):
+        assert wgrad(flags) == 2 and b"bad argument" in _lib.lib.pcb_last_error()
+
+
 def test_offset_tables_match_oracle():
     from pointcontrast_b200 import me
     for ks in ([3, 3, 3], [2, 2, 2], [1, 1, 1]):
