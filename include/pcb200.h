@@ -23,7 +23,10 @@
  *   - every function returns 0 on success, non-zero on failure; pcb_last_error() returns the message
  *     of the last failure on the calling thread.  Nothing throws across this boundary.
  *   - all data pointers are CALLER-OWNED DEVICE memory (16-byte aligned); the library never allocates
- *     device memory.  Workspaces are sized by the *_ws_bytes queries.
+ *     device memory.  Workspaces: an entry point that takes `ws` accepts any ws_bytes >= its *_ws_bytes query for the
+ *     same arguments; with less it returns PCB_ERR_ARG before any CUDA call or launch (a call with nothing to compute,
+ *     e.g. n == 0, may return earlier without looking at ws).  It touches no byte of ws at or beyond the query, and its
+ *     results do not depend on how much larger ws is.
  *   - `stream` is a cudaStream_t passed as void*; every call is asynchronous on it unless stated.
  *   - feature matrices are fp32 row-major [rows, channels]; coordinates int32 [rows, 4] = (batch, x, y, z).
  *   - a kernel map is a dense neighbour table  tbl[K][n_out]  (int32): tbl[k][j] = input row feeding output

@@ -17,7 +17,6 @@ constexpr int VB = 1 << 20;          // |voxel index| < 2^20, as pcb_voxelize
 constexpr int RB = 256;              // blocks of the partial-reduction passes
 constexpr int RT = 256;              // threads per block
 
-inline unsigned blocks_for(int64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
 inline unsigned reduce_blocks(int64_t n) { const unsigned b = blocks_for(n, RT); return b < RB ? (b ? b : 1) : RB; }
 
 // in-block min / max of K lanes per thread (float), thread 0's lanes hold the result
@@ -233,41 +232,57 @@ __global__ void tf_apply_kernel(int32_t* __restrict__ coords, float* __restrict_
   for (int k = 0; k < 3; ++k) feats[3 * i + k] = f[k];
 }
 
-inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
+// ---------------------------------------------------------------- workspace layouts
+
+// per-block partials, then the final (lo[3], hi[3])
+struct BoundsWs { float* part; float* out; };
+BoundsWs bounds_layout(Carve& c) { return {c.take<float>(RB * 6), c.take<float>(6)}; }
+
+// the blur's second buffer (the noise grid is the first)
+float* elastic_layout(Carve& c, int gx, int gy, int gz) { return c.take<float>((int64_t)gx * gy * gz * 3); }
+
+// mins[0..2], mins[4] = the range status: one copy back to the host
+int32_t* affine_layout(Carve& c) { return c.take<int32_t>(5); }
+
+// per-block partials (colour floats, coordinate ints), the reduced colour range (lo[3], hi[3]), coordinate maxima, auto-contrast status
+struct TfWs { float* fpart; int32_t* ipart; float* red; int32_t* cmax; int32_t* status; };
+TfWs tf_layout(Carve& c) { return {c.take<float>(RB * 6), c.take<int32_t>(RB * 3), c.take<float>(6), c.take<int32_t>(3), c.take<int32_t>(1)}; }
 
 }  // namespace
 
-extern "C" size_t pcb_point_bounds_ws_bytes(void) { return align_up(RB * 6 * sizeof(float)) + 256; }
+extern "C" size_t pcb_point_bounds_ws_bytes(void) {
+  return layout_bytes(bounds_layout);
+}
 
 extern "C" int pcb_point_bounds(const float* xyz, int64_t n, float* lo, float* hi, void* ws, size_t ws_bytes, void* stream) {
-  PCB_ARG(n > 0 && xyz && lo && hi && ws && ws_bytes >= pcb_point_bounds_ws_bytes());
+  Carve c{(char*)ws};
+  const BoundsWs w = bounds_layout(c);
+  PCB_ARG(n > 0 && xyz && lo && hi && ws && ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
-  float* part = (float*)ws;
-  float* out = (float*)((char*)ws + align_up(RB * 6 * sizeof(float)));
   const unsigned nb = reduce_blocks(n);
-  bounds_partial_kernel<<<nb, RT, 0, st>>>(xyz, n, part);
+  bounds_partial_kernel<<<nb, RT, 0, st>>>(xyz, n, w.part);
   if (int e = check_launch("bounds_partial_kernel")) return e;
-  bounds_final_kernel<<<1, RT, 0, st>>>(part, (int)nb, out);
+  bounds_final_kernel<<<1, RT, 0, st>>>(w.part, (int)nb, w.out);
   if (int e = check_launch("bounds_final_kernel")) return e;
   float h[6];
-  PCB_CUDA(cudaMemcpyAsync(h, out, sizeof(h), cudaMemcpyDeviceToHost, st));
+  PCB_CUDA(cudaMemcpyAsync(h, w.out, sizeof(h), cudaMemcpyDeviceToHost, st));
   PCB_CUDA(cudaStreamSynchronize(st));
   for (int k = 0; k < 3; ++k) { lo[k] = h[k]; hi[k] = h[3 + k]; }
   return PCB_OK;
 }
 
 extern "C" size_t pcb_elastic_distort_ws_bytes(int gx, int gy, int gz) {
-  const int64_t cells = (int64_t)(gx > 0 ? gx : 1) * (gy > 0 ? gy : 1) * (gz > 0 ? gz : 1);
-  return align_up(cells * 3 * sizeof(float));
+  return layout_bytes(elastic_layout, gx > 0 ? gx : 1, gy > 0 ? gy : 1, gz > 0 ? gz : 1);
 }
 
 extern "C" int pcb_elastic_distort(float* xyz, int64_t n, float* noise, int gx, int gy, int gz, const double* axes, double magnitude, void* ws,
                                    size_t ws_bytes, void* stream) {
   PCB_ARG(n >= 0 && n < (1ll << 31) && gx >= 2 && gy >= 2 && gz >= 2 && (int64_t)gx * gy * gz < (1ll << 29));
-  PCB_ARG(noise && axes && ws && ws_bytes >= pcb_elastic_distort_ws_bytes(gx, gy, gz) && (n == 0 || xyz));
+  Carve c{(char*)ws};
+  float* tmp = elastic_layout(c, gx, gy, gz);
+  PCB_ARG(noise && axes && ws && ws_bytes >= c.used && (n == 0 || xyz));
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t total = (int64_t)gx * gy * gz * 3;
-  float* tmp = (float*)ws;
   float* bufs[2] = {noise, tmp};
   for (int pass = 0; pass < 6; ++pass) {             // two rounds of x, y, z; even count: the result lands back in `noise`
     blur_kernel<<<blocks_for(total, 256), 256, 0, st>>>(bufs[pass & 1], bufs[(pass & 1) ^ 1], gx, gy, gz, pass % 3);
@@ -278,15 +293,18 @@ extern "C" int pcb_elastic_distort(float* xyz, int64_t n, float* noise, int gx, 
   return check_launch("elastic_kernel");
 }
 
-extern "C" size_t pcb_affine_floor_ws_bytes(void) { return 256; }
+extern "C" size_t pcb_affine_floor_ws_bytes(void) {
+  return layout_bytes(affine_layout);
+}
 
 extern "C" int pcb_affine_floor(const float* xyz, int64_t n, const double* T, int32_t* out, int32_t* min_out, void* ws, size_t ws_bytes,
                                 void* stream) {
-  PCB_ARG(n > 0 && n < (1ll << 31) && xyz && T && out && min_out && ws && ws_bytes >= pcb_affine_floor_ws_bytes());
+  Carve c{(char*)ws};
+  int32_t* mins = affine_layout(c);
+  PCB_ARG(n > 0 && n < (1ll << 31) && xyz && T && out && min_out && ws && ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
   Rows3x4 R;
   for (int k = 0; k < 12; ++k) R.m[k] = T[k];
-  int32_t* mins = (int32_t*)ws;
   int32_t* status = mins + 4;
   PCB_CUDA(cudaMemsetAsync(mins, 0x7F, 3 * sizeof(int32_t), st));      // 0x7F7F7F7F: above every in-range index
   PCB_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
@@ -303,37 +321,33 @@ extern "C" int pcb_affine_floor(const float* xyz, int64_t n, const double* T, in
 }
 
 extern "C" size_t pcb_semseg_input_transform_ws_bytes(void) {
-  return align_up(RB * 6 * sizeof(float)) + align_up(RB * 3 * sizeof(int32_t)) + 256;
+  return layout_bytes(tf_layout);
 }
 
 extern "C" int pcb_semseg_input_transform(int32_t* coords, float* feats, int64_t n, int flip_mask, int contrast, double blend,
                                           const double* translation, const double* jitter_noise, double jitter_scale, int normalize, void* ws,
                                           size_t ws_bytes, void* stream) {
-  PCB_ARG(n > 0 && n < (1ll << 31) && (coords || flip_mask == 0) && feats && (flip_mask & ~7) == 0 && ws && ws_bytes >= pcb_semseg_input_transform_ws_bytes());
+  Carve c{(char*)ws};
+  const TfWs w = tf_layout(c);
+  PCB_ARG(n > 0 && n < (1ll << 31) && (coords || flip_mask == 0) && feats && (flip_mask & ~7) == 0 && ws && ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
-  char* p = (char*)ws;
-  float* fpart = (float*)p; p += align_up(RB * 6 * sizeof(float));
-  int32_t* ipart = (int32_t*)p; p += align_up(RB * 3 * sizeof(int32_t));
-  float* red = (float*)p;
-  int32_t* cmax = (int32_t*)(p + 32);
-  int32_t* status = (int32_t*)(p + 64);
   TfArgs a;
   a.flip_mask = flip_mask; a.contrast = contrast != 0; a.translate = translation != nullptr; a.normalize = normalize != 0;
   a.blend = blend; a.jitter_scale = jitter_scale;
   for (int k = 0; k < 3; ++k) a.tr[k] = translation ? translation[k] : 0.0;
   if (flip_mask || a.contrast) {                    // the reductions the flip and the auto-contrast read
-    PCB_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
+    PCB_CUDA(cudaMemsetAsync(w.status, 0, sizeof(int32_t), st));
     const unsigned nb = reduce_blocks(n);
-    tf_partial_kernel<<<nb, RT, 0, st>>>(coords, feats, n, fpart, ipart);
+    tf_partial_kernel<<<nb, RT, 0, st>>>(coords, feats, n, w.fpart, w.ipart);
     if (int e = check_launch("tf_partial_kernel")) return e;
-    tf_final_kernel<<<1, RT, 0, st>>>(fpart, ipart, (int)nb, a.contrast, red, cmax, status);
+    tf_final_kernel<<<1, RT, 0, st>>>(w.fpart, w.ipart, (int)nb, a.contrast, w.red, w.cmax, w.status);
     if (int e = check_launch("tf_final_kernel")) return e;
   }
-  tf_apply_kernel<<<blocks_for(n, 256), 256, 0, st>>>(coords, feats, n, red, cmax, jitter_noise, a);
+  tf_apply_kernel<<<blocks_for(n, 256), 256, 0, st>>>(coords, feats, n, w.red, w.cmax, jitter_noise, a);
   if (int e = check_launch("tf_apply_kernel")) return e;
   if (a.contrast) {
     int32_t h = 0;
-    PCB_CUDA(cudaMemcpyAsync(&h, status, sizeof(h), cudaMemcpyDeviceToHost, st));
+    PCB_CUDA(cudaMemcpyAsync(&h, w.status, sizeof(h), cudaMemcpyDeviceToHost, st));
     PCB_CUDA(cudaStreamSynchronize(st));
     if (h) { set_error("pcb_semseg_input_transform: colour maximum <= 1 (colours must be in [0, 255])"); return PCB_ERR_RANGE; }
   }

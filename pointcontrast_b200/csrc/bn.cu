@@ -358,6 +358,11 @@ __global__ void bn_eval_stats_kernel(const float* __restrict__ running_mean, con
   if (c < C) { mean[c] = running_mean[c]; invstd[c] = 1.0f / sqrtf(running_var[c] + eps); }
 }
 
+// per-chunk partials [chunks][2][C] (at most one chunk more than n rows make: the two segments round up separately), then the
+// backward pass's [2 segments][dbeta | dgamma][C]
+struct BnWs { float* partial; float* sums; };
+BnWs bn_layout(Carve& c, int64_t n, int C) { return {c.take<float>((int64_t)(chunks_of(n, chunk_rows(n)) + 1) * 2 * C), c.take<float>(2 * 2 * C)}; }
+
 inline int colsum_threads(int C) {       // (C/4) * row lanes, <= 256, at least one row lane
   int cv = C / 4;
   int rp = 256 / cv; if (rp < 1) rp = 1;
@@ -367,16 +372,16 @@ inline int colsum_threads(int C) {       // (C/4) * row lanes, <= 256, at least 
 }  // namespace
 
 extern "C" size_t pcb_bn_ws_bytes(int64_t n, int C) {
-  if (n < 1) n = 1;
-  // per-chunk partial sums (two segments round up separately) + [2 segments][2][C] sums
-  return (size_t)(chunks_of(n, chunk_rows(n)) + 2 + 2) * 2 * C * sizeof(float) + 256;
+  return layout_bytes(bn_layout, n < 1 ? 1 : n, C);
 }
 
 // n0: rows [0, n0) and [n0, n) are separate BatchNorm batches (n0 == n: one batch).  mean / invstd: [segments][C].
 extern "C" int pcb_bn_stats_seg(const float* X, int ldx, int64_t n, int64_t n0, int C, float eps, float momentum, float* mean,
                                 float* invstd, float* running_mean, float* running_var, void* ws, size_t ws_bytes, void* stream) {
   PCB_ARG(X && mean && invstd && ws && n >= 1 && n0 >= 1 && n0 <= n && C >= 4 && C % 4 == 0 && C <= 1024 && ldx >= C && ldx % 4 == 0);
-  PCB_ARG(ws_bytes >= pcb_bn_ws_bytes(n, C) - 256);
+  Carve c{(char*)ws};
+  const BnWs w = bn_layout(c, n, C);
+  PCB_ARG(ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
   const int R = chunk_rows(n);
   int chunks, chunks0;
@@ -384,9 +389,9 @@ extern "C" int pcb_bn_stats_seg(const float* X, int ldx, int64_t n, int64_t n0, 
   const int thr = colsum_threads(C);
   const int rp = thr / (C / 4);
   launch_kernel(colstat_kernel<0>, chunks, thr, (size_t)rp * 2 * C * sizeof(float), st, X, ldx, nullptr, 0, nullptr, 0, nullptr, 0, 0, nullptr, 0,
-                n, n0, chunks0, R, C, nullptr, nullptr, (float*)ws);
+                n, n0, chunks0, R, C, nullptr, nullptr, w.partial);
   if (int e = check_launch("colstat_kernel<fwd>")) return e;
-  launch_kernel(bn_finalize_kernel, (C + 7) / 8, 256, 0, st, (const float*)ws, chunks, chunks0, R, n, n0, C, eps, momentum, mean, invstd,
+  launch_kernel(bn_finalize_kernel, (C + 7) / 8, 256, 0, st, (const float*)w.partial, chunks, chunks0, R, n, n0, C, eps, momentum, mean, invstd,
                 running_mean, running_var);
   return check_launch("bn_finalize_kernel");
 }
@@ -430,24 +435,24 @@ int bn_backward_impl(const float* dY, int lddy, const float* X, int ldx, const f
   PCB_ARG(!relu_out || (ldm >= C && ldm % 4 == 0));
   PCB_ARG(!relu_hi || (!relu_out && ldmh >= C && ldmh % 4 == 0));
   PCB_ARG(gout_mode == 0 || (gout && ldg >= C && ldg % 4 == 0));
-  PCB_ARG(ws_bytes >= pcb_bn_ws_bytes(n, C) - 256);
+  Carve c{(char*)ws};
+  const BnWs w = bn_layout(c, n, C);
+  PCB_ARG(ws_bytes >= c.used);
   const int nseg = n0 < n ? 2 : 1;
   const int R = chunk_rows(n);
   int chunks, chunks0;
   chunk_layout(n, n0, R, &chunks, &chunks0);
   const int thr = colsum_threads(C);
   const int rp = thr / (C / 4);
-  float* partial = (float*)ws;
-  float* sums = partial + (size_t)chunks * 2 * C;        // [segments][2][C]: dbeta, dgamma of THIS call (the apply pass needs them)
   launch_kernel(colstat_kernel<1>, chunks, thr, (size_t)rp * 2 * C * sizeof(float), st, dY, lddy, X, ldx, (const __nv_bfloat16*)relu_hi, ldmh,
-                relu_out, ldm, 0, nullptr, 0, n, n0, chunks0, R, C, mean, invstd, partial);
+                relu_out, ldm, 0, nullptr, 0, n, n0, chunks0, R, C, mean, invstd, w.partial);
   if (int e = check_launch("colstat_kernel<bwd>")) return e;
-  launch_kernel(bn_bwd_finalize_kernel, (C + 7) / 8, 256, 0, st, partial, chunks, chunks0, nseg, C, dgamma, dbeta, accumulate_param_grads, sums);
+  launch_kernel(bn_bwd_finalize_kernel, (C + 7) / 8, 256, 0, st, w.partial, chunks, chunks0, nseg, C, dgamma, dbeta, accumulate_param_grads, w.sums);
   if (int e = check_launch("bn_bwd_finalize_kernel")) return e;
   int64_t n4 = n * (C / 4);
   launch_kernel(bn_bwd_apply_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, dY, lddy, X, ldx, relu_out, ldm, (const __nv_bfloat16*)relu_hi, ldmh, n4,
                                                                     C / 4, n0, 1.0f / (float)n0, nseg == 2 ? 1.0f / (float)(n - n0) : 0.f, mean,
-                                                                    invstd, gamma, sums, dX, lddx, gout, ldg, gout_mode,
+                                                                    invstd, gamma, w.sums, dX, lddx, gout, ldg, gout_mode,
                                                                     (__nv_bfloat16*)dXhi, (__nv_bfloat16*)dXlo, lds);
   return check_launch("bn_bwd_apply_kernel");
 }
@@ -463,16 +468,18 @@ int bn_eval_stats_launch(const float* running_mean, const float* running_var, in
 int bn_reduce_stats_launch(const float* P, int nsplit, float* Y, int ldy, int64_t n, int64_t n0, int C, float eps, float momentum,
                            float* mean, float* invstd, float* running_mean, float* running_var, void* ws, size_t ws_bytes, cudaStream_t st) {
   PCB_ARG(P && Y && ws && nsplit >= 1 && n >= 1 && n0 >= 1 && n0 <= n && C % 4 == 0 && C <= 1024 && ldy >= C && ldy % 4 == 0);
-  PCB_ARG(ws_bytes >= pcb_bn_ws_bytes(n, C) - 256);
+  Carve c{(char*)ws};
+  const BnWs w = bn_layout(c, n, C);
+  PCB_ARG(ws_bytes >= c.used);
   const int R = chunk_rows(n);
   int chunks, chunks0;
   chunk_layout(n, n0, R, &chunks, &chunks0);
   const int thr = colsum_threads(C);
   const int rp = thr / (C / 4);
   launch_kernel(colstat_kernel<2>, chunks, thr, (size_t)rp * 2 * C * sizeof(float), st, P, 0, nullptr, 0, nullptr, 0, nullptr, 0, nsplit, Y, ldy,
-                n, n0, chunks0, R, C, nullptr, nullptr, (float*)ws);
+                n, n0, chunks0, R, C, nullptr, nullptr, w.partial);
   if (int e = check_launch("colstat_kernel<reduce+stats>")) return e;
-  launch_kernel(bn_finalize_kernel, (C + 7) / 8, 256, 0, st, (const float*)ws, chunks, chunks0, R, n, n0, C, eps, momentum, mean, invstd,
+  launch_kernel(bn_finalize_kernel, (C + 7) / 8, 256, 0, st, (const float*)w.partial, chunks, chunks0, R, n, n0, C, eps, momentum, mean, invstd,
                 running_mean, running_var);
   return check_launch("bn_finalize_kernel");
 }

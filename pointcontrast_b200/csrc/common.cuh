@@ -21,6 +21,28 @@ inline int check_launch(const char* what) {
 #define PCB_CUDA(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { pcb::set_error("%s: %s", #call, cudaGetErrorString(e_)); return PCB_ERR_CUDA; } } while (0)
 #define PCB_ARG(cond) do { if (!(cond)) { pcb::set_error("bad argument: %s (%s:%d)", #cond, __FILE__, __LINE__); return PCB_ERR_ARG; } } while (0)
 
+inline unsigned blocks_for(int64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
+inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// Workspace layouts.  Each entry point that takes `ws` has ONE layout function that takes its pieces from a Carve in order.  Run on a
+// null base it only counts (the *_ws_bytes query returns `used`); run on the caller's ws it hands out the same pieces, each at a
+// 256-byte aligned offset.  An entry point never touches a byte at or beyond `used`.
+struct Carve {
+  char* base;
+  size_t used = 0;
+  template <class T> T* take(int64_t count) {
+    T* p = base ? reinterpret_cast<T*>(base + used) : nullptr;
+    used += align_up((size_t)count * sizeof(T));
+    return p;
+  }
+};
+// the *_ws_bytes query of a layout function
+template <class Layout, class... Args> size_t layout_bytes(Layout layout, Args... args) {
+  Carve c{nullptr};
+  layout(c, args...);
+  return c.used;
+}
+
 constexpr uint64_t KEY_EMPTY = 0xFFFFFFFFFFFFFFFFull;
 constexpr int COORD_BIAS = 32768;
 

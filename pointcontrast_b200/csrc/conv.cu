@@ -12,6 +12,7 @@
 // parity (tests: 1e-3 relative against the fp64 oracle after 63 layers).  The exact fp32 entry points (pcb_conv_forward /
 // pcb_conv_wgrad) cover the channel counts the tensor-core tiling does not (Cin = 3, odd widths) and are the in-library
 // cross-check of the tensor-core ones.
+#include <algorithm>
 #include <cuda_fp16.h>
 #include "common.cuh"
 
@@ -251,6 +252,15 @@ int wgrad_splits(int K, int64_t n_out, int Ca, int Cb, int tm, int tn) {
   return (int)s;
 }
 
+bool stem_shape(int Ca, int Cb) { return Ca == 3 && Cb == 32; }
+
+// [partials][K][Ca][Cb]: one partial per CTA of the stem kernel (at most 2 x num_sms) or per row split of the generic kernel,
+// enough for whichever of the two the call takes
+float* wgrad_layout(Carve& c, int K, int64_t n_out, int Ca, int Cb) {
+  const int64_t splits = wgrad_splits(K, n_out, Ca, Cb, 0, 0);
+  return c.take<float>((stem_shape(Ca, Cb) ? std::max<int64_t>(2 * num_sms(), splits) : splits) * K * Ca * Cb);
+}
+
 }  // namespace
 
 namespace pcb {
@@ -297,8 +307,7 @@ extern "C" int pcb_gather_sum(const float* X, int ldx, const int32_t* tbl, int64
 }
 
 extern "C" size_t pcb_conv_wgrad_ws_bytes(int K, int64_t n_out, int Ca, int Cb) {
-  if (Ca == 3 && Cb == 32) return (size_t)2 * num_sms() * K * Ca * Cb * sizeof(float) + 256;
-  return (size_t)wgrad_splits(K, n_out, Ca, Cb, 0, 0) * K * Ca * Cb * sizeof(float) + 256;
+  return layout_bytes(wgrad_layout, K, n_out, Ca, Cb);
 }
 
 // Exact fp32 weight gradient (the 3-channel stem layer, widths the tensor-core tiling does not cover, PCB_CONV_FORCE_SIMT cross-checks).
@@ -313,30 +322,29 @@ extern "C" int pcb_conv_wgrad(const float* A, int lda, const float* B, int ldb, 
     if (!(flags & PCB_CONV_ACCUMULATE)) PCB_CUDA(cudaMemsetAsync(dW, 0, nW * sizeof(float), st));
     return PCB_OK;
   }
-  PCB_ARG(A && B && tbl && ws && tbl_stride >= n_out);
+  Carve c{(char*)ws};
+  float* partial = wgrad_layout(c, K, n_out, Ca, Cb);
+  PCB_ARG(A && B && tbl && ws && ws_bytes >= c.used && tbl_stride >= n_out);
   ProfScope prof(st, 1);
-  if (Ca == 3 && Cb == 32 && !transpose_out && !(flags & PCB_CONV_FORCE_SIMT)) {      // the stem layer: dedicated exact-fp32 kernel
-    const int blocks = (int)((size_t)ws_bytes / ((size_t)nW * sizeof(float)));
-    PCB_ARG(blocks >= 1);
-    int nb = blocks < 2 * num_sms() ? blocks : 2 * num_sms();
+  if (stem_shape(Ca, Cb) && !transpose_out && !(flags & PCB_CONV_FORCE_SIMT)) {      // the stem layer: dedicated exact-fp32 kernel
+    int nb = 2 * num_sms();
     int64_t rpb = (n_out + nb - 1) / nb;
     rpb = (rpb + 63) / 64 * 64;
     nb = (int)((n_out + rpb - 1) / rpb);
-    launch_kernel(wgrad_stem_kernel<3>, nb, 256, 0, st, A, lda, B, ldb, tbl, tbl_stride, K, n_out, (int)rpb, (float*)ws);
+    launch_kernel(wgrad_stem_kernel<3>, nb, 256, 0, st, A, lda, B, ldb, tbl, tbl_stride, K, n_out, (int)rpb, partial);
     if (int e = check_launch("wgrad_stem_kernel")) return e;
-    launch_kernel(wgrad_reduce_kernel, (unsigned)((nW + 255) / 256), 256, 0, st, (const float*)ws, nb, nW, dW, (flags & PCB_CONV_ACCUMULATE) ? 1 : 0);
+    launch_kernel(wgrad_reduce_kernel, (unsigned)((nW + 255) / 256), 256, 0, st, (const float*)partial, nb, nW, dW, (flags & PCB_CONV_ACCUMULATE) ? 1 : 0);
     return check_launch("wgrad_reduce_kernel");
   }
   const int splits = wgrad_splits(K, n_out, Ca, Cb, 0, 0);
-  PCB_ARG(ws_bytes >= (size_t)splits * nW * sizeof(float));
   WgradArgs a;
   a.A = A; a.lda = lda; a.B = B; a.ldb = ldb; a.tbl = tbl; a.tbl_stride = tbl_stride; a.K = K; a.n_out = n_out;
-  a.Ca = Ca; a.Cb = Cb; a.partial = (float*)ws; a.transpose_out = transpose_out;
+  a.Ca = Ca; a.Cb = Cb; a.partial = partial; a.transpose_out = transpose_out;
   a.rows_per_split = (int)((n_out + splits - 1) / splits);
   dim3 grid(K, splits);
   wgrad_simt_kernel<<<grid, 256, 0, st>>>(a);
   if (int e = check_launch("wgrad_simt_kernel")) return e;
-  launch_kernel(wgrad_reduce_kernel, (unsigned)((nW + 255) / 256), 256, 0, st, (const float*)ws, splits, nW, dW,
+  launch_kernel(wgrad_reduce_kernel, (unsigned)((nW + 255) / 256), 256, 0, st, (const float*)partial, splits, nW, dW,
                 (flags & PCB_CONV_ACCUMULATE) ? 1 : 0);
   return check_launch("wgrad_reduce_kernel");
 }
@@ -482,6 +490,9 @@ int bn_reduce_stats_launch(const float* P, int nsplit, float* Y, int ldy, int64_
 // over Y) and *bn_done = 1; in direct mode nothing changes and *bn_done = 0 (the caller runs pcb_bn_stats_seg: fusing the column
 // sums into the epilogue is not done: each thread holds scattered fragment rows, the separate pass reads Y once, coalesced).
 struct BnFuse { int64_t n0; float eps, momentum; float* mean; float* invstd; float* running_mean; float* running_var; void* ws; size_t ws_bytes; };
+// the offset-split partial planes [nsplit][n_out][Cout]; none (NULL: the kernel writes Y directly) when the convolution runs unsplit
+float* conv_split_layout(Carve& c, int nsplit, int64_t n_out, int Cout) { return nsplit > 1 ? c.take<float>(nsplit * n_out * Cout) : nullptr; }
+
 int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap,
                             int K, int64_t n_out, int Cin, int Cout, const void* w_tiles, const float* bias, float* Y, int ldy, void* ws,
                             size_t ws_bytes, int flags, cudaStream_t st, const BnFuse* bn, int* bn_done) {
@@ -490,24 +501,26 @@ int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, c
   if (bn_done) *bn_done = 0;
   if (n_out == 0) return PCB_OK;
   PCB_ARG(Xhi && Xlo && tbl && Y && w_tiles && tbl_stride >= n_out);
+  const int nsplit = conv_splits(K, n_out, Cin, Cout);
+  Carve c{(char*)ws};
+  float* partial = conv_split_layout(c, nsplit, n_out, Cout);
+  PCB_ARG(c.used == 0 || (ws && ws_bytes >= c.used));
   ProfScope prof(st, 0);
   int km[PCB_MAX_KERNEL_VOLUME];
   for (int k = 0; k < K; ++k) { km[k] = kmap ? kmap[k] : k; PCB_ARG(km[k] >= 0 && km[k] < PCB_MAX_KERNEL_VOLUME); }
   const int accumulate = (flags & PCB_CONV_ACCUMULATE) ? 1 : 0;
-  const int nsplit = conv_splits(K, n_out, Cin, Cout);
-  if (nsplit > 1) PCB_ARG(ws && ws_bytes >= (size_t)nsplit * n_out * Cout * sizeof(float));
   if (bn) PCB_ARG(!bias && !accumulate && bn->n0 >= 1 && bn->n0 <= n_out && bn_done);
   if (int e = launch_conv_wgmma(Xhi, Xlo, lds, w_tiles, tbl, tbl_stride, km, K, n_out, Cin, Cout, bias, Y, ldy,
-                                nsplit > 1 ? (float*)ws : nullptr, nsplit, pick_tile(Cout), accumulate, st,
+                                partial, nsplit, pick_tile(Cout), accumulate, st,
                                 (flags & PCB_PLANES_A_FP16) ? 1 : 0, (flags & PCB_PLANES_B_FP16) ? 1 : 0)) return e;
   if (nsplit > 1) {
     if (bn) {
       *bn_done = 1;
-      return bn_reduce_stats_launch((const float*)ws, nsplit, Y, ldy, n_out, bn->n0, Cout, bn->eps, bn->momentum, bn->mean, bn->invstd,
+      return bn_reduce_stats_launch(partial, nsplit, Y, ldy, n_out, bn->n0, Cout, bn->eps, bn->momentum, bn->mean, bn->invstd,
                                     bn->running_mean, bn->running_var, bn->ws, bn->ws_bytes, st);
     }
     int64_t n4 = n_out * (Cout / 4);
-    launch_kernel(conv_split_reduce_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, (const float*)ws, nsplit, n_out, Cout, bias, Y, ldy, accumulate);
+    launch_kernel(conv_split_reduce_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, (const float*)partial, nsplit, n_out, Cout, bias, Y, ldy, accumulate);
     return check_launch("conv_split_reduce_kernel");
   }
   return PCB_OK;
@@ -515,9 +528,8 @@ int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, c
 }  // namespace pcb
 
 extern "C" size_t pcb_conv_forward_split_ws_bytes(int K, int64_t n_out, int Cin, int Cout) {
-  if (Cin % 32 || Cout % 32 || n_out <= 0) return 256;
-  int s = conv_splits(K, n_out, Cin, Cout);
-  return s > 1 ? (size_t)s * n_out * Cout * sizeof(float) + 256 : 256;
+  if (Cin % 32 || Cout % 32 || n_out <= 0) return 0;
+  return layout_bytes(conv_split_layout, conv_splits(K, n_out, Cin, Cout), n_out, Cout);
 }
 
 extern "C" int pcb_conv_forward_split(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride,
@@ -543,11 +555,14 @@ int wgrad_split_splits(int K, int64_t n_out, int Ca, int Cb) {
   if (s > 96) s = 96;
   return (int)s;
 }
+
+// [splits][K][Ca][Cb] partial weight gradients
+float* wgrad_split_layout(Carve& c, int splits, int K, int Ca, int Cb) { return c.take<float>((int64_t)splits * K * Ca * Cb); }
 }  // namespace
 
 extern "C" size_t pcb_conv_wgrad_split_ws_bytes(int K, int64_t n_out, int Ca, int Cb) {
-  if (Ca % 32 || Cb % 32 || n_out <= 0) return 256;
-  return (size_t)wgrad_split_splits(K, n_out, Ca, Cb) * K * Ca * Cb * sizeof(float) + 256;
+  if (Ca % 32 || Cb % 32 || n_out <= 0) return 0;
+  return layout_bytes(wgrad_split_layout, wgrad_split_splits(K, n_out, Ca, Cb), K, Ca, Cb);
 }
 
 extern "C" int pcb_conv_wgrad_split(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
@@ -562,15 +577,16 @@ extern "C" int pcb_conv_wgrad_split(const uint16_t* Ahi, const uint16_t* Alo, in
     if (!(flags & PCB_CONV_ACCUMULATE)) PCB_CUDA(cudaMemsetAsync(dW, 0, nW * sizeof(float), st));
     return PCB_OK;
   }
-  PCB_ARG(Ahi && Alo && Bhi && Blo && tbl && ws && tbl_stride >= n_out);
-  ProfScope prof(st, 1);
   const int splits = wgrad_split_splits(K, n_out, Ca, Cb);
-  PCB_ARG(ws_bytes >= (size_t)splits * nW * sizeof(float));
+  Carve c{(char*)ws};
+  float* partial = wgrad_split_layout(c, splits, K, Ca, Cb);
+  PCB_ARG(Ahi && Alo && Bhi && Blo && tbl && ws && ws_bytes >= c.used && tbl_stride >= n_out);
+  ProfScope prof(st, 1);
   int64_t rps = (n_out + splits - 1) / splits;
   rps = (rps + 15) / 16 * 16;
-  if (int e = launch_wgrad_wgmma(Ahi, Alo, lda, Bhi, Blo, ldb, tbl, tbl_stride, K, n_out, Ca, Cb, (int)rps, splits, (float*)ws,
+  if (int e = launch_wgrad_wgmma(Ahi, Alo, lda, Bhi, Blo, ldb, tbl, tbl_stride, K, n_out, Ca, Cb, (int)rps, splits, partial,
                                  transpose_out, pick_tile(Cb), st)) return e;
-  launch_kernel(wgrad_reduce_kernel, (unsigned)((nW + 255) / 256), 256, 0, st, (const float*)ws, splits, nW, dW,
+  launch_kernel(wgrad_reduce_kernel, (unsigned)((nW + 255) / 256), 256, 0, st, (const float*)partial, splits, nW, dW,
                                                                     (flags & PCB_CONV_ACCUMULATE) ? 1 : 0);
   return check_launch("wgrad_reduce_kernel");
 }

@@ -1,9 +1,8 @@
 // Coordinate manager kernels: key packing, hash table, stride (sort + unique), neighbour-table kernel maps.
 // Replaces MinkowskiEngine 0.4.3's CPU CoordsManager (see include/pcb200.h for the reference call sites).
 // Integer-only: results are bit-exact against oracle/me_cpu.py (tests/test_gpu_coords.py).
-#include <cub/cub.cuh>
 #include <stdarg.h>
-#include "common.cuh"
+#include "sort.cuh"
 
 namespace pcb {
 static thread_local char g_err[512] = "";
@@ -80,12 +79,6 @@ __global__ void coarse_key_kernel(const uint64_t* __restrict__ keys, int64_t n, 
   idx[i] = (int32_t)i;
 }
 
-__global__ void head_flag_kernel(const uint64_t* __restrict__ sk, int64_t n, int32_t* __restrict__ flag) {
-  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  flag[i] = (i == 0 || sk[i] != sk[i - 1]) ? 1 : 0;
-}
-
 __global__ void unique_write_kernel(const uint64_t* __restrict__ sk, const int32_t* __restrict__ sidx,
                                     const int32_t* __restrict__ rank, int64_t n, uint64_t* __restrict__ out_keys,
                                     int32_t* __restrict__ parent, int64_t* n_out) {
@@ -124,21 +117,6 @@ __global__ void map_count_kernel(const int32_t* __restrict__ tbl, int64_t n_out,
   if ((threadIdx.x & 31) == 0 && b) atomicAdd(counts + k, (unsigned long long)__popc(b));
 }
 
-inline unsigned blocks_for(int64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
-
-struct StrideWs {
-  uint64_t* ck; uint64_t* sk; int32_t* idx; int32_t* sidx; int32_t* flag; int32_t* rank; int64_t* n_out; void* cub; size_t cub_bytes;
-};
-
-size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
-
-size_t stride_cub_bytes(int64_t n) {
-  size_t a = 0, b = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, a, (uint64_t*)nullptr, (uint64_t*)nullptr, (int32_t*)nullptr, (int32_t*)nullptr, (int)n);
-  cub::DeviceScan::InclusiveSum(nullptr, b, (int32_t*)nullptr, (int32_t*)nullptr, (int)n);
-  return a > b ? a : b;
-}
-
 }  // namespace
 
 extern "C" int pcb_coords_pack(const int32_t* coords, int64_t n, uint64_t* keys, int32_t* status, void* stream) {
@@ -168,8 +146,7 @@ extern "C" int pcb_hash_build(const uint64_t* keys, int64_t n, uint64_t* table_k
 }
 
 extern "C" size_t pcb_coords_stride_ws_bytes(int64_t n) {
-  if (n <= 0) n = 1;
-  return 2 * align_up(n * 8) + 4 * align_up(n * 4) + 256 + align_up(stride_cub_bytes(n)) + 256;
+  return layout_bytes(sort_layout, n < 1 ? 1 : n);
 }
 
 extern "C" int pcb_coords_stride(const uint64_t* keys, int64_t n, int32_t new_ts, uint64_t* out_keys, int32_t* parent,
@@ -177,32 +154,16 @@ extern "C" int pcb_coords_stride(const uint64_t* keys, int64_t n, int32_t new_ts
   PCB_ARG(n >= 0 && n < (1ll << 31) && new_ts >= 1 && n_out);
   *n_out = 0;
   if (n == 0) return PCB_OK;
-  PCB_ARG(keys && out_keys && ws && ws_bytes >= pcb_coords_stride_ws_bytes(n));
+  Carve c{(char*)ws};
+  const SortWs w = sort_layout(c, n);
+  PCB_ARG(keys && out_keys && ws && ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
-  char* p = (char*)ws;
-  StrideWs w;
-  w.ck = (uint64_t*)p; p += align_up(n * 8);
-  w.sk = (uint64_t*)p; p += align_up(n * 8);
-  w.idx = (int32_t*)p; p += align_up(n * 4);
-  w.sidx = (int32_t*)p; p += align_up(n * 4);
-  w.flag = (int32_t*)p; p += align_up(n * 4);
-  w.rank = (int32_t*)p; p += align_up(n * 4);
-  w.n_out = (int64_t*)p; p += 256;
-  w.cub = p; w.cub_bytes = stride_cub_bytes(n);
-  unsigned g = blocks_for(n, 256);
-  coarse_key_kernel<<<g, 256, 0, st>>>(keys, n, new_ts, w.ck, w.idx);
+  coarse_key_kernel<<<blocks_for(n, 256), 256, 0, st>>>(keys, n, new_ts, w.k, w.idx);
   if (int e = check_launch("coarse_key_kernel")) return e;
-  size_t cb = w.cub_bytes;
-  PCB_CUDA(cub::DeviceRadixSort::SortPairs(w.cub, cb, w.ck, w.sk, w.idx, w.sidx, (int)n, 0, 64, st));
-  g_launches.fetch_add(8);
-  head_flag_kernel<<<g, 256, 0, st>>>(w.sk, n, w.flag);
-  if (int e = check_launch("head_flag_kernel")) return e;
-  cb = w.cub_bytes;
-  PCB_CUDA(cub::DeviceScan::InclusiveSum(w.cub, cb, w.flag, w.rank, (int)n, st));
-  g_launches.fetch_add(2);
-  unique_write_kernel<<<g, 256, 0, st>>>(w.sk, w.sidx, w.rank, n, out_keys, parent, w.n_out);
+  if (int e = sort_runs(n, w, 64, st)) return e;      // all 64 bits: the batch index is the top 16
+  unique_write_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, w.sidx, w.rank, n, out_keys, parent, w.count);
   if (int e = check_launch("unique_write_kernel")) return e;
-  PCB_CUDA(cudaMemcpyAsync(n_out, w.n_out, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  PCB_CUDA(cudaMemcpyAsync(n_out, w.count, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
   PCB_CUDA(cudaStreamSynchronize(st));
   return PCB_OK;
 }

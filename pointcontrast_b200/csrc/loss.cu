@@ -175,6 +175,10 @@ __global__ void sgd_kernel(float* __restrict__ p, const float* __restrict__ g, f
   }
 }
 
+// exact-fp32 PointInfoNCE: the n x n logits (turned into the softmax gradient in place), then the per-row losses
+struct NceWs { float* L; float* rowloss; };
+NceWs nce_simt_layout(Carve& c, int64_t n) { return {c.take<float>(n * n), c.take<float>(n)}; }
+
 template <bool TA, bool TB>
 int launch_sgemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K, float alpha,
                  cudaStream_t st) {
@@ -193,21 +197,23 @@ int nce_tc_forward_backward(const float* q, const float* k, int64_t n, int D, fl
 }
 
 // scratch: the tensor-core path needs O(n * D) (partial statistics / gradients); the exact-fp32 SIMT path (feature widths other
-// than 32 / 64) materialises the n x n logits
+// than 32 / 64) materialises the n x n logits.  The query does not know D: it is the larger of the two.
 extern "C" size_t pcb_nce_ws_bytes(int64_t n) {
-  size_t simt = (size_t)n * n * sizeof(float) + (size_t)n * sizeof(float) + 512, tc = nce_tc_ws_bytes(n, 64);
-  return simt > tc ? simt : tc;
+  Carve c{nullptr};
+  nce_simt_layout(c, n);
+  const size_t tc = nce_tc_ws_bytes(n, 64);
+  return c.used > tc ? c.used : tc;
 }
 
 extern "C" int pcb_nce_forward_backward(const float* q, const float* k, int64_t n, int D, float inv_T, float* loss, float* dq,
                                         float* dk, void* ws, size_t ws_bytes, void* stream) {
   PCB_ARG(q && k && loss && dq && dk && ws && n >= 1 && n <= 46000 && D >= 1);
-  PCB_ARG(ws_bytes >= pcb_nce_ws_bytes(n) - 512);
+  PCB_ARG(ws_bytes >= pcb_nce_ws_bytes(n));
   cudaStream_t st = (cudaStream_t)stream;
   ProfScope prof(st, 4);
   if (nce_tc_supported(n, D)) return nce_tc_forward_backward(q, k, n, D, inv_T, loss, dq, dk, ws, st);
-  float* L = (float*)ws;
-  float* rowloss = L + n * n;
+  Carve c{(char*)ws};
+  const auto [L, rowloss] = nce_simt_layout(c, n);
   if (int e = launch_sgemm<false, true>(q, D, k, D, L, (int)n, (int)n, (int)n, D, inv_T, st)) return e;
   nce_softmax_kernel<<<(unsigned)n, 256, 0, st>>>(L, n, inv_T / (float)n, rowloss);
   if (int e = check_launch("nce_softmax_kernel")) return e;
@@ -341,17 +347,22 @@ __global__ void ce_grad_kernel(const float* __restrict__ X, const int64_t* __res
   if (!(t == ignore || t < 0 || t >= C)) g = (expf(X[e] - rowlse[row]) - (c == t ? 1.f : 0.f)) * (scale / stats[1]);
   dX[e] = g;
 }
+// per-row loss and log-sum-exp, then (mean loss, valid-row count)
+struct CeWs { float* rowloss; float* rowlse; float* stats; };
+CeWs ce_layout(Carve& c, int64_t n) { return {c.take<float>(n), c.take<float>(n), c.take<float>(2)}; }
 }  // namespace
 
-extern "C" size_t pcb_ce_ws_bytes(int64_t n) { return (size_t)(2 * n + 4) * sizeof(float) + 256; }
+extern "C" size_t pcb_ce_ws_bytes(int64_t n) {
+  return layout_bytes(ce_layout, n);
+}
 
 extern "C" int pcb_ce_forward_backward(const float* logits, const int64_t* target, int64_t n, int C, int64_t ignore_index, float grad_scale,
                                        float* loss, float* dlogits, void* ws, size_t ws_bytes, void* stream) {
-  PCB_ARG(logits && target && loss && dlogits && ws && n >= 1 && C >= 1 && C <= 1024 && ws_bytes >= pcb_ce_ws_bytes(n) - 256);
+  PCB_ARG(logits && target && loss && dlogits && ws && n >= 1 && C >= 1 && C <= 1024);
+  Carve c{(char*)ws};
+  const auto [rowloss, rowlse, stats] = ce_layout(c, n);
+  PCB_ARG(ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
-  float* rowloss = (float*)ws;
-  float* rowlse = rowloss + n;
-  float* stats = rowlse + n;
   launch_kernel(ce_rows_kernel, (unsigned)((n + 7) / 8), 256, 0, st, logits, target, n, C, ignore_index, rowloss, rowlse);
   if (int e = check_launch("ce_rows_kernel")) return e;
   launch_kernel(ce_mean_kernel, 1, 1024, 0, st, (const float*)rowloss, target, n, C, ignore_index, stats);

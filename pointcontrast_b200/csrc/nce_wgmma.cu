@@ -277,6 +277,13 @@ int launch_nce(const NceArgs& a, int splits, cudaStream_t st) {
   return a.D == 32 ? launch_nce_d<MODE, 32>(a, splits, st) : launch_nce_d<MODE, 64>(a, splits, st);
 }
 
+// [part_ml: ntiles*n*2][diag: n][lse: n][rowloss: n][part_d: ntiles*n*D]  (splits <= ntiles)
+struct NceTcWs { float* part_ml; float* diag; float* lse; float* rowloss; float* part_d; };
+NceTcWs nce_tc_layout(Carve& c, int64_t n, int D) {
+  const int64_t ntiles = (n + YN - 1) / YN;
+  return {c.take<float>(ntiles * n * 2), c.take<float>(n), c.take<float>(n), c.take<float>(n), c.take<float>(ntiles * n * D)};
+}
+
 }  // namespace
 
 namespace pcb {
@@ -284,11 +291,9 @@ namespace pcb {
 bool nce_tc_supported(int64_t n, int D) { return (D == 32 || D == 64) && n >= 1; }
 
 size_t nce_tc_ws_bytes(int64_t n, int D) {
-  const int ntiles = (int)((n + YN - 1) / YN);
-  return ((size_t)ntiles * n * (2 + (size_t)D) + 3 * (size_t)n) * sizeof(float) + 1024;      // splits <= ntiles
+  return layout_bytes(nce_tc_layout, n, D);
 }
 
-// ws: [part_ml: splits*n*2][diag: n][lse: n][rowloss: n][part_d: splits*n*D]
 int nce_tc_forward_backward(const float* q, const float* k, int64_t n, int D, float inv_T, float* loss, float* dq, float* dk, void* ws,
                             cudaStream_t st) {
   const int rowblocks = (int)((n + XM - 1) / XM), ntiles = (int)((n + YN - 1) / YN);
@@ -297,11 +302,8 @@ int nce_tc_forward_backward(const float* q, const float* k, int64_t n, int D, fl
   if (splits > ntiles) splits = ntiles;
   const int tps = (ntiles + splits - 1) / splits;
   splits = (ntiles + tps - 1) / tps;
-  float* part_ml = (float*)ws;
-  float* diag = part_ml + (size_t)splits * n * 2;
-  float* lse = diag + n;
-  float* rowloss = lse + n;
-  float* part_d = rowloss + n;
+  Carve c{(char*)ws};
+  const auto [part_ml, diag, lse, rowloss, part_d] = nce_tc_layout(c, n, D);
   NceArgs a;
   a.X = q; a.Y = k; a.n = n; a.D = D; a.inv_T = inv_T; a.lse = nullptr; a.part_ml = part_ml; a.diag = diag; a.part_d = part_d; a.tiles_per_split = tps;
   if (int e = launch_nce<MODE_LSE>(a, splits, st)) return e;

@@ -15,7 +15,6 @@ using namespace pcb;
 namespace {
 
 constexpr int64_t LIM = 1ll << 31;
-inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
 
 __device__ __forceinline__ float dist2_rn(float ax, float ay, float az, float bx, float by, float bz) {
   const float dx = __fsub_rn(ax, bx), dy = __fsub_rn(ay, by), dz = __fsub_rn(az, bz);
@@ -319,25 +318,28 @@ dim3 gather_grid(int64_t cols, int64_t C, int64_t B) {
   return dim3((unsigned)((cols + G_THREADS - 1) / G_THREADS), (unsigned)((C + G_CH - 1) / G_CH), (unsigned)std::min<int64_t>(B, 65535));
 }
 
-// readers of every source point: off [B*N + 1], svals (reader positions, ascending within a source point), carved from ws
-int csr_build(const int32_t* idx, int64_t B, int64_t N, int64_t L, void* ws, int32_t*& off, int32_t*& svals, cudaStream_t st) {
+// the CSR transpose of B * L readers of B * N source points: sort keys / values before and after the sort, the offsets, CUB storage
+struct CsrWs { uint32_t* keys; uint32_t* skeys; int32_t* vals; int32_t* svals; int32_t* off; void* cub; size_t cub_bytes; };
+CsrWs csr_layout(Carve& c, int64_t B, int64_t N, int64_t L) {
+  const int64_t total = B * L;
+  const size_t cub_bytes = cub_sort_bytes(total);
+  return {c.take<uint32_t>(total), c.take<uint32_t>(total), c.take<int32_t>(total), c.take<int32_t>(total), c.take<int32_t>(B * N + 1),
+          c.take<char>(cub_bytes), cub_bytes};
+}
+
+// readers of every source point: w.off [B*N + 1], w.svals (reader positions, ascending within a source point)
+int csr_build(const int32_t* idx, int64_t B, int64_t N, int64_t L, const CsrWs& w, cudaStream_t st) {
   const int64_t total = B * L, rows = B * N;
-  char* p = (char*)ws;
-  uint32_t* keys = (uint32_t*)p; p += align_up(total * 4);
-  uint32_t* skeys = (uint32_t*)p; p += align_up(total * 4);
-  int32_t* vals = (int32_t*)p; p += align_up(total * 4);
-  svals = (int32_t*)p; p += align_up(total * 4);
-  off = (int32_t*)p; p += align_up((rows + 1) * 4);
-  size_t cb = cub_sort_bytes(total);
+  size_t cb = w.cub_bytes;
   int end_bit = 1;
   while (end_bit < 32 && ((uint64_t)1 << end_bit) <= (uint64_t)rows) ++end_bit;     // keys are <= rows (the sentinel)
   if (total > 0) {
-    csr_key_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(idx, N, L, total, (uint32_t)rows, keys, vals);
+    csr_key_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(idx, N, L, total, (uint32_t)rows, w.keys, w.vals);
     if (int e = check_launch("csr_key_kernel")) return e;
-    PCB_CUDA(cub::DeviceRadixSort::SortPairs(p, cb, keys, skeys, vals, svals, (int)total, 0, end_bit, st));
+    PCB_CUDA(cub::DeviceRadixSort::SortPairs(w.cub, cb, w.keys, w.skeys, w.vals, w.svals, (int)total, 0, end_bit, st));
     g_launches.fetch_add(4);
   }
-  csr_offsets_kernel<<<(unsigned)((rows + 1 + 255) / 256), 256, 0, st>>>(skeys, total, rows, off);
+  csr_offsets_kernel<<<(unsigned)((rows + 1 + 255) / 256), 256, 0, st>>>(w.skeys, total, rows, w.off);
   return check_launch("csr_offsets_kernel");
 }
 
@@ -352,12 +354,11 @@ __global__ void __launch_bounds__(G_THREADS) rows_sum_kernel(const float* __rest
   grad[t] = (float)acc;
 }
 
-int points_grad(const float* g, const int32_t* idx, const float* w, int R, int64_t B, int64_t C, int64_t N, int64_t L, float* grad, void* ws,
-                size_t ws_bytes, cudaStream_t st) {
-  int32_t *off = nullptr, *svals = nullptr;
-  if (int e = csr_build(idx, B, N, L, ws, off, svals, st)) return e;
-  if (R == 1) csr_sum_kernel<1><<<gather_grid(N, C, B), G_THREADS, 0, st>>>(g, w, off, svals, B, C, N, L, grad);
-  else csr_sum_kernel<3><<<gather_grid(N, C, B), G_THREADS, 0, st>>>(g, w, off, svals, B, C, N, L, grad);
+int points_grad(const float* g, const int32_t* idx, const float* w, int R, int64_t B, int64_t C, int64_t N, int64_t L, float* grad,
+                const CsrWs& ws, cudaStream_t st) {
+  if (int e = csr_build(idx, B, N, L, ws, st)) return e;
+  if (R == 1) csr_sum_kernel<1><<<gather_grid(N, C, B), G_THREADS, 0, st>>>(g, w, ws.off, ws.svals, B, C, N, L, grad);
+  else csr_sum_kernel<3><<<gather_grid(N, C, B), G_THREADS, 0, st>>>(g, w, ws.off, ws.svals, B, C, N, L, grad);
   return check_launch("csr_sum_kernel");
 }
 
@@ -451,27 +452,29 @@ extern "C" int pcb_three_interpolate(const float* features, const int32_t* idx, 
 
 extern "C" size_t pcb_points_grad_ws_bytes(int64_t B, int64_t N, int64_t L) {
   if (B < 0 || N < 0 || L < 0 || B * L >= LIM || B * N >= LIM) return 0;
-  const int64_t total = B * L;
-  return 4 * align_up(total * 4) + align_up((B * N + 1) * 4) + align_up(cub_sort_bytes(total)) + 256;
+  return layout_bytes(csr_layout, B, N, L);
 }
 
 extern "C" int pcb_gather_points_grad(const float* grad_out, const int32_t* idx, int64_t B, int64_t C, int64_t N, int64_t L, float* grad_features,
                                       void* ws, size_t ws_bytes, void* stream) {
   PCB_ARG(B >= 0 && C >= 0 && N >= 0 && L >= 0 && B < LIM && C < LIM && N < LIM && L < LIM && B * L < LIM && B * N < LIM);
   if (B == 0 || C == 0 || N == 0) return PCB_OK;
-  PCB_ARG(grad_features && ws && ws_bytes >= pcb_points_grad_ws_bytes(B, N, L) && ((grad_out && idx) || L == 0));
-  return points_grad(grad_out, idx, nullptr, 1, B, C, N, L, grad_features, ws, ws_bytes, (cudaStream_t)stream);
+  Carve c{(char*)ws};
+  const CsrWs w = csr_layout(c, B, N, L);
+  PCB_ARG(grad_features && ws && ws_bytes >= c.used && ((grad_out && idx) || L == 0));
+  return points_grad(grad_out, idx, nullptr, 1, B, C, N, L, grad_features, w, (cudaStream_t)stream);
 }
 
 extern "C" int pcb_gather_rows_grad(const float* grad_out, const int32_t* idx, int64_t L, int64_t C, int64_t M, float* grad_rows, void* ws,
                                     size_t ws_bytes, void* stream) {
   PCB_ARG(L >= 0 && C >= 0 && M >= 0 && L < LIM && C < LIM && M < LIM && M * C < (1ll << 40));
   if (C == 0 || M == 0) return PCB_OK;
-  PCB_ARG(grad_rows && ws && ws_bytes >= pcb_points_grad_ws_bytes(1, M, L) && ((grad_out && idx) || L == 0));
+  Carve c{(char*)ws};
+  const CsrWs w = csr_layout(c, 1, M, L);
+  PCB_ARG(grad_rows && ws && ws_bytes >= c.used && ((grad_out && idx) || L == 0));
   cudaStream_t st = (cudaStream_t)stream;
-  int32_t *off = nullptr, *svals = nullptr;
-  if (int e = csr_build(idx, 1, M, L, ws, off, svals, st)) return e;
-  rows_sum_kernel<<<(unsigned)((M * C + G_THREADS - 1) / G_THREADS), G_THREADS, 0, st>>>(grad_out, off, svals, C, M, grad_rows);
+  if (int e = csr_build(idx, 1, M, L, w, st)) return e;
+  rows_sum_kernel<<<(unsigned)((M * C + G_THREADS - 1) / G_THREADS), G_THREADS, 0, st>>>(grad_out, w.off, w.svals, C, M, grad_rows);
   return check_launch("rows_sum_kernel");
 }
 
@@ -479,6 +482,8 @@ extern "C" int pcb_three_interpolate_grad(const float* grad_out, const int32_t* 
                                           float* grad_features, void* ws, size_t ws_bytes, void* stream) {
   PCB_ARG(B >= 0 && C >= 0 && n >= 0 && m >= 0 && B < LIM && C < LIM && n < LIM && m < LIM && B * n * 3 < LIM && B * m < LIM);
   if (B == 0 || C == 0 || m == 0) return PCB_OK;
-  PCB_ARG(grad_features && ws && ws_bytes >= pcb_points_grad_ws_bytes(B, m, 3 * n) && ((grad_out && idx && weight) || n == 0));
-  return points_grad(grad_out, idx, weight, 3, B, C, m, 3 * n, grad_features, ws, ws_bytes, (cudaStream_t)stream);
+  Carve c{(char*)ws};
+  const CsrWs w = csr_layout(c, B, m, 3 * n);
+  PCB_ARG(grad_features && ws && ws_bytes >= c.used && ((grad_out && idx && weight) || n == 0));
+  return points_grad(grad_out, idx, weight, 3, B, C, m, 3 * n, grad_features, w, (cudaStream_t)stream);
 }

@@ -75,10 +75,9 @@ extern "C" int pcb_profile_read(float* ms, int32_t* kinds, int max_records, int*
 }
 
 namespace {
-inline size_t up256(size_t v) { return (v + 255) / 256 * 256; }
 inline bool tensor_core_shape(int Cin, int Cout) { return Cin % 32 == 0 && Cout % 32 == 0; }
 
-// scratch layout: [convolution scratch (largest of forward / data gradient / weight gradient) | BatchNorm partial sums]
+// convolution scratch: the largest of forward / data gradient / weight gradient
 size_t conv_part_bytes(int K, int64_t n_in, int64_t n_out, int Cin, int Cout) {
   size_t a = pcb_conv_forward_split_ws_bytes(K, n_out, Cin, Cout), b = pcb_conv_forward_split_ws_bytes(K, n_in, Cout, Cin);
   size_t c = tensor_core_shape(Cin, Cout) ? pcb_conv_wgrad_split_ws_bytes(K, n_out > n_in ? n_out : n_in, Cin, Cout)
@@ -87,31 +86,37 @@ size_t conv_part_bytes(int K, int64_t n_in, int64_t n_out, int Cin, int Cout) {
   size_t m = a > b ? a : b;
   if (c > m) m = c;
   if (d > m) m = d;
-  return up256(m);
+  return m;
+}
+
+// [convolution scratch | BatchNorm scratch]
+struct UnitWs { void* conv; size_t conv_bytes; void* bn; size_t bn_bytes; };
+UnitWs unit_layout(Carve& c, int K, int64_t n_in, int64_t n_out, int Cin, int Cout) {
+  const size_t conv = conv_part_bytes(K, n_in, n_out, Cin, Cout), bn = pcb_bn_ws_bytes(n_out, Cout);
+  return {c.take<char>(conv), conv, c.take<char>(bn), bn};
 }
 }  // namespace
 
 extern "C" size_t pcb_unit_ws_bytes(int K, int64_t n_in, int64_t n_out, int Cin, int Cout) {
-  return conv_part_bytes(K, n_in, n_out, Cin, Cout) + up256(pcb_bn_ws_bytes(n_out, Cout));
+  return layout_bytes(unit_layout, K, n_in, n_out, Cin, Cout);
 }
 
 extern "C" int pcb_unit_forward(const pcb_unit* u, void* stream) {
   PCB_ARG(u && u->K >= 1 && u->K <= PCB_MAX_KERNEL_VOLUME && u->n_out >= 1 && u->n_in >= 1 && u->n0 >= 1 && u->n0 <= u->n_out);
   PCB_ARG(u->fwd_tbl && u->z_p && u->out_hi && u->out_lo && u->mean && u->invstd && u->gamma && u->beta && u->ws);
   PCB_ARG(!(u->flags & PCB_UNIT_FP16_FORWARD) || (u->flags & PCB_UNIT_EVAL) || (u->out_bhi && u->out_blo));
-  PCB_ARG(u->ws_bytes >= pcb_unit_ws_bytes(u->K, u->n_in, u->n_out, u->Cin, u->Cout));
+  Carve c{(char*)u->ws};
+  const UnitWs w = unit_layout(c, u->K, u->n_in, u->n_out, u->Cin, u->Cout);
+  PCB_ARG(u->ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t conv_bytes = conv_part_bytes(u->K, u->n_in, u->n_out, u->Cin, u->Cout);
-  unsigned char* bn_ws = (unsigned char*)u->ws + conv_bytes;
-  const size_t bn_bytes = u->ws_bytes - conv_bytes;
   int have_stats = 0;
   const bool f16 = (u->flags & PCB_UNIT_FP16_FORWARD) != 0;      // activations (x, out planes) and forward weight tiles are fp16 hi/lo
   if (tensor_core_shape(u->Cin, u->Cout)) {
     PCB_ARG(u->x_hi && u->x_lo && u->wt_fwd);
-    BnFuse bn{u->n0, u->eps, u->momentum, u->mean, u->invstd, u->running_mean, u->running_var, bn_ws, bn_bytes};
+    BnFuse bn{u->n0, u->eps, u->momentum, u->mean, u->invstd, u->running_mean, u->running_var, w.bn, w.bn_bytes};
     const bool fuse = !(u->flags & (PCB_UNIT_SEPARATE_STATS | PCB_UNIT_EVAL));
     if (int e = conv_forward_split_impl(u->x_hi, u->x_lo, u->x_lds, u->fwd_tbl, u->fwd_stride, u->fwd_kmap, u->K, u->n_out, u->Cin, u->Cout,
-                                        u->wt_fwd, nullptr, u->z_p, u->z_ld, u->ws, conv_bytes, f16 ? (PCB_PLANES_A_FP16 | PCB_PLANES_B_FP16) : 0,
+                                        u->wt_fwd, nullptr, u->z_p, u->z_ld, w.conv, w.conv_bytes, f16 ? (PCB_PLANES_A_FP16 | PCB_PLANES_B_FP16) : 0,
                                         st, fuse ? &bn : nullptr, &have_stats)) return e;
   } else {
     PCB_ARG(u->x_p && u->W);
@@ -124,7 +129,7 @@ extern "C" int pcb_unit_forward(const pcb_unit* u, void* stream) {
     if (int e = bn_eval_stats_launch(u->running_mean, u->running_var, u->Cout, u->eps, u->mean, u->invstd, st)) return e;
   } else if (!have_stats) {
     if (int e = pcb_bn_stats_seg(u->z_p, u->z_ld, u->n_out, u->n0, u->Cout, u->eps, u->momentum, u->mean, u->invstd, u->running_mean,
-                                 u->running_var, bn_ws, bn_bytes, stream)) return e;
+                                 u->running_var, w.bn, w.bn_bytes, stream)) return e;
   }
   return pcb_bn_apply_seg(u->z_p, u->z_ld, u->n_out, u->n0, u->Cout, u->mean, u->invstd, u->gamma, u->beta, u->res_p, u->res_ld,
                           (u->relu ? PCB_BN_RELU : 0) | (f16 ? PCB_PLANES_A_FP16 : 0), u->out_p, u->out_ld, u->out_hi, u->out_lo, u->out_lds,
@@ -134,19 +139,19 @@ extern "C" int pcb_unit_forward(const pcb_unit* u, void* stream) {
 extern "C" int pcb_unit_backward(const pcb_unit* u, void* stream) {
   PCB_ARG(u && u->K >= 1 && u->K <= PCB_MAX_KERNEL_VOLUME && u->n_out >= 1 && u->n_in >= 1 && u->n0 >= 1 && u->n0 <= u->n_out);
   PCB_ARG(u->g_p && u->z_p && u->mean && u->invstd && u->gamma && u->dgamma && u->dbeta && u->dW && u->wg_tbl && u->ws);
-  PCB_ARG(u->ws_bytes >= pcb_unit_ws_bytes(u->K, u->n_in, u->n_out, u->Cin, u->Cout));
+  Carve c{(char*)u->ws};
+  const UnitWs w = unit_layout(c, u->K, u->n_in, u->n_out, u->Cin, u->Cout);
+  PCB_ARG(u->ws_bytes >= c.used);
   const bool tc = tensor_core_shape(u->Cin, u->Cout);
   const bool f16 = (u->flags & PCB_UNIT_FP16_FORWARD) != 0;
   PCB_ARG(tc ? (u->dz_hi && u->dz_lo && u->x_hi && u->x_lo) : (u->dz_p && u->x_p));
   PCB_ARG(tc || u->gin_mode == 0);               // only the 3-channel stem is not tensor-core shaped: its input wants no gradient
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t conv_bytes = conv_part_bytes(u->K, u->n_in, u->n_out, u->Cin, u->Cout);
-  unsigned char* bn_ws = (unsigned char*)u->ws + conv_bytes;
   // 1. g * (out > 0) -> BatchNorm backward -> dz (split planes), residual-gradient fan-out, dgamma / dbeta accumulated
   prof_begin(st);
   if (int e = bn_backward_impl(u->g_p, u->g_ld, u->z_p, u->z_ld, nullptr, 0, u->relu ? u->out_hi : nullptr, u->out_lds, u->n_out, u->n0, u->Cout,
                                u->mean, u->invstd, u->gamma, u->dz_p, u->dz_ld, u->dgamma, u->dbeta, 1, u->gres_p, u->gres_ld, u->gres_mode,
-                               u->dz_hi, u->dz_lo, u->dz_ld, bn_ws, u->ws_bytes - conv_bytes, st)) return e;
+                               u->dz_hi, u->dz_lo, u->dz_ld, w.bn, w.bn_bytes, st)) return e;
   prof_end(st, 3);
   // 2. weight gradient, accumulated into dW (the flat parameter-gradient buffer)
   if (tc) {
@@ -157,18 +162,18 @@ extern "C" int pcb_unit_backward(const pcb_unit* u, void* stream) {
     const uint16_t *Ahi, *Alo, *Bhi, *Blo; int lda, ldb, Ca, Cb, tr; int64_t rows;
     if (u->wg_gather_x) { Ahi = xh; Alo = xl; lda = u->x_lds; Bhi = u->dz_hi; Blo = u->dz_lo; ldb = u->dz_ld; Ca = u->Cin; Cb = u->Cout; tr = 0; rows = u->n_out; }
     else { Ahi = u->dz_hi; Alo = u->dz_lo; lda = u->dz_ld; Bhi = xh; Blo = xl; ldb = u->x_lds; Ca = u->Cout; Cb = u->Cin; tr = 1; rows = u->n_in; }
-    if (int e = pcb_conv_wgrad_split(Ahi, Alo, lda, Bhi, Blo, ldb, u->wg_tbl, u->wg_stride, u->K, rows, Ca, Cb, u->dW, tr, u->ws, conv_bytes,
+    if (int e = pcb_conv_wgrad_split(Ahi, Alo, lda, Bhi, Blo, ldb, u->wg_tbl, u->wg_stride, u->K, rows, Ca, Cb, u->dW, tr, w.conv, w.conv_bytes,
                                      PCB_CONV_ACCUMULATE, stream)) return e;
   } else {
     PCB_ARG(u->wg_gather_x);
-    if (int e = pcb_conv_wgrad(u->x_p, u->x_ld, u->dz_p, u->dz_ld, u->wg_tbl, u->wg_stride, u->K, u->n_out, u->Cin, u->Cout, u->dW, 0, u->ws,
-                               conv_bytes, PCB_CONV_ACCUMULATE, stream)) return e;
+    if (int e = pcb_conv_wgrad(u->x_p, u->x_ld, u->dz_p, u->dz_ld, u->wg_tbl, u->wg_stride, u->K, u->n_out, u->Cin, u->Cout, u->dW, 0, w.conv,
+                               w.conv_bytes, PCB_CONV_ACCUMULATE, stream)) return e;
   }
   // 3. data gradient: the forward kernel on the data-gradient weight tiles and the opposite-offset table
   if (u->gin_mode) {
     PCB_ARG(u->gin_p && u->dg_tbl && u->wt_dg);
     if (int e = pcb_conv_forward_split(u->dz_hi, u->dz_lo, u->dz_ld, u->dg_tbl, u->dg_stride, u->dg_kmap, u->K, u->n_in, u->Cout, u->Cin, u->wt_dg,
-                                       nullptr, u->gin_p, u->gin_ld, u->ws, conv_bytes, u->gin_mode == 2 ? PCB_CONV_ACCUMULATE : 0, stream)) return e;
+                                       nullptr, u->gin_p, u->gin_ld, w.conv, w.conv_bytes, u->gin_mode == 2 ? PCB_CONV_ACCUMULATE : 0, stream)) return e;
   }
   return PCB_OK;
 }

@@ -12,7 +12,7 @@
 #include <algorithm>
 #include <vector>
 #include <cub/cub.cuh>
-#include "common.cuh"
+#include "sort.cuh"
 
 using namespace pcb;
 
@@ -125,9 +125,6 @@ __global__ void radius_kernel(const float* __restrict__ src, int64_t ns, const f
   }
 }
 
-inline unsigned blocks_for(int64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
-inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
-
 size_t sort_scan_bytes(int64_t n) {
   size_t a = 0, b = 0, c = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, a, (uint64_t*)nullptr, (uint64_t*)nullptr, (int32_t*)nullptr, (int32_t*)nullptr, (int)n);
@@ -137,36 +134,25 @@ size_t sort_scan_bytes(int64_t n) {
   return m > c ? m : c;
 }
 
-struct SortWs { uint64_t* k; uint64_t* sk; int32_t* idx; int32_t* sidx; int32_t* flag; int32_t* rank; int64_t* count; int32_t* status; void* cub; size_t cub_bytes; char* end; };
+}  // namespace
 
-SortWs carve(void* ws, int64_t n) {
-  char* p = (char*)ws;
-  SortWs w;
-  w.k = (uint64_t*)p; p += align_up(n * 8);
-  w.sk = (uint64_t*)p; p += align_up(n * 8);
-  w.idx = (int32_t*)p; p += align_up(n * 4);
-  w.sidx = (int32_t*)p; p += align_up(n * 4);
-  w.flag = (int32_t*)p; p += align_up(n * 4);
-  w.rank = (int32_t*)p; p += align_up(n * 4);
-  w.count = (int64_t*)p; p += 256;
-  w.status = (int32_t*)p; p += 256;
-  w.cub = p; w.cub_bytes = sort_scan_bytes(n); p += align_up(w.cub_bytes);
-  w.end = p;
-  return w;
+namespace pcb {
+
+SortWs sort_layout(Carve& c, int64_t n) {
+  const size_t cub_bytes = sort_scan_bytes(n);
+  return {c.take<uint64_t>(n), c.take<uint64_t>(n), c.take<int32_t>(n), c.take<int32_t>(n), c.take<int32_t>(n), c.take<int32_t>(n),
+          c.take<int64_t>(1), c.take<int32_t>(1), c.take<char>(cub_bytes), cub_bytes};
 }
-size_t carve_bytes(int64_t n) { return 2 * align_up(n * 8) + 4 * align_up(n * 4) + 512 + align_up(sort_scan_bytes(n)) + 256; }
 
-// keys w.k / indices w.idx -> stable sort (w.sk / w.sidx); w.k keeps each point's key at its original position
-int sort_keys(int64_t n, SortWs& w, cudaStream_t st) {
+int sort_keys(int64_t n, const SortWs& w, int end_bit, cudaStream_t st) {
   size_t cb = w.cub_bytes;
-  PCB_CUDA(cub::DeviceRadixSort::SortPairs(w.cub, cb, w.k, w.sk, w.idx, w.sidx, (int)n, 0, 63, st));
+  PCB_CUDA(cub::DeviceRadixSort::SortPairs(w.cub, cb, w.k, w.sk, w.idx, w.sidx, (int)n, 0, end_bit, st));
   g_launches.fetch_add(8);
   return PCB_OK;
 }
 
-// stable sort -> head flags -> inclusive scan (rank)
-int sort_runs(int64_t n, SortWs& w, cudaStream_t st) {
-  if (int e = sort_keys(n, w, st)) return e;
+int sort_runs(int64_t n, const SortWs& w, int end_bit, cudaStream_t st) {
+  if (int e = sort_keys(n, w, end_bit, st)) return e;
   head_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, n, w.flag);
   if (int e = check_launch("head_kernel")) return e;
   size_t cb = w.cub_bytes;
@@ -175,16 +161,20 @@ int sort_runs(int64_t n, SortWs& w, cudaStream_t st) {
   return PCB_OK;
 }
 
-int point_keys(const float* xyz, int64_t n, float size, SortWs& w, cudaStream_t st) {
+}  // namespace pcb
+
+namespace {
+
+int point_keys(const float* xyz, int64_t n, float size, const SortWs& w, cudaStream_t st) {
   PCB_CUDA(cudaMemsetAsync(w.status, 0, sizeof(int32_t), st));
   point_key_kernel<<<blocks_for(n, 256), 256, 0, st>>>(xyz, n, size, w.k, w.idx, w.status);
   return check_launch("point_key_kernel");
 }
 
 // keys of the points' cells -> sort_runs
-int sort_cells(const float* xyz, int64_t n, float size, SortWs& w, cudaStream_t st) {
+int sort_cells(const float* xyz, int64_t n, float size, const SortWs& w, cudaStream_t st) {
   if (int e = point_keys(xyz, n, size, w, st)) return e;
-  return sort_runs(n, w, st);
+  return sort_runs(n, w, 63, st);
 }
 
 // Batched voxelisation.  After the stable sort by cell key alone, a run of equal keys lists its points in ascending GLOBAL index, i.e.
@@ -245,18 +235,42 @@ __global__ void voxel_label_write_kernel(const uint64_t* __restrict__ sk, const 
   out_labels[r] = lo == hi ? lo : ignore_label;
 }
 
+// the sort pipeline, then stage[B + 2]: offsets[0..B] and the range status, one copy back to the host
+SortWs scenes_layout(Carve& c, int64_t B, int64_t N, int64_t*& stage) {
+  SortWs w = sort_layout(c, B * N);
+  stage = c.take<int64_t>(B + 2);
+  w.status = (int32_t*)(stage + B + 1);
+  return w;
+}
+
+// the cell sort of the targets, their runs, the hash table of the runs (a power of two >= 2 nd slots), per-source counts / offsets
+struct PairsWs {
+  SortWs s; uint64_t* run_key; int32_t* run_start; int32_t* run_end; int64_t tcap; uint64_t* tk; int32_t* tv; int32_t* cnt; int64_t* off;
+  void* cub; size_t cub_bytes;
+};
+PairsWs pairs_layout(Carve& c, int64_t ns, int64_t nd) {
+  int64_t tcap = 16;
+  while (tcap < 2 * nd) tcap <<= 1;
+  const size_t cub_bytes = sort_scan_bytes(ns);
+  return {sort_layout(c, nd), c.take<uint64_t>(nd), c.take<int32_t>(nd), c.take<int32_t>(nd), tcap, c.take<uint64_t>(tcap),
+          c.take<int32_t>(tcap), c.take<int32_t>(ns), c.take<int64_t>(ns), c.take<char>(cub_bytes), cub_bytes};
+}
+
 }  // namespace
 
-extern "C" size_t pcb_voxelize_ws_bytes(int64_t n) { return carve_bytes(n < 1 ? 1 : n); }
+extern "C" size_t pcb_voxelize_ws_bytes(int64_t n) {
+  return layout_bytes(sort_layout, n < 1 ? 1 : n);
+}
 
 extern "C" int pcb_voxelize(const float* xyz, int64_t n, float voxel_size, int32_t* out_coords, int32_t* sel, int64_t* m_out, void* ws,
                             size_t ws_bytes, void* stream) {
   PCB_ARG(n >= 0 && n < (1ll << 31) && voxel_size > 0.f && m_out);
   *m_out = 0;
   if (n == 0) return PCB_OK;
-  PCB_ARG(xyz && out_coords && sel && ws && ws_bytes >= pcb_voxelize_ws_bytes(n));
+  Carve c{(char*)ws};
+  const SortWs w = sort_layout(c, n);
+  PCB_ARG(xyz && out_coords && sel && ws && ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
-  SortWs w = carve(ws, n);
   if (int e = sort_cells(xyz, n, voxel_size, w, st)) return e;
   voxel_write_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, w.sidx, w.rank, n, out_coords, sel, w.count);
   if (int e = check_launch("voxel_write_kernel")) return e;
@@ -270,21 +284,24 @@ extern "C" int pcb_voxelize(const float* xyz, int64_t n, float voxel_size, int32
 
 extern "C" size_t pcb_voxelize_scenes_ws_bytes(int64_t B, int64_t N) {
   if (B < 1 || N < 1 || B * N >= (1ll << 31)) return 0;
-  return carve_bytes(B * N) + align_up((B + 2) * 8);
+  Carve c{nullptr};
+  int64_t* stage;
+  scenes_layout(c, B, N, stage);
+  return c.used;
 }
 
 extern "C" int pcb_voxelize_scenes(const float* xyz, int64_t B, int64_t N, float voxel_size, int32_t* out_coords, int32_t* inds, int64_t* offsets,
                                    int64_t* offsets_host, void* ws, size_t ws_bytes, void* stream) {
   PCB_ARG(B >= 1 && N >= 1 && B * N < (1ll << 31) && voxel_size > 0.f);
-  PCB_ARG(xyz && out_coords && inds && offsets && offsets_host && ws && ws_bytes >= pcb_voxelize_scenes_ws_bytes(B, N));
+  Carve c{(char*)ws};
+  int64_t* stage;
+  const SortWs w = scenes_layout(c, B, N, stage);
+  PCB_ARG(xyz && out_coords && inds && offsets && offsets_host && ws && ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t n = B * N;
-  SortWs w = carve(ws, n);
-  int64_t* stage = (int64_t*)w.end;                // offsets[0..B], then the range status: one copy back to the host
-  w.status = (int32_t*)(stage + B + 1);
   PCB_CUDA(cudaMemsetAsync(stage + B + 1, 0, sizeof(int64_t), st));
   if (int e = point_keys(xyz, n, voxel_size, w, st)) return e;
-  if (int e = sort_keys(n, w, st)) return e;
+  if (int e = sort_keys(n, w, 63, st)) return e;
   scene_head_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, w.sidx, n, N, w.flag);
   if (int e = check_launch("scene_head_kernel")) return e;
   int64_t* row = (int64_t*)w.sk;                   // the sorted keys are dead after the head flags
@@ -301,20 +318,23 @@ extern "C" int pcb_voxelize_scenes(const float* xyz, int64_t B, int64_t N, float
   return PCB_OK;
 }
 
-extern "C" size_t pcb_voxelize_labels_ws_bytes(int64_t n) { return carve_bytes(n < 1 ? 1 : n); }
+extern "C" size_t pcb_voxelize_labels_ws_bytes(int64_t n) {
+  return layout_bytes(sort_layout, n < 1 ? 1 : n);
+}
 
 extern "C" int pcb_voxelize_labels(const int32_t* coords, const int32_t* labels, int64_t n, int32_t ignore_label, int32_t* out_coords,
                                    int32_t* sel, int32_t* out_labels, int64_t* m_out, void* ws, size_t ws_bytes, void* stream) {
   PCB_ARG(n >= 0 && n < (1ll << 31) && m_out);
   *m_out = 0;
   if (n == 0) return PCB_OK;
-  PCB_ARG(coords && labels && out_coords && sel && out_labels && ws && ws_bytes >= pcb_voxelize_labels_ws_bytes(n));
+  Carve c{(char*)ws};
+  const SortWs w = sort_layout(c, n);
+  PCB_ARG(coords && labels && out_coords && sel && out_labels && ws && ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
-  SortWs w = carve(ws, n);
   PCB_CUDA(cudaMemsetAsync(w.status, 0, sizeof(int32_t), st));
   int_key_kernel<<<blocks_for(n, 256), 256, 0, st>>>(coords, n, w.k, w.idx, w.status);
   if (int e = check_launch("int_key_kernel")) return e;
-  if (int e = sort_runs(n, w, st)) return e;
+  if (int e = sort_runs(n, w, 63, st)) return e;
   voxel_label_write_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, w.sidx, w.rank, labels, n, ignore_label, out_coords, sel, out_labels,
                                                                w.count);
   if (int e = check_launch("voxel_label_write_kernel")) return e;
@@ -327,12 +347,7 @@ extern "C" int pcb_voxelize_labels(const int32_t* coords, const int32_t* labels,
 }
 
 extern "C" size_t pcb_radius_pairs_ws_bytes(int64_t ns, int64_t nd) {
-  if (nd < 1) nd = 1;
-  if (ns < 1) ns = 1;
-  int64_t cap = 16;
-  while (cap < 2 * nd) cap <<= 1;
-  return carve_bytes(nd) + align_up(nd * 8) + 2 * align_up(nd * 4) + align_up(cap * 8) + align_up(cap * 4) + align_up(ns * 4) +
-         align_up(ns * 8) + align_up(sort_scan_bytes(ns)) + 1024;
+  return layout_bytes(pairs_layout, ns < 1 ? 1 : ns, nd < 1 ? 1 : nd);
 }
 
 // pairs == NULL / cap == 0: only counts (*n_pairs = total).  Otherwise writes min(total, cap) pairs (i ascending, j ascending within i).
@@ -341,38 +356,30 @@ extern "C" int pcb_radius_pairs(const float* src, int64_t ns, const float* dst, 
   PCB_ARG(ns >= 0 && nd >= 0 && ns < (1ll << 31) && nd < (1ll << 31) && radius > 0.f && n_pairs);
   *n_pairs = 0;
   if (ns == 0 || nd == 0) return PCB_OK;
-  PCB_ARG(src && dst && ws && ws_bytes >= pcb_radius_pairs_ws_bytes(ns, nd));
+  Carve c{(char*)ws};
+  const PairsWs w = pairs_layout(c, ns, nd);
+  PCB_ARG(src && dst && ws && ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
-  SortWs w = carve(ws, nd);
-  if (int e = sort_cells(dst, nd, radius, w, st)) return e;
-  char* p = w.end;
-  uint64_t* run_key = (uint64_t*)p; p += align_up(nd * 8);
-  int32_t* run_start = (int32_t*)p; p += align_up(nd * 4);
-  int32_t* run_end = (int32_t*)p; p += align_up(nd * 4);
-  int64_t tcap = 16;
-  while (tcap < 2 * nd) tcap <<= 1;
-  uint64_t* tk = (uint64_t*)p; p += align_up(tcap * 8);
-  int32_t* tv = (int32_t*)p; p += align_up(tcap * 4);
-  int32_t* cnt = (int32_t*)p; p += align_up(ns * 4);
-  int64_t* off = (int64_t*)p; p += align_up(ns * 8);
-  void* cub2 = p; size_t cub2_bytes = sort_scan_bytes(ns);
-  run_bounds_kernel<<<blocks_for(nd, 256), 256, 0, st>>>(w.sk, w.rank, nd, run_key, run_start, run_end, w.count);
+  if (int e = sort_cells(dst, nd, radius, w.s, st)) return e;
+  const uint64_t mask = (uint64_t)w.tcap - 1;
+  run_bounds_kernel<<<blocks_for(nd, 256), 256, 0, st>>>(w.s.sk, w.s.rank, nd, w.run_key, w.run_start, w.run_end, w.s.count);
   if (int e = check_launch("run_bounds_kernel")) return e;
-  PCB_CUDA(cudaMemsetAsync(tk, 0xFF, (size_t)tcap * 8, st));
-  run_insert_kernel<<<blocks_for(nd, 256), 256, 0, st>>>(run_key, w.count, tk, tv, (uint64_t)tcap - 1);
+  PCB_CUDA(cudaMemsetAsync(w.tk, 0xFF, (size_t)w.tcap * 8, st));
+  run_insert_kernel<<<blocks_for(nd, 256), 256, 0, st>>>(w.run_key, w.s.count, w.tk, w.tv, mask);
   if (int e = check_launch("run_insert_kernel")) return e;
-  radius_kernel<false><<<blocks_for(ns, 128), 128, 0, st>>>(src, ns, dst, radius, tk, tv, (uint64_t)tcap - 1, run_start, run_end, w.sidx, cnt,
+  radius_kernel<false><<<blocks_for(ns, 128), 128, 0, st>>>(src, ns, dst, radius, w.tk, w.tv, mask, w.run_start, w.run_end, w.s.sidx, w.cnt,
                                                             nullptr, nullptr, 0);
   if (int e = check_launch("radius_kernel<count>")) return e;
-  PCB_CUDA(cub::DeviceScan::ExclusiveSum(cub2, cub2_bytes, cnt, off, (int)ns, st));
+  size_t cb = w.cub_bytes;
+  PCB_CUDA(cub::DeviceScan::ExclusiveSum(w.cub, cb, w.cnt, w.off, (int)ns, st));
   g_launches.fetch_add(2);
   int64_t last_off = 0; int32_t last_cnt = 0;
-  PCB_CUDA(cudaMemcpyAsync(&last_off, off + ns - 1, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-  PCB_CUDA(cudaMemcpyAsync(&last_cnt, cnt + ns - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  PCB_CUDA(cudaMemcpyAsync(&last_off, w.off + ns - 1, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  PCB_CUDA(cudaMemcpyAsync(&last_cnt, w.cnt + ns - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   PCB_CUDA(cudaStreamSynchronize(st));
   *n_pairs = last_off + last_cnt;
   if (!pairs || cap <= 0) return PCB_OK;
-  radius_kernel<true><<<blocks_for(ns, 128), 128, 0, st>>>(src, ns, dst, radius, tk, tv, (uint64_t)tcap - 1, run_start, run_end, w.sidx, cnt, off,
-                                                           pairs, cap);
+  radius_kernel<true><<<blocks_for(ns, 128), 128, 0, st>>>(src, ns, dst, radius, w.tk, w.tv, mask, w.run_start, w.run_end, w.s.sidx, w.cnt,
+                                                           w.off, pairs, cap);
   return check_launch("radius_kernel<fill>");
 }

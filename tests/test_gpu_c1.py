@@ -46,7 +46,7 @@ def test_direct_epilogue_conv_at_c1_rows(cin, cout):
     n = len(coords)
     assert n >= 40000
     # direct mode: no partial-sum workspace is requested for these shapes (conv_splits == 1), both role assignments
-    assert lib.pcb_conv_forward_split_ws_bytes(27, n, cin, cout) == 256 and lib.pcb_conv_forward_split_ws_bytes(27, n, cout, cin) == 256
+    assert lib.pcb_conv_forward_split_ws_bytes(27, n, cin, cout) == 0 and lib.pcb_conv_forward_split_ws_bytes(27, n, cout, cin) == 0
     g = torch.Generator().manual_seed(cin * 3 + cout)
     st = me.SparseTensor(torch.zeros(n, 1, device="cuda"), coords=torch.from_numpy(coords))
     kg = me.KernelGenerator(3, 1, 1, region_type=me.RegionType.HYBRID, axis_types=[me.RegionType.HYPERCUBE] * 3, dimension=3)
