@@ -215,7 +215,9 @@ int pcb_conv_wgrad_split(const uint16_t* Ahi, const uint16_t* Alo, int lda, cons
  *   apply   : Y = [relu]( (X-mean)*invstd*gamma+beta [+ residual] ), as fp32 (Y, may be NULL) and/or split planes (Yhi/Ylo);
  *             flags: PCB_BN_RELU, PCB_PLANES_A_FP16 (Yhi/Ylo are fp16 hi/lo instead of bf16 hi/lo; Ybhi/Yblo, if non-NULL, then
  *             receive the bf16 hi/lo planes as well)
- *   backward: g = dY * (relu_out > 0) if relu_out else dY;   dgamma/dbeta (+)= sum(g*xhat) / sum(g), summed over both segments;
+ *   backward: g = dY * (relu > 0) if relu_hi else dY, where relu_hi is the 16-bit hi plane of the ReLU output (Yhi of the apply
+ *             pass; row stride ldmh in elements) and relu > 0 <=> its sign bit is clear and it is not zero;
+ *             dgamma/dbeta (+)= sum(g*xhat) / sum(g), summed over both segments;
  *             dX = gamma*invstd*(g - mean(g) - xhat*mean(g*xhat));   gout (=|+=) g  (gout_mode 0 none, 1 write, 2 add)
  *             -- gout is the gradient of the residual input of the forward unit; it may alias dY. */
 #define PCB_BN_RELU 1
@@ -225,7 +227,7 @@ int pcb_bn_stats_seg(const float* X, int ldx, int64_t n, int64_t n0, int C, floa
 int pcb_bn_apply_seg(const float* X, int ldx, int64_t n, int64_t n0, int C, const float* mean, const float* invstd,
                      const float* gamma, const float* beta, const float* residual, int ldr, int flags, float* Y, int ldy,
                      uint16_t* Yhi, uint16_t* Ylo, int lds, uint16_t* Ybhi, uint16_t* Yblo, void* stream);
-int pcb_bn_backward_seg(const float* dY, int lddy, const float* X, int ldx, const float* relu_out, int ldm, int64_t n, int64_t n0,
+int pcb_bn_backward_seg(const float* dY, int lddy, const float* X, int ldx, const uint16_t* relu_hi, int ldmh, int64_t n, int64_t n0,
                         int C, const float* mean, const float* invstd, const float* gamma, float* dX, int lddx, float* dgamma,
                         float* dbeta, int accumulate_param_grads, float* gout, int ldg, int gout_mode, uint16_t* dXhi,
                         uint16_t* dXlo, int lds, void* ws, size_t ws_bytes, void* stream);

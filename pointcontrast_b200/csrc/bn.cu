@@ -53,11 +53,12 @@ __global__ void split_rows_kernel(const float* __restrict__ X, int ldx, int64_t 
 
 // partial[chunk][0][C] = sum(a), partial[chunk][1][C] = sum(a*b)    (b == a for the forward statistics)
 // block: (C/4) channel-vectors x RP row lanes; grid: one CTA per chunk of rows.
-// Strides: lda / ldb / ldm (floats).  Mask (backward only): a is zeroed where mask <= 0 (ReLU folded into the BN backward).
+// Strides: lda / ldb (floats), ldm (elements).  Mask (backward only): a is zeroed where the ReLU output is not positive (ReLU folded
+// into the BN backward).
 // Row segments: rows [0, n0) and [n0, n) are two independent BatchNorm batches (the two views of a pair stacked in one
 // matrix); chunks never straddle the boundary: CTAs [0, chunks0) cover segment 0, the rest segment 1.  n0 == n: one segment.
 // mean / invstd are [segments][C].
-// ReLU mask from the bf16 hi plane of the unit's output: out > 0  <=>  hi > 0 (bf16 keeps fp32's exponent range; the only
+// ReLU mask from the 16-bit hi plane of the ReLU output: out > 0  <=>  hi > 0 (bf16 keeps fp32's exponent range; the only
 // difference is an fp32 denormal below 2^-134 rounding to 0).  4 channels = 8 bytes.
 __device__ __forceinline__ void mask4_bf16(const __nv_bfloat16* m, float4& a) {
   const uint2 b = __ldg(reinterpret_cast<const uint2*>(m));
@@ -76,10 +77,10 @@ __device__ __forceinline__ void mask4_bf16(const __nv_bfloat16* m, float4& a) {
 //   MODE 1  backward sums: a = dY (ReLU-masked), partial = { sum(a), sum(a * xhat) }
 template <int MODE>
 __global__ void __launch_bounds__(256) colstat_kernel(const float* __restrict__ A, int lda, const float* __restrict__ Bm, int ldb,
-                                                      const __nv_bfloat16* __restrict__ MaskH, int ldmh, const float* __restrict__ MaskF,
-                                                      int ldmf, int nsplit, float* __restrict__ Y, int ldy, int64_t n, int64_t n0,
-                                                      int chunks0, int R, int C, const float* __restrict__ mean,
-                                                      const float* __restrict__ invstd, float* __restrict__ partial) {
+                                                      const __nv_bfloat16* __restrict__ Mask, int ldm, int nsplit, float* __restrict__ Y,
+                                                      int ldy, int64_t n, int64_t n0, int chunks0, int R, int C,
+                                                      const float* __restrict__ mean, const float* __restrict__ invstd,
+                                                      float* __restrict__ partial) {
   pdl_wait(); pdl_trigger();
   extern __shared__ float sm[];      // [RP][2][C]
   const int cv = C / 4;
@@ -116,11 +117,7 @@ __global__ void __launch_bounds__(256) colstat_kernel(const float* __restrict__ 
       float4 a = load_a(r);
       if (MODE == 2) *reinterpret_cast<float4*>(Y + r * ldy + c4 * 4) = a;
       if (MODE == 1) {
-        if (MaskH) mask4_bf16(MaskH + r * ldmh + c4 * 4, a);
-        else if (MaskF) {
-          const float4 m = __ldg(reinterpret_cast<const float4*>(MaskF + r * ldmf) + c4);
-          a.x = m.x > 0.f ? a.x : 0.f; a.y = m.y > 0.f ? a.y : 0.f; a.z = m.z > 0.f ? a.z : 0.f; a.w = m.w > 0.f ? a.w : 0.f;
-        }
+        if (Mask) mask4_bf16(Mask + r * ldm + c4 * 4, a);
         const float4 x = __ldg(reinterpret_cast<const float4*>(Bm + r * ldb) + c4);
         s1.x += a.x; s1.y += a.y; s1.z += a.z; s1.w += a.w;
         s2.x += a.x * ((x.x - mu.x) * is.x); s2.y += a.y * ((x.y - mu.y) * is.y);
@@ -158,15 +155,10 @@ __global__ void __launch_bounds__(256) colstat_kernel(const float* __restrict__ 
 // is reduced: the kernel is a single memory round trip plus shuffles instead of four dependent passes over the partial rows (it runs 62
 // times per step on a few hundred KB: pure latency).
 constexpr int FIN_PER_LANE = 12;          // 32 x 12 = 384 chunks per segment held in registers; beyond that a plain loop
-__global__ void bn_finalize_kernel(const float* __restrict__ partial, int chunks, int chunks0, int R, int64_t n, int64_t n0, int C, float eps,
-                                   float momentum, float* __restrict__ mean, float* __restrict__ invstd, float* running_mean,
-                                   float* running_var) {
-  pdl_wait(); pdl_trigger();
-  int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (c >= C) return;
-  const int lane = threadIdx.x & 31;
-  const int nseg = n0 < n ? 2 : 1;
-  float v1[2][FIN_PER_LANE], v2[2][FIN_PER_LANE];
+// The prefetch of both finalize kernels: v1 / v2[seg][j] = entries 0 / 1 of channel c in chunk lane + 32 j of segment seg, all loads
+// independent; 0 past the segment's chunks and for seg >= nseg.
+__device__ __forceinline__ void load_partials(const float* partial, int chunks, int chunks0, int nseg, int C, int c, int lane,
+                                              float (&v1)[2][FIN_PER_LANE], float (&v2)[2][FIN_PER_LANE]) {
 #pragma unroll
   for (int seg = 0; seg < 2; ++seg) {
     const float* p = partial + (seg ? (int64_t)chunks0 * 2 * C : 0);
@@ -178,6 +170,18 @@ __global__ void bn_finalize_kernel(const float* __restrict__ partial, int chunks
       v2[seg][j] = k < ch ? __ldg(p + (int64_t)k * 2 * C + C + c) : 0.f;
     }
   }
+}
+
+__global__ void bn_finalize_kernel(const float* __restrict__ partial, int chunks, int chunks0, int R, int64_t n, int64_t n0, int C, float eps,
+                                   float momentum, float* __restrict__ mean, float* __restrict__ invstd, float* running_mean,
+                                   float* running_var) {
+  pdl_wait(); pdl_trigger();
+  int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (c >= C) return;
+  const int lane = threadIdx.x & 31;
+  const int nseg = n0 < n ? 2 : 1;
+  float v1[2][FIN_PER_LANE], v2[2][FIN_PER_LANE];
+  load_partials(partial, chunks, chunks0, nseg, C, c, lane, v1, v2);
 #pragma unroll
   for (int seg = 0; seg < 2; ++seg) {
     if (seg >= nseg) break;
@@ -259,17 +263,7 @@ __global__ void bn_bwd_finalize_kernel(const float* __restrict__ partial, int ch
   const int lane = threadIdx.x & 31;
   // both segments' partials of this lane in registers first (independent loads, one round trip), then the fp64 shuffle reductions
   float v1[2][FIN_PER_LANE], v2[2][FIN_PER_LANE];
-#pragma unroll
-  for (int seg = 0; seg < 2; ++seg) {
-    const float* p = partial + (seg ? (int64_t)chunks0 * 2 * C : 0);
-    const int ch = seg < nseg ? (seg ? chunks - chunks0 : chunks0) : 0;
-#pragma unroll
-    for (int j = 0; j < FIN_PER_LANE; ++j) {
-      const int k = lane + 32 * j;
-      v1[seg][j] = k < ch ? __ldg(p + (int64_t)k * 2 * C + c) : 0.f;
-      v2[seg][j] = k < ch ? __ldg(p + (int64_t)k * 2 * C + C + c) : 0.f;
-    }
-  }
+  load_partials(partial, chunks, chunks0, nseg, C, c, lane, v1, v2);
   float tb = 0.f, tg = 0.f;
 #pragma unroll
   for (int seg = 0; seg < 2; ++seg) {
@@ -295,8 +289,7 @@ __global__ void bn_bwd_finalize_kernel(const float* __restrict__ partial, int ch
 
 // gout_mode: 0 none, 1 write, 2 accumulate -- the (ReLU-masked) incoming gradient, i.e. the gradient of the residual input
 __global__ void bn_bwd_apply_kernel(const float* dY, int lddy, const float* __restrict__ X, int ldx,
-                                    const float* __restrict__ Mask, int ldm, const __nv_bfloat16* __restrict__ MaskH, int ldmh,
-                                    int64_t n4, int cv, int64_t n0, float inv_n0,
+                                    const __nv_bfloat16* __restrict__ Mask, int ldm, int64_t n4, int cv, int64_t n0, float inv_n0,
                                     float inv_n1, const float* __restrict__ mean, const float* __restrict__ invstd,
                                     const float* __restrict__ gamma, const float* __restrict__ sums, float* __restrict__ dX, int lddx,
                                     float* gout, int ldg, int gout_mode, __nv_bfloat16* __restrict__ dXhi,
@@ -307,12 +300,7 @@ __global__ void bn_bwd_apply_kernel(const float* dY, int lddy, const float* __re
   int c4 = (int)(i % cv);
   const int64_t row = i / cv;
   float4 dy = *(reinterpret_cast<const float4*>(dY + row * lddy) + c4);
-  if (Mask) {
-    float4 m = __ldg(reinterpret_cast<const float4*>(Mask + row * ldm) + c4);
-    dy.x = m.x > 0.f ? dy.x : 0.f; dy.y = m.y > 0.f ? dy.y : 0.f; dy.z = m.z > 0.f ? dy.z : 0.f; dy.w = m.w > 0.f ? dy.w : 0.f;
-  } else if (MaskH) {
-    mask4_bf16(MaskH + row * ldmh + c4 * 4, dy);
-  }
+  if (Mask) mask4_bf16(Mask + row * ldm + c4 * 4, dy);
   if (gout_mode) {
     float4* gp = reinterpret_cast<float4*>(gout + row * ldg) + c4;
     float4 gv = dy;
@@ -344,10 +332,15 @@ inline int chunk_rows(int64_t n) {
   return R;
 }
 inline int chunks_of(int64_t rows, int R) { return (int)((rows + R - 1) / R); }
-// chunks0 / chunks of rows [0, n0) / [0, n) cut into R-row chunks that never straddle n0
-inline void chunk_layout(int64_t n, int64_t n0, int R, int* chunks, int* chunks0) {
-  *chunks0 = chunks_of(n0 < n ? n0 : n, R);
-  *chunks = *chunks0 + (n0 < n ? chunks_of(n - n0, R) : 0);
+// A column-statistics launch over rows [0, n) with the segment boundary n0: one CTA per R-row chunk, chunks never straddle n0 (chunks0
+// of them in segment 0); block = (C/4) channel-vectors x row lanes, <= 256 threads and at least one row lane; smem: [lanes][2][C].
+struct Chunks { int R, chunks, chunks0, threads; size_t smem; };
+Chunks chunk_geometry(int64_t n, int64_t n0, int C) {
+  const int R = chunk_rows(n);
+  const int chunks0 = chunks_of(n0 < n ? n0 : n, R);
+  const int cv = C / 4;
+  const int rp = 256 / cv < 1 ? 1 : 256 / cv;
+  return {R, chunks0 + (n0 < n ? chunks_of(n - n0, R) : 0), chunks0, cv * rp, (size_t)rp * 2 * C * sizeof(float)};
 }
 
 // eval-mode BatchNorm: "statistics" = the running ones
@@ -363,10 +356,21 @@ __global__ void bn_eval_stats_kernel(const float* __restrict__ running_mean, con
 struct BnWs { float* partial; float* sums; };
 BnWs bn_layout(Carve& c, int64_t n, int C) { return {c.take<float>((int64_t)(chunks_of(n, chunk_rows(n)) + 1) * 2 * C), c.take<float>(2 * 2 * C)}; }
 
-inline int colsum_threads(int C) {       // (C/4) * row lanes, <= 256, at least one row lane
-  int cv = C / 4;
-  int rp = 256 / cv; if (rp < 1) rp = 1;
-  return cv * rp;
+// Forward statistics: colstat_kernel<MODE> (0: of A; 2: of A = the sum of nsplit planes, also written to Y) -> per-chunk partials
+// -> bn_finalize_kernel -> mean / invstd / running statistics.
+template <int MODE>
+int stats_launch(const float* A, int lda, int nsplit, float* Y, int ldy, int64_t n, int64_t n0, int C, float eps, float momentum,
+                 float* mean, float* invstd, float* running_mean, float* running_var, void* ws, size_t ws_bytes, cudaStream_t st) {
+  Carve c{(char*)ws};
+  const BnWs w = bn_layout(c, n, C);
+  PCB_ARG(ws_bytes >= c.used);
+  const Chunks g = chunk_geometry(n, n0, C);
+  launch_kernel(colstat_kernel<MODE>, g.chunks, g.threads, g.smem, st, A, lda, nullptr, 0, nullptr, 0, nsplit, Y, ldy, n, n0, g.chunks0, g.R, C,
+                nullptr, nullptr, w.partial);
+  if (int e = check_launch(MODE == 2 ? "colstat_kernel<reduce+stats>" : "colstat_kernel<fwd>")) return e;
+  launch_kernel(bn_finalize_kernel, (C + 7) / 8, 256, 0, st, (const float*)w.partial, g.chunks, g.chunks0, g.R, n, n0, C, eps, momentum, mean,
+                invstd, running_mean, running_var);
+  return check_launch("bn_finalize_kernel");
 }
 
 }  // namespace
@@ -379,21 +383,8 @@ extern "C" size_t pcb_bn_ws_bytes(int64_t n, int C) {
 extern "C" int pcb_bn_stats_seg(const float* X, int ldx, int64_t n, int64_t n0, int C, float eps, float momentum, float* mean,
                                 float* invstd, float* running_mean, float* running_var, void* ws, size_t ws_bytes, void* stream) {
   PCB_ARG(X && mean && invstd && ws && n >= 1 && n0 >= 1 && n0 <= n && C >= 4 && C % 4 == 0 && C <= 1024 && ldx >= C && ldx % 4 == 0);
-  Carve c{(char*)ws};
-  const BnWs w = bn_layout(c, n, C);
-  PCB_ARG(ws_bytes >= c.used);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int R = chunk_rows(n);
-  int chunks, chunks0;
-  chunk_layout(n, n0, R, &chunks, &chunks0);
-  const int thr = colsum_threads(C);
-  const int rp = thr / (C / 4);
-  launch_kernel(colstat_kernel<0>, chunks, thr, (size_t)rp * 2 * C * sizeof(float), st, X, ldx, nullptr, 0, nullptr, 0, nullptr, 0, 0, nullptr, 0,
-                n, n0, chunks0, R, C, nullptr, nullptr, w.partial);
-  if (int e = check_launch("colstat_kernel<fwd>")) return e;
-  launch_kernel(bn_finalize_kernel, (C + 7) / 8, 256, 0, st, (const float*)w.partial, chunks, chunks0, R, n, n0, C, eps, momentum, mean, invstd,
-                running_mean, running_var);
-  return check_launch("bn_finalize_kernel");
+  return stats_launch<0>(X, ldx, 0, nullptr, 0, n, n0, C, eps, momentum, mean, invstd, running_mean, running_var, ws, ws_bytes,
+                         (cudaStream_t)stream);
 }
 
 extern "C" int pcb_split_rows(const float* X, int ldx, int64_t n, int C, uint16_t* hi, uint16_t* lo, int lds, int flags, void* stream) {
@@ -422,41 +413,38 @@ extern "C" int pcb_bn_apply_seg(const float* X, int ldx, int64_t n, int64_t n0, 
   return check_launch("bn_apply_kernel");
 }
 
-namespace pcb {
-// mask: the unit's ReLU output as fp32 (relu_out) or as its bf16 hi plane (relu_hi); neither: no ReLU
-int bn_backward_impl(const float* dY, int lddy, const float* X, int ldx, const float* relu_out, int ldm, const uint16_t* relu_hi, int ldmh,
-                     int64_t n, int64_t n0, int C, const float* mean, const float* invstd, const float* gamma, float* dX, int lddx,
-                     float* dgamma, float* dbeta, int accumulate_param_grads, float* gout, int ldg, int gout_mode, uint16_t* dXhi,
-                     uint16_t* dXlo, int lds, void* ws, size_t ws_bytes, cudaStream_t st) {
+// relu_hi: the 16-bit hi plane of the ReLU output (row stride ldmh in elements); NULL: no ReLU
+extern "C" int pcb_bn_backward_seg(const float* dY, int lddy, const float* X, int ldx, const uint16_t* relu_hi, int ldmh, int64_t n,
+                                   int64_t n0, int C, const float* mean, const float* invstd, const float* gamma, float* dX, int lddx,
+                                   float* dgamma, float* dbeta, int accumulate_param_grads, float* gout, int ldg, int gout_mode,
+                                   uint16_t* dXhi, uint16_t* dXlo, int lds, void* ws, size_t ws_bytes, void* stream) {
   PCB_ARG(dY && X && mean && invstd && gamma && (dX || dXhi) && dgamma && dbeta && ws && n >= 1 && C >= 4 && C % 4 == 0 && C <= 1024);
   PCB_ARG(n0 >= 1 && n0 <= n);
   PCB_ARG(lddy >= C && ldx >= C && lddy % 4 == 0 && ldx % 4 == 0 && (!dX || (lddx >= C && lddx % 4 == 0)));
   PCB_ARG(!dXhi || (dXlo && lds >= C && lds % 4 == 0));
-  PCB_ARG(!relu_out || (ldm >= C && ldm % 4 == 0));
-  PCB_ARG(!relu_hi || (!relu_out && ldmh >= C && ldmh % 4 == 0));
+  PCB_ARG(!relu_hi || (ldmh >= C && ldmh % 4 == 0));
   PCB_ARG(gout_mode == 0 || (gout && ldg >= C && ldg % 4 == 0));
   Carve c{(char*)ws};
   const BnWs w = bn_layout(c, n, C);
   PCB_ARG(ws_bytes >= c.used);
+  cudaStream_t st = (cudaStream_t)stream;
   const int nseg = n0 < n ? 2 : 1;
-  const int R = chunk_rows(n);
-  int chunks, chunks0;
-  chunk_layout(n, n0, R, &chunks, &chunks0);
-  const int thr = colsum_threads(C);
-  const int rp = thr / (C / 4);
-  launch_kernel(colstat_kernel<1>, chunks, thr, (size_t)rp * 2 * C * sizeof(float), st, dY, lddy, X, ldx, (const __nv_bfloat16*)relu_hi, ldmh,
-                relu_out, ldm, 0, nullptr, 0, n, n0, chunks0, R, C, mean, invstd, w.partial);
+  const Chunks g = chunk_geometry(n, n0, C);
+  launch_kernel(colstat_kernel<1>, g.chunks, g.threads, g.smem, st, dY, lddy, X, ldx, (const __nv_bfloat16*)relu_hi, ldmh, 0, nullptr, 0, n, n0,
+                g.chunks0, g.R, C, mean, invstd, w.partial);
   if (int e = check_launch("colstat_kernel<bwd>")) return e;
-  launch_kernel(bn_bwd_finalize_kernel, (C + 7) / 8, 256, 0, st, w.partial, chunks, chunks0, nseg, C, dgamma, dbeta, accumulate_param_grads, w.sums);
+  launch_kernel(bn_bwd_finalize_kernel, (C + 7) / 8, 256, 0, st, w.partial, g.chunks, g.chunks0, nseg, C, dgamma, dbeta, accumulate_param_grads,
+                w.sums);
   if (int e = check_launch("bn_bwd_finalize_kernel")) return e;
   int64_t n4 = n * (C / 4);
-  launch_kernel(bn_bwd_apply_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, dY, lddy, X, ldx, relu_out, ldm, (const __nv_bfloat16*)relu_hi, ldmh, n4,
+  launch_kernel(bn_bwd_apply_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, dY, lddy, X, ldx, (const __nv_bfloat16*)relu_hi, ldmh, n4,
                                                                     C / 4, n0, 1.0f / (float)n0, nseg == 2 ? 1.0f / (float)(n - n0) : 0.f, mean,
                                                                     invstd, gamma, w.sums, dX, lddx, gout, ldg, gout_mode,
                                                                     (__nv_bfloat16*)dXhi, (__nv_bfloat16*)dXlo, lds);
   return check_launch("bn_bwd_apply_kernel");
 }
 
+namespace pcb {
 int bn_eval_stats_launch(const float* running_mean, const float* running_var, int C, float eps, float* mean, float* invstd, cudaStream_t st) {
   PCB_ARG(running_mean && running_var && mean && invstd && C >= 1);
   launch_kernel(bn_eval_stats_kernel, (C + 127) / 128, 128, 0, st, running_mean, running_var, C, eps, mean, invstd);
@@ -468,27 +456,6 @@ int bn_eval_stats_launch(const float* running_mean, const float* running_var, in
 int bn_reduce_stats_launch(const float* P, int nsplit, float* Y, int ldy, int64_t n, int64_t n0, int C, float eps, float momentum,
                            float* mean, float* invstd, float* running_mean, float* running_var, void* ws, size_t ws_bytes, cudaStream_t st) {
   PCB_ARG(P && Y && ws && nsplit >= 1 && n >= 1 && n0 >= 1 && n0 <= n && C % 4 == 0 && C <= 1024 && ldy >= C && ldy % 4 == 0);
-  Carve c{(char*)ws};
-  const BnWs w = bn_layout(c, n, C);
-  PCB_ARG(ws_bytes >= c.used);
-  const int R = chunk_rows(n);
-  int chunks, chunks0;
-  chunk_layout(n, n0, R, &chunks, &chunks0);
-  const int thr = colsum_threads(C);
-  const int rp = thr / (C / 4);
-  launch_kernel(colstat_kernel<2>, chunks, thr, (size_t)rp * 2 * C * sizeof(float), st, P, 0, nullptr, 0, nullptr, 0, nullptr, 0, nsplit, Y, ldy,
-                n, n0, chunks0, R, C, nullptr, nullptr, w.partial);
-  if (int e = check_launch("colstat_kernel<reduce+stats>")) return e;
-  launch_kernel(bn_finalize_kernel, (C + 7) / 8, 256, 0, st, (const float*)w.partial, chunks, chunks0, R, n, n0, C, eps, momentum, mean, invstd,
-                running_mean, running_var);
-  return check_launch("bn_finalize_kernel");
+  return stats_launch<2>(P, 0, nsplit, Y, ldy, n, n0, C, eps, momentum, mean, invstd, running_mean, running_var, ws, ws_bytes, st);
 }
 }  // namespace pcb
-
-extern "C" int pcb_bn_backward_seg(const float* dY, int lddy, const float* X, int ldx, const float* relu_out, int ldm, int64_t n,
-                                   int64_t n0, int C, const float* mean, const float* invstd, const float* gamma, float* dX, int lddx,
-                                   float* dgamma, float* dbeta, int accumulate_param_grads, float* gout, int ldg, int gout_mode,
-                                   uint16_t* dXhi, uint16_t* dXlo, int lds, void* ws, size_t ws_bytes, void* stream) {
-  return pcb::bn_backward_impl(dY, lddy, X, ldx, relu_out, ldm, nullptr, 0, n, n0, C, mean, invstd, gamma, dX, lddx, dgamma, dbeta,
-                               accumulate_param_grads, gout, ldg, gout_mode, dXhi, dXlo, lds, ws, ws_bytes, (cudaStream_t)stream);
-}

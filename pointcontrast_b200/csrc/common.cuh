@@ -72,6 +72,31 @@ struct ProfScope {
   ~ProfScope() { prof_end(st, kind); }
 };
 
+// ---- functions one .cu file defines and another calls.  Declared only here, so each definition is checked against its callers.
+// conv.cu: the tensor-core forward / data gradient of pcb_conv_forward_split, without its profile scope.  partials != NULL: the caller
+// runs the reduction of an offset-split launch itself (bias and PCB_CONV_ACCUMULATE are then rejected: that pass applies them);
+// *partials receives the planes P[*nsplit][n_out][Cout] in ws, or NULL when the convolution ran unsplit and wrote Y.
+int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap,
+                            int K, int64_t n_out, int Cin, int Cout, const void* w_tiles, const float* bias, float* Y, int ldy, void* ws,
+                            size_t ws_bytes, int flags, cudaStream_t st, const float** partials, int* nsplit);
+// conv_wgmma.cu: the wgmma kernels behind conv.cu's split-operand entry points
+int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl, int64_t tbl_stride,
+                      const int* kmap, int K, int64_t n_out, int Cin, int Cout, const float* bias, float* Y, int ldy,
+                      float* partial, int nsplit, int bn, int accumulate, cudaStream_t st, int x_fp16, int w_fp16);
+int launch_wgrad_wgmma(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
+                       const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int Ca, int Cb, int rows_per_split, int splits,
+                       float* partial, int transpose_out, int tn, cudaStream_t st);
+int wgrad_group();
+// bn.cu: the statistics passes of pcb_unit_forward -- eval mode, and fused into the reduction of an offset-split convolution
+int bn_eval_stats_launch(const float* running_mean, const float* running_var, int C, float eps, float* mean, float* invstd, cudaStream_t st);
+int bn_reduce_stats_launch(const float* P, int nsplit, float* Y, int ldy, int64_t n, int64_t n0, int C, float eps, float momentum,
+                           float* mean, float* invstd, float* running_mean, float* running_var, void* ws, size_t ws_bytes, cudaStream_t st);
+// nce_wgmma.cu: the tensor-core PointInfoNCE behind pcb_nce_forward_backward (loss.cu)
+bool nce_tc_supported(int64_t n, int D);
+size_t nce_tc_ws_bytes(int64_t n, int D);
+int nce_tc_forward_backward(const float* q, const float* k, int64_t n, int D, float inv_T, float* loss, float* dq, float* dk, void* ws,
+                            cudaStream_t st);
+
 // Programmatic dependent launch: launch_kernel() launches every kernel with programmatic stream serialisation, and every kernel
 // below starts with pdl_wait() -- it blocks until the preceding kernel of the stream has completed and its writes are visible --
 // followed by pdl_trigger(), which lets the NEXT kernel's CTAs be scheduled as soon as all of this kernel's CTAs are running.  The

@@ -263,16 +263,6 @@ float* wgrad_layout(Carve& c, int K, int64_t n_out, int Ca, int Cb) {
 
 }  // namespace
 
-namespace pcb {
-int wgrad_group();
-int launch_wgrad_wgmma(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
-                         const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int Ca, int Cb, int rows_per_split, int splits,
-                         float* partial, int transpose_out, int tn, cudaStream_t st);
-int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl, int64_t tbl_stride,
-                      const int* kmap, int K, int64_t n_out, int Cin, int Cout, const float* bias, float* Y, int ldy,
-                      float* partial, int nsplit, int bn, int accumulate, cudaStream_t st, int x_fp16, int w_fp16);
-}
-
 // Exact fp32 forward / data gradient: the stem kernel for the 3 -> 32 layer, the generic SIMT kernel for every other width.
 extern "C" int pcb_conv_forward(const float* X, int ldx, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap, int K,
                                 int64_t n_out, int Cin, int Cout, const float* W, const float* bias, float* Y, int ldy, void* stream) {
@@ -482,48 +472,37 @@ extern "C" int pcb_weight_tile(const float* W, int K, int Cin, int Cout, void* f
 }
 
 namespace pcb {
-int bn_reduce_stats_launch(const float* P, int nsplit, float* Y, int ldy, int64_t n, int64_t n0, int C, float eps, float momentum,
-                           float* mean, float* invstd, float* running_mean, float* running_var, void* ws, size_t ws_bytes, cudaStream_t st);
-
-// bn != NULL: a BatchNorm follows this convolution (no bias, no accumulate).  When the convolution runs offset-split (small levels)
-// its reduction pass also produces the BatchNorm statistics (one read of the partial planes instead of reduce + a column-sum pass
-// over Y) and *bn_done = 1; in direct mode nothing changes and *bn_done = 0 (the caller runs pcb_bn_stats_seg: fusing the column
-// sums into the epilogue is not done: each thread holds scattered fragment rows, the separate pass reads Y once, coalesced).
-struct BnFuse { int64_t n0; float eps, momentum; float* mean; float* invstd; float* running_mean; float* running_var; void* ws; size_t ws_bytes; };
 // the offset-split partial planes [nsplit][n_out][Cout]; none (NULL: the kernel writes Y directly) when the convolution runs unsplit
 float* conv_split_layout(Carve& c, int nsplit, int64_t n_out, int Cout) { return nsplit > 1 ? c.take<float>(nsplit * n_out * Cout) : nullptr; }
 
 int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap,
                             int K, int64_t n_out, int Cin, int Cout, const void* w_tiles, const float* bias, float* Y, int ldy, void* ws,
-                            size_t ws_bytes, int flags, cudaStream_t st, const BnFuse* bn, int* bn_done) {
+                            size_t ws_bytes, int flags, cudaStream_t st, const float** partials, int* nsplit_out) {
   PCB_ARG(K >= 1 && K <= PCB_MAX_KERNEL_VOLUME && n_out >= 0 && Cin % 32 == 0 && Cout % 32 == 0 && Cin >= 32 && Cout >= 32);
   PCB_ARG(lds >= Cin && lds % 8 == 0 && ldy >= Cout && ldy % 4 == 0);
-  if (bn_done) *bn_done = 0;
+  if (partials) *partials = nullptr;
   if (n_out == 0) return PCB_OK;
   PCB_ARG(Xhi && Xlo && tbl && Y && w_tiles && tbl_stride >= n_out);
   const int nsplit = conv_splits(K, n_out, Cin, Cout);
   Carve c{(char*)ws};
   float* partial = conv_split_layout(c, nsplit, n_out, Cout);
   PCB_ARG(c.used == 0 || (ws && ws_bytes >= c.used));
-  ProfScope prof(st, 0);
   int km[PCB_MAX_KERNEL_VOLUME];
   for (int k = 0; k < K; ++k) { km[k] = kmap ? kmap[k] : k; PCB_ARG(km[k] >= 0 && km[k] < PCB_MAX_KERNEL_VOLUME); }
   const int accumulate = (flags & PCB_CONV_ACCUMULATE) ? 1 : 0;
-  if (bn) PCB_ARG(!bias && !accumulate && bn->n0 >= 1 && bn->n0 <= n_out && bn_done);
+  PCB_ARG(!partials || (nsplit_out && !bias && !accumulate));
   if (int e = launch_conv_wgmma(Xhi, Xlo, lds, w_tiles, tbl, tbl_stride, km, K, n_out, Cin, Cout, bias, Y, ldy,
                                 partial, nsplit, pick_tile(Cout), accumulate, st,
                                 (flags & PCB_PLANES_A_FP16) ? 1 : 0, (flags & PCB_PLANES_B_FP16) ? 1 : 0)) return e;
-  if (nsplit > 1) {
-    if (bn) {
-      *bn_done = 1;
-      return bn_reduce_stats_launch(partial, nsplit, Y, ldy, n_out, bn->n0, Cout, bn->eps, bn->momentum, bn->mean, bn->invstd,
-                                    bn->running_mean, bn->running_var, bn->ws, bn->ws_bytes, st);
-    }
-    int64_t n4 = n_out * (Cout / 4);
-    launch_kernel(conv_split_reduce_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, (const float*)partial, nsplit, n_out, Cout, bias, Y, ldy, accumulate);
-    return check_launch("conv_split_reduce_kernel");
+  if (nsplit == 1) return PCB_OK;
+  if (partials) {
+    *partials = partial;
+    *nsplit_out = nsplit;
+    return PCB_OK;
   }
-  return PCB_OK;
+  int64_t n4 = n_out * (Cout / 4);
+  launch_kernel(conv_split_reduce_kernel, (unsigned)((n4 + 255) / 256), 256, 0, st, (const float*)partial, nsplit, n_out, Cout, bias, Y, ldy, accumulate);
+  return check_launch("conv_split_reduce_kernel");
 }
 }  // namespace pcb
 
@@ -536,8 +515,10 @@ extern "C" int pcb_conv_forward_split(const uint16_t* Xhi, const uint16_t* Xlo, 
                                       const int32_t* kmap, int K, int64_t n_out, int Cin, int Cout, const void* w_tiles,
                                       const float* bias, float* Y, int ldy, void* ws, size_t ws_bytes,
                                       int flags, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  ProfScope prof(st, 0);
   return pcb::conv_forward_split_impl(Xhi, Xlo, lds, tbl, tbl_stride, kmap, K, n_out, Cin, Cout, w_tiles, bias, Y, ldy, ws, ws_bytes, flags,
-                                      (cudaStream_t)stream, nullptr, nullptr);
+                                      st, nullptr, nullptr);
 }
 
 namespace {

@@ -189,13 +189,6 @@ int launch_sgemm(const float* A, int lda, const float* B, int ldb, float* C, int
 
 }  // namespace
 
-namespace pcb {
-bool nce_tc_supported(int64_t n, int D);
-size_t nce_tc_ws_bytes(int64_t n, int D);
-int nce_tc_forward_backward(const float* q, const float* k, int64_t n, int D, float inv_T, float* loss, float* dq, float* dk, void* ws,
-                            cudaStream_t st);
-}
-
 // scratch: the tensor-core path needs O(n * D) (partial statistics / gradients); the exact-fp32 SIMT path (feature widths other
 // than 32 / 64) materialises the n x n logits.  The query does not know D: it is the larger of the two.
 extern "C" size_t pcb_nce_ws_bytes(int64_t n) {

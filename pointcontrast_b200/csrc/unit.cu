@@ -1,23 +1,11 @@
 // Fused "units" of the Res16UNet graph: convolution -> BatchNorm -> (+ residual) -> (ReLU) issued from one C call, and the
 // reverse sweep of the same unit (include/pcb200.h: pcb_unit).  Host-side sequencing only -- the kernels live in
 // conv_wgmma.cu / conv.cu / bn.cu; what this file adds over calling them one by one from the host language:
-//   * the BatchNorm statistics come from the convolution's own epilogue (or from its offset-split reduction pass), so the
-//     separate column-sum pass over z and its launch disappear;
+//   * on small levels the BatchNorm statistics come from the convolution's offset-split reduction pass, so the separate
+//     column-sum pass over z and its launch disappear;
 //   * one boundary crossing per unit instead of three to five.
 // Replaces the per-module call sequence of `model/modules/resnet_block.py:44-60` / `model/res16unet.py:206-268`.
 #include "common.cuh"
-
-namespace pcb {
-struct BnFuse { int64_t n0; float eps, momentum; float* mean; float* invstd; float* running_mean; float* running_var; void* ws; size_t ws_bytes; };
-int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap,
-                            int K, int64_t n_out, int Cin, int Cout, const void* w_tiles, const float* bias, float* Y, int ldy, void* ws,
-                            size_t ws_bytes, int flags, cudaStream_t st, const BnFuse* bn, int* bn_done);
-int bn_eval_stats_launch(const float* running_mean, const float* running_var, int C, float eps, float* mean, float* invstd, cudaStream_t st);
-int bn_backward_impl(const float* dY, int lddy, const float* X, int ldx, const float* relu_out, int ldm, const uint16_t* relu_hi, int ldmh,
-                     int64_t n, int64_t n0, int C, const float* mean, const float* invstd, const float* gamma, float* dX, int lddx,
-                     float* dgamma, float* dbeta, int accumulate_param_grads, float* gout, int ldg, int gout_mode, uint16_t* dXhi,
-                     uint16_t* dXlo, int lds, void* ws, size_t ws_bytes, cudaStream_t st);
-}
 
 using namespace pcb;
 
@@ -109,15 +97,23 @@ extern "C" int pcb_unit_forward(const pcb_unit* u, void* stream) {
   const UnitWs w = unit_layout(c, u->K, u->n_in, u->n_out, u->Cin, u->Cout);
   PCB_ARG(u->ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
-  int have_stats = 0;
   const bool f16 = (u->flags & PCB_UNIT_FP16_FORWARD) != 0;      // activations (x, out planes) and forward weight tiles are fp16 hi/lo
+  // An offset-split convolution (small levels) leaves its partial planes to one pass that sums them into z and takes the BatchNorm
+  // statistics: one read of the planes instead of a reduction plus a column-sum pass over z.  Unsplit, the statistics are a separate
+  // pass (in the epilogue each thread holds scattered fragment rows; the separate pass reads z once, coalesced).
+  const float* partials = nullptr;
+  int nsplit = 0;
   if (tensor_core_shape(u->Cin, u->Cout)) {
     PCB_ARG(u->x_hi && u->x_lo && u->wt_fwd);
-    BnFuse bn{u->n0, u->eps, u->momentum, u->mean, u->invstd, u->running_mean, u->running_var, w.bn, w.bn_bytes};
     const bool fuse = !(u->flags & (PCB_UNIT_SEPARATE_STATS | PCB_UNIT_EVAL));
+    ProfScope prof(st, 0);                   // the convolution, and the reduction + statistics pass when it has one
     if (int e = conv_forward_split_impl(u->x_hi, u->x_lo, u->x_lds, u->fwd_tbl, u->fwd_stride, u->fwd_kmap, u->K, u->n_out, u->Cin, u->Cout,
                                         u->wt_fwd, nullptr, u->z_p, u->z_ld, w.conv, w.conv_bytes, f16 ? (PCB_PLANES_A_FP16 | PCB_PLANES_B_FP16) : 0,
-                                        st, fuse ? &bn : nullptr, &have_stats)) return e;
+                                        st, fuse ? &partials : nullptr, &nsplit)) return e;
+    if (partials) {
+      if (int e = bn_reduce_stats_launch(partials, nsplit, u->z_p, u->z_ld, u->n_out, u->n0, u->Cout, u->eps, u->momentum, u->mean, u->invstd,
+                                         u->running_mean, u->running_var, w.bn, w.bn_bytes, st)) return e;
+    }
   } else {
     PCB_ARG(u->x_p && u->W);
     if (int e = pcb_conv_forward(u->x_p, u->x_ld, u->fwd_tbl, u->fwd_stride, u->fwd_kmap, u->K, u->n_out, u->Cin, u->Cout, u->W,
@@ -127,7 +123,7 @@ extern "C" int pcb_unit_forward(const pcb_unit* u, void* stream) {
   if (u->flags & PCB_UNIT_EVAL) {            // eval-mode BatchNorm (`downstream/semseg/lib/test.py:95-117`): normalise with the running statistics
     PCB_ARG(u->n0 == u->n_out && u->running_mean && u->running_var);
     if (int e = bn_eval_stats_launch(u->running_mean, u->running_var, u->Cout, u->eps, u->mean, u->invstd, st)) return e;
-  } else if (!have_stats) {
+  } else if (!partials) {
     if (int e = pcb_bn_stats_seg(u->z_p, u->z_ld, u->n_out, u->n0, u->Cout, u->eps, u->momentum, u->mean, u->invstd, u->running_mean,
                                  u->running_var, w.bn, w.bn_bytes, stream)) return e;
   }
@@ -149,9 +145,9 @@ extern "C" int pcb_unit_backward(const pcb_unit* u, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   // 1. g * (out > 0) -> BatchNorm backward -> dz (split planes), residual-gradient fan-out, dgamma / dbeta accumulated
   prof_begin(st);
-  if (int e = bn_backward_impl(u->g_p, u->g_ld, u->z_p, u->z_ld, nullptr, 0, u->relu ? u->out_hi : nullptr, u->out_lds, u->n_out, u->n0, u->Cout,
-                               u->mean, u->invstd, u->gamma, u->dz_p, u->dz_ld, u->dgamma, u->dbeta, 1, u->gres_p, u->gres_ld, u->gres_mode,
-                               u->dz_hi, u->dz_lo, u->dz_ld, w.bn, w.bn_bytes, st)) return e;
+  if (int e = pcb_bn_backward_seg(u->g_p, u->g_ld, u->z_p, u->z_ld, u->relu ? u->out_hi : nullptr, u->out_lds, u->n_out, u->n0, u->Cout,
+                                  u->mean, u->invstd, u->gamma, u->dz_p, u->dz_ld, u->dgamma, u->dbeta, 1, u->gres_p, u->gres_ld, u->gres_mode,
+                                  u->dz_hi, u->dz_lo, u->dz_ld, w.bn, w.bn_bytes, stream)) return e;
   prof_end(st, 3);
   // 2. weight gradient, accumulated into dW (the flat parameter-gradient buffer)
   if (tc) {

@@ -296,10 +296,11 @@ def test_split_operand_conv_forward_matches_exact_fp32_kernel(cin, cout):
 
 
 @pytest.mark.parametrize("n0,n1,C", [(5000, 3777, 32), (130, 1, 96), (128, 128, 64), (1, 300, 256)])
-def test_segmented_batchnorm_equals_two_batches(n0, n1, C):
+def test_segmented_batchnorm_relu_hi_plane_equals_two_batches(n0, n1, C):
     """pcb_bn_*_seg: rows [0,n0) and [n0,n0+n1) normalised as two batches (the two views of a pair stacked in one matrix)
     == torch BatchNorm1d applied to view 0 and then to view 1 (fp64), including the sequential running-stat updates and
-    the summed parameter gradients; residual + ReLU folded in as in the fused executor."""
+    the summed parameter gradients; residual + ReLU folded in as in the fused executor, the backward taking its ReLU mask
+    from the bf16 hi plane the apply pass wrote."""
     from pointcontrast_b200 import _lib
     from pointcontrast_b200._lib import check, lib, ptr, stream
     n = n0 + n1
@@ -343,7 +344,7 @@ def test_segmented_batchnorm_equals_two_batches(n0, n1, C):
     assert rel_err(rm, ref.running_mean) < 1e-5 and rel_err(rv, ref.running_var) < 1e-5
     dX = torch.empty(n, C, device=dev); dW = torch.zeros(C, device=dev); dB = torch.zeros(C, device=dev)
     gout = torch.empty(n, C, device=dev)
-    check(lib.pcb_bn_backward_seg(ptr(DY), C, ptr(X), C, ptr(Y), C, n, n0, C, ptr(mean), ptr(invstd), ptr(W), ptr(dX), C, ptr(dW), ptr(dB), 1,
+    check(lib.pcb_bn_backward_seg(ptr(DY), C, ptr(X), C, ptr(hi), C, n, n0, C, ptr(mean), ptr(invstd), ptr(W), ptr(dX), C, ptr(dW), ptr(dB), 1,
                                   ptr(gout), C, 1, None, None, 0, ptr(ws), wsb, st))
     assert max_rel_err(dX, xo.grad) < 1e-4 and max_rel_err(gout, ro.grad) < 1e-5
     assert rel_err(dW, ref.weight.grad) < 1e-4 and rel_err(dB, ref.bias.grad) < 1e-4

@@ -183,7 +183,8 @@ def bn_stats(n, n0, C):
 
 def bn_backward(n, n0, C):
     i = _In(14)
-    dY, X, relu, mean, invstd, gamma = i.rand(n, C), i.rand(n, C), i.rand(n, C, scale=2.0) - 0.5, i.rand(2 * C), i.rand(2 * C) + 0.5, i.rand(C)
+    dY, X, relu = i.rand(n, C), i.rand(n, C), (i.rand(n, C, scale=2.0) - 0.5).to(torch.bfloat16)      # relu: a bf16 hi plane
+    mean, invstd, gamma = i.rand(2 * C), i.rand(2 * C) + 0.5, i.rand(C)
     dX, dgamma, dbeta = i.zeros(n, C), i.zeros(C), i.zeros(C)
     return (L.pcb_bn_ws_bytes(n, C),
             lambda ws, b: L.pcb_bn_backward_seg(dY.data_ptr(), C, X.data_ptr(), C, relu.data_ptr(), C, n, n0, C, mean.data_ptr(), invstd.data_ptr(),
