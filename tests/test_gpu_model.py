@@ -30,11 +30,11 @@ def _grad_tol(floor, factor):
     return np.full_like(floor, max(1e-3, factor * float(floor.max())))
 
 
-def _gpu_net(seed=0, normalize=True):
+def _gpu_net(seed=0, normalize=True, model="Res16UNet34C"):
     from pointcontrast_b200.model import load_model
     cfg = refload.default_config()
     cfg["net"]["normalize_feature"] = normalize
-    net = load_model("Res16UNet34C")(3, 32, cfg, D=3)
+    net = load_model(model)(3, 32, cfg, D=3)
     det_init(net, seed)
     return net.cuda().train()
 
@@ -205,6 +205,11 @@ def test_eval_mode_forward_matches_oracle_semseg_shape():
 def test_fused_executor_matches_modular_path():
     """One-autograd-node fused executor (pointcontrast_b200/fused.py) vs the per-module ME-style path: same kernels, so
     features, every parameter gradient and the BatchNorm running statistics agree to fp32 rounding."""
+    check_fused_matches_modular("Res16UNet34C")
+
+
+def check_fused_matches_modular(model):
+    """test_fused_executor_matches_modular_path on the model class `model` (also run on Res16UNet14 by tests/test_gpu_conv_exact.py)."""
     from pointcontrast_b200 import fused, losses, me, synth
     batch = synth.collate_pairs([synth.synth_pair(5, scale=0.15), synth.synth_pair(6, scale=0.12)])
     rng = np.random.default_rng(1)
@@ -218,9 +223,10 @@ def test_fused_executor_matches_modular_path():
     for mode in (True, False):
         fused.ENABLED = mode
         try:
-            net = _gpu_net(4)
+            net = _gpu_net(4, model=model)
             F = [net(me.SparseTensor(torch.from_numpy(batch[f"sinput{v}_F"]), coords=torch.from_numpy(batch[f"sinput{v}_C"])).to("cuda")).F
                  for v in "01"]
+            assert ("_fused_runner" in net.__dict__) == mode
             loss = losses.point_nce_loss(F[0], F[1], q.cuda(), k.cuda(), 0.4)
             loss.backward()
             out[mode] = (F[0].detach(), F[1].detach(), float(loss.detach()), {n: p.grad.clone() for n, p in net.named_parameters()},
