@@ -1,9 +1,10 @@
 // Hopper sparse convolution: the output-stationary gather-GEMM of conv.cu with the per-offset Cin x Cout contraction issued as
-// wgmma.mma_async, fp32 accumulators in registers.  CTA = 128 output rows x BN channels = two warpgroups of M64.  The input arrives as
-// 16-bit hi/lo planes, gathered per offset by cp.async (zero-filled where there is no neighbour) into the K-major no-swizzle
-// core-matrix layout; the weights arrive pre-tiled as shared-memory images, one TMA bulk copy per stage on an mbarrier.  Per
-// 32-channel step each warpgroup issues 2 k16-steps x 3 products (lo.hi + hi.lo + hi.hi).  Offsets without a neighbour in the
-// tile are skipped; small levels split the steps over gridDim.z (partial planes + fixed-order reduce).
+// wgmma.mma_async, fp32 accumulators in registers.  CTA = 128 output rows x BN channels = one producer warpgroup and two consumer
+// warpgroups of M64.  The producer gathers the input, 16-bit hi/lo planes, per offset by cp.async (zero-filled where there is no
+// neighbour) into the K-major no-swizzle core-matrix layout, and fetches the weights, pre-tiled as shared-memory images, by one TMA
+// bulk copy per stage; both complete on the stage's mbarrier.  Per 32-channel step each consumer warpgroup issues 2 k16-steps x 3
+// products (lo.hi + hi.lo + hi.hi).  Offsets without a neighbour in the tile are skipped; small levels split the steps over
+// gridDim.z (partial planes + fixed-order reduce).
 #include "common.cuh"
 #include "wgmma_ptx.cuh"
 
@@ -13,9 +14,11 @@ namespace pcb {
 
 namespace hw {
 
-// NS-slot ring, loads PF = NS - 2 steps ahead: the slot written at step i was last read by the MMAs of step i - 2, which every
-// warpgroup has waited for (wgmma.wait_group 1) before the barrier of step i - 1.
-constexpr int BM = 128, BK = 32, NTHR = 256, NS = 4, PF = NS - 2;
+// Warpgroup 0 produces, warpgroups 1 and 2 consume.  Ring slot s has two mbarriers: full[s] (the producer's 128 threads arrive
+// through cp.async.mbarrier.arrive.noinc, thread 0 once more with the weight tile's expect_tx) and empty[s] (lane 0 of each of the
+// 8 consumer warps, once wgmma.wait_group shows that the MMAs reading the slot have retired).
+constexpr int BM = 128, BK = 32, NPROD = 128, NCONS_WARPS = 8, NTHR = NPROD + 32 * NCONS_WARPS;
+constexpr int SMEM_OPTIN = 227 * 1024, SMEM_PER_SM = 228 * 1024;      // sm_90: largest dynamic shared memory of one CTA, of one SM
 constexpr int A_SBO = 128;
 // k8-chunk stride of the A tile: +32 bytes, so that the four 16-byte chunks (t & 3) x two rows (t >> 2) written by a quarter-warp of a
 // 128-bit st.shared cover eight different 16-byte slots of a 128-byte bank line.
@@ -35,21 +38,30 @@ struct Args {
   float out_scale;      // applied to the accumulators on the way out (2^-10 when the weight tiles hold fp16(W * 2^10))
 };
 
+// The ring takes every slot that fits beside the table slice in the CTA's share of shared memory.  BN = 128 and 96 run one CTA per
+// SM, with 6 and 7 slots.  BN = 64 and 32 run two CTAs per SM with 4 slots each: on an H100 that beat one CTA with 8 and 10 slots
+// at every BN <= 64 layer shape of the C1 training step (up to 22 % less kernel time, 0.65 ms less per step).
 template <int BN>
 struct Smem {
   static constexpr int B_SBO = 128;
   static constexpr int B_LBO = (BN / 8) * 128 + 16;
   static constexpr int B_PLANE = (BK / 8) * B_LBO;
   static constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
+  static constexpr int CTAS = BN <= 64 ? 2 : 1;                                  // resident CTAs per SM
+  static constexpr int BUDGET = CTAS == 1 ? SMEM_OPTIN : SMEM_PER_SM / 2 - 1024;  // 1 KB per CTA is reserved by the system
+  static constexpr int FIXED = PCB_MAX_KERNEL_VOLUME * BM * 4 + 72 * 4 + 16;
+  static constexpr int NS = (BUDGET - FIXED) / (STAGE + 16);                      // + full and empty barrier per slot
   static constexpr int IDX_OFF = NS * STAGE;
   static constexpr int META_OFF = IDX_OFF + PCB_MAX_KERNEL_VOLUME * BM * 4;     // flags[32] klist[32] nk
-  static constexpr int BAR_OFF = META_OFF + 72 * 4;
-  static constexpr int TOTAL = BAR_OFF + NS * 8 + 16;
+  static constexpr int BAR_OFF = META_OFF + 72 * 4;                               // full[NS], empty[NS]
+  static constexpr int TOTAL = BAR_OFF + 2 * NS * 8 + 16;
+  static_assert(TOTAL <= BUDGET, "ring does not fit");
 };
 
 template <int BN, bool F16>
-__global__ void __launch_bounds__(NTHR, 1) conv_wgmma_kernel(const Args p) {
+__global__ void __launch_bounds__(NTHR, Smem<BN>::CTAS) conv_wgmma_kernel(const Args p) {
   using S = Smem<BN>;
+  constexpr int NS = S::NS;
   extern __shared__ __align__(128) unsigned char smem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2;
   const int64_t row0 = (int64_t)blockIdx.x * BM;
@@ -59,10 +71,14 @@ __global__ void __launch_bounds__(NTHR, 1) conv_wgmma_kernel(const Args p) {
   int* s_klist = s_flag + 32;
   int* s_nk = s_klist + 32;
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full_bar = smem_base + S::BAR_OFF;          // "weight tile of slot s landed"
+  const uint32_t full_bar = smem_base + S::BAR_OFF;          // "A rows and weight tile of slot s landed"
+  const uint32_t empty_bar = full_bar + 8 * NS;              // "the MMAs reading slot s have retired"
 
   if (tid == 0) {
-    for (int i = 0; i < NS; ++i) mbar_init(full_bar + 8 * i, 1);
+    for (int i = 0; i < NS; ++i) {
+      mbar_init(full_bar + 8 * i, NPROD + 1);
+      mbar_init(empty_bar + 8 * i, NCONS_WARPS);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   pdl_wait(); pdl_trigger();        // no global memory touched before this
@@ -112,44 +128,48 @@ __global__ void __launch_bounds__(NTHR, 1) conv_wgmma_kernel(const Args p) {
   const int nblk = p.Cout / BN;
   constexpr uint32_t BLOB = 2 * S::B_PLANE;
 
-  // ---- pipeline step i (relative to it0) uses slot i % NS
-  // asynchronous copies of step i: one cp.async group per call (possibly empty)
-  auto load_async = [&](int i) {
-    if (i < n_it) {
+  // ---- pipeline step i (relative to it0) uses slot i % NS, in its (i / NS)-th round
+  if (wg == 0) {
+    // producer: thread t copies the 16-byte k8-chunk t % 4 of rows t / 4 + 32 q (q < 4) of both planes, zero-filled where there
+    // is no neighbour; thread 0 also issues the stage's weight tile, one TMA bulk copy of the pre-tiled image
+    const int k8 = tid & 3, r0 = tid >> 2;
+#pragma unroll 1
+    for (int i = 0; i < n_it; ++i) {
       const int it = it0 + i, s = i % NS;
       const int k = s_klist[it / nkc], kc = it % nkc;
       const uint32_t sb = smem_base + s * S::STAGE;
-      // A: 128 rows x 4 k8-chunks x 2 planes of 16 bytes, zero-filled where there is no neighbour
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int c = tid + j * NTHR;
-        const int plane = c >> 9, rem = c & 511, r = rem >> 2, k8 = rem & 3;
-        const int idx = s_idx[k * BM + r];
-        const __nv_bfloat16* src = (plane ? p.Xlo : p.Xhi) + (int64_t)(idx >= 0 ? idx : 0) * p.lds + kc * BK + k8 * 8;
-        cp_async16_zfill(sb + plane * A_PLANE + k8 * A_LBO + (r >> 3) * A_SBO + (r & 7) * 16, src, idx >= 0 ? 16u : 0u);
-      }
-      // B: the stage's weight tile is one TMA bulk copy of the pre-tiled image
+      mbar_wait(empty_bar + 8 * s, (uint32_t)(((i / NS) & 1) ^ 1));    // round 0 passes at once
       if (tid == 0) {
         mbar_arrive_expect_tx(full_bar + 8 * s, BLOB);
         tma_bulk_load(sb + 2 * A_PLANE, p.wt + ((int64_t)(k * nkc + kc) * nblk + blockIdx.y) * BLOB, BLOB, full_bar + 8 * s);
       }
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int r = r0 + 32 * q;
+        const int idx = s_idx[k * BM + r];
+        const int64_t off = (int64_t)(idx >= 0 ? idx : 0) * p.lds + kc * BK + k8 * 8;
+        const uint32_t dst = sb + k8 * A_LBO + (r >> 3) * A_SBO + (r & 7) * 16;
+        cp_async16_zfill(dst, p.Xhi + off, idx >= 0 ? 16u : 0u);
+        cp_async16_zfill(dst + A_PLANE, p.Xlo + off, idx >= 0 ? 16u : 0u);
+      }
+      cp_async_mbar_arrive_noinc(full_bar + 8 * s);
     }
     cp_async_commit();
-  };
+    cp_async_wait<0>();         // no copy of this thread outlives it
+    return;
+  }
 
+  // consumers: warpgroup 1 + h owns the rows 64 h .. 64 h + 63 of the tile
+  const int h64 = wg - 1;
   float acc[BN / 2];
 #pragma unroll
   for (int e = 0; e < BN / 2; ++e) acc[e] = 0.f;
   if (n_it > 0) {
-#pragma unroll 1
-    for (int i = 0; i < PF; ++i) load_async(i);
     for (int i = 0; i < n_it; ++i) {
       const int s = i % NS;
-      cp_async_wait<PF - 1>();                         // this thread's copies of step i have landed
       mbar_wait(full_bar + 8 * s, (uint32_t)((i / NS) & 1));
-      fence_proxy_async();                             // generic-proxy smem writes -> visible to the tensor cores (async proxy)
-      __syncthreads();
-      const uint32_t a_hi = smem_base + s * S::STAGE + wg * 8 * A_SBO, a_lo = a_hi + A_PLANE;
+      fence_proxy_async();                             // generic-proxy smem writes (cp.async) -> visible to the tensor cores
+      const uint32_t a_hi = smem_base + s * S::STAGE + h64 * 8 * A_SBO, a_lo = a_hi + A_PLANE;
       const uint32_t b_hi = smem_base + s * S::STAGE + 2 * A_PLANE, b_lo = b_hi + S::B_PLANE;
       fence_regs(acc);
       wgmma_fence();
@@ -163,21 +183,21 @@ __global__ void __launch_bounds__(NTHR, 1) conv_wgmma_kernel(const Args p) {
         wgmma<BN, F16, 0, 0>(acc, dah, dbh, 1u);
       }
       wgmma_commit();
-      wgmma_wait<1>();
+      wgmma_wait<1>();                                 // the MMAs of step i - 1 have retired: release its slot
       fence_regs(acc);
-      load_async(i + PF);      // its slot was last read by the MMAs of step i - 2, done in every warpgroup before this step's barrier
+      if (i > 0 && lane == 0) mbar_arrive(empty_bar + 8 * ((i - 1) % NS));
     }
     wgmma_wait<0>();
     fence_regs(acc);
   }
 
-  // ---- epilogue from the accumulator fragments: row 64 wg + 16 (warp % 4) + lane / 4 (+ 8), columns 8 c + 2 (lane % 4) (+ 1)
+  // ---- epilogue from the accumulator fragments: row 64 h64 + 16 (warp % 4) + lane / 4 (+ 8), columns 8 c + 2 (lane % 4) (+ 1)
   float* outp = p.partial ? p.partial + (int64_t)blockIdx.z * p.n_out * p.Cout : p.Y;
   const int ldo = p.partial ? p.Cout : p.ldy;
   const float* bias = p.partial ? nullptr : p.bias;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int64_t row = row0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    const int64_t row = row0 + h64 * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
     if (row >= p.n_out) continue;
     float* dst = outp + row * ldo + n0;
 #pragma unroll
@@ -252,6 +272,8 @@ int wgrad_group() { return 2; }
 
 namespace wg {
 
+// NS-slot ring, loads PF = NS - 2 steps ahead: the slot written at step i was last read by the MMAs of step i - 2, which every
+// warpgroup has waited for (wgmma.wait_group 1) before the barrier of step i - 1.
 constexpr int WM = 128, WK = 16, GK = 2, NTHR = 256, NS = 4, PF = NS - 2, TF = 2;
 
 struct Args {
