@@ -86,7 +86,8 @@ int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const v
 int launch_wgrad_wgmma(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
                        const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int Ca, int Cb, int rows_per_split, int splits,
                        float* partial, int transpose_out, int tn, cudaStream_t st);
-int wgrad_group();
+// conv.cu: the channel tile of the tensor-core kernels, the largest of {128, 96, 64, 32} dividing C (0 if none does)
+int pick_tile(int C);
 // bn.cu: the statistics passes of pcb_unit_forward -- eval mode, and fused into the reduction of an offset-split convolution
 int bn_eval_stats_launch(const float* running_mean, const float* running_var, int C, float eps, float* mean, float* invstd, cudaStream_t st);
 int bn_reduce_stats_launch(const float* P, int nsplit, float* Y, int ldy, int64_t n, int64_t n0, int C, float eps, float momentum,

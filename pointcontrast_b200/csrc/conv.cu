@@ -18,6 +18,14 @@
 
 using namespace pcb;
 
+int pcb::pick_tile(int C) {
+  if (C % 128 == 0) return 128;
+  if (C % 96 == 0) return 96;
+  if (C % 64 == 0) return 64;
+  if (C % 32 == 0) return 32;
+  return 0;
+}
+
 namespace {
 
 struct KMap { int v[PCB_MAX_KERNEL_VOLUME]; };
@@ -216,14 +224,6 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int split
   float s = 0.f;
   for (int sp = 0; sp < splits; ++sp) s += partial[(int64_t)sp * n + i];
   dW[i] = accumulate ? dW[i] + s : s;
-}
-
-int pick_tile(int C) {      // largest of {128, 96, 64, 32} dividing C
-  if (C % 128 == 0) return 128;
-  if (C % 96 == 0) return 96;
-  if (C % 64 == 0) return 64;
-  if (C % 32 == 0) return 32;
-  return 0;
 }
 
 // Small levels (a few hundred rows at 256 channels) would otherwise be a handful of CTAs each walking 27 x Cin/32
@@ -524,11 +524,13 @@ extern "C" int pcb_conv_forward_split(const uint16_t* Xhi, const uint16_t* Xlo, 
 namespace {
 int wgrad_split_splits(int K, int64_t n_out, int Ca, int Cb) {
   int tn = pick_tile(Cb);
-  const int gk = pcb::wgrad_group();          // offsets per CTA
-  int64_t base = (int64_t)((K + gk - 1) / gk) * ((Ca + 127) / 128) * (Cb / tn);      // CTAs per split: offset groups x channel blocks
+  // the row partition counts units of 2 offsets x 128 channels of A, whatever the kernel's tile: it fixes which rows each fp32 partial
+  // sums, and so the result bits
+  constexpr int UNIT_OFFSETS = 2, UNIT_CHANNELS = 128;
+  int64_t base = (int64_t)((K + UNIT_OFFSETS - 1) / UNIT_OFFSETS) * ((Ca + UNIT_CHANNELS - 1) / UNIT_CHANNELS) * (Cb / tn);
   const double wwaves = 1.0;
-  // heuristic, not tuned on H100: aim for 2 x num_sms CTAs (two waves of a kernel that fits once per SM), never a nearly-empty extra
-  // wave; shorter row ranges per split also keep each fp32 accumulator's sum short
+  // heuristic, not tuned on H100: aim for 2 x num_sms units, never a nearly-empty extra wave; shorter row ranges per split
+  // also keep each fp32 accumulator's sum short
   int64_t s = (int64_t)(wwaves * 2 * num_sms()) / base;
   int64_t max_s = (n_out + 63) / 64;          // small levels: rather many short CTAs than a few long serial ones
   if (s > max_s) s = max_s;

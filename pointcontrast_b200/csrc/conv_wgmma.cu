@@ -260,21 +260,22 @@ int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const v
 
 // ------------------------------------------------------------------------------------------------ weight gradient
 // dW[k] (Ca x Cb) = sum_j A[tbl[k][j], :]^T . B[j, :] on split (16-bit hi/lo) operands.
-// wgmma view: D_k[M = Ca-block (padded to 128)][N = Cb-block] += A_k[M x 16 rows] . B[16 rows x N]; both operands MN-major
-// (a matrix row is contiguous along channels): core matrix = 8 rows (K) x 16 B (8 channels), channel-chunk stride SBO = 144 B,
-// 8-row-group stride LBO.  Warpgroup g computes the channel rows 64g .. 64g + 63 of the block.
-// A CTA owns a GROUP of WG_GROUP kernel offsets and a range of table rows: the row-aligned operand B is staged ONCE per 16-row step and
-// shared by the gathered operands A_k, each accumulating into its own register accumulator.  Thread = (row, 16-byte channel chunk) of
-// the step; its copies are cp.async (zero-filled where there is no neighbour), the table entries they depend on are fetched TF steps
-// earlier into registers so that no dependent global-load latency sits on the per-step path.
+// A CTA owns a group of GK kernel offsets, a CB-channel block of A (CB = pick_tile(Ca)), a TN-channel block of B and one row split.
+// The offsets are stacked along M: D[M = GK offsets x CB channels][N = TN] += A[M x 16 rows] . B[16 rows x N], so the row-aligned
+// operand B is staged once per row step and shared by every offset of the group, and GK * CB fills whole M64 slices without padding.
+// Both operands are MN-major (a matrix row is contiguous along channels): core matrix = 8 rows (K) x 16 B (8 channels), chunk stride
+// 128 B, 8-row-group stride LBO; the stacked A tile's chunks run (offset, channel).
+// Warpgroup 0 produces: per 32-row stage, the zero-filling cp.async copies of B's rows (not read where no offset of the group has a
+// neighbour) and of every offset's gathered A rows, completing on the slot's "full" mbarrier; the table entries they depend on are
+// loaded TF stages earlier into registers.  Warpgroups 1 and 2 consume, each SL of the tile's M64 slices, and release a slot on its
+// "empty" mbarrier once wgmma.wait_group shows that the MMAs reading it have retired.  Within a split, every accumulator element takes
+// the k16 steps in ascending row order and per step the products lo.hi, hi.lo, hi.hi.
 // grid: x = groups * mblocks * nblocks, y = row splits; partial tiles are reduced by wgrad_reduce_kernel (conv.cu).
-int wgrad_group() { return 2; }
-
 namespace wg {
 
-// NS-slot ring, loads PF = NS - 2 steps ahead: the slot written at step i was last read by the MMAs of step i - 2, which every
-// warpgroup has waited for (wgmma.wait_group 1) before the barrier of step i - 1.
-constexpr int WM = 128, WK = 16, GK = 2, NTHR = 256, NS = 4, PF = NS - 2, TF = 2;
+constexpr int WK = 16, NPROD = 128, NCONS_WARPS = 8, NTHR = NPROD + 32 * NCONS_WARPS, TF = 4;
+// registers per thread after setmaxnreg: 128 x 40 + 256 x 232 <= 64 K; the consumers hold up to 3 x 64 accumulators (CB = 96, TN = 128)
+constexpr int PROD_REGS = 40, CONS_REGS = 232;
 
 struct Args {
   const __nv_bfloat16* Ahi; const __nv_bfloat16* Alo; int lda;      // gathered operand (elements)
@@ -284,167 +285,211 @@ struct Args {
   float* partial; int transpose_out;
 };
 
-// channel-chunk (core-matrix) stride 144 B, not 128: the 16 threads of one row write 16 consecutive chunks, and a 128-byte stride
-// would put them on the same shared-memory banks
-constexpr int SBO = 144;
-__host__ __device__ inline int a_lbo(int mrows) { return (mrows / 8) * SBO + 16; }
-__host__ __device__ inline int b_lbo(int tn) { return (tn / 8) * SBO + 16; }
-__host__ __device__ inline int stage_bytes(int mrows, int tn) { return 4 * b_lbo(tn) + GK * 4 * a_lbo(mrows); }
+// Stage = B hi, B lo, A hi, A lo planes of RS rows; the ring takes every slot that fits.
+template <int CB, int TN>
+struct Smem {
+  static constexpr int GK = CB % 64 == 0 ? 2 : 4;        // offsets per CTA: GK * CB is a multiple of 128 (two consumers x M64)
+  static constexpr int MT = GK * CB;
+  static constexpr int SL = MT / 128;                     // M64 slices per consumer warpgroup
+  static constexpr int RS = 32;                           // rows per stage
+  static constexpr int NQ = RS / 32;                      // rows per producer thread
+  static constexpr int A_LBO = MT / 8 * 128, B_LBO = TN / 8 * 128;
+  static constexpr int A_PLANE = RS / 8 * A_LBO, B_PLANE = RS / 8 * B_LBO;
+  static constexpr int A_OFF = 2 * B_PLANE;
+  static constexpr int STAGE = 2 * B_PLANE + 2 * A_PLANE;
+  static constexpr int NS = (hw::SMEM_OPTIN - 16) / (STAGE + 16);    // + full and empty barrier per slot
+  static constexpr int BAR_OFF = NS * STAGE;
+  static constexpr int TOTAL = BAR_OFF + 2 * NS * 8;
+  static_assert(MT % 128 == 0 && NS >= 3 && TOTAL <= hw::SMEM_OPTIN, "weight-gradient tile does not fit");
+};
 
-template <int TN>
+template <int CB, int TN>
 __global__ void __launch_bounds__(NTHR, 1) wgrad_wgmma_kernel(const Args p) {
   using namespace hw;
+  using S = Smem<CB, TN>;
+  constexpr int GK = S::GK, NS = S::NS, RS = S::RS, NQ = S::NQ, ACH = CB / 8, BCH = TN / 8;
   extern __shared__ __align__(128) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = warp >> 2;
-  const int mblocks = (p.Ca + WM - 1) / WM, nblocks = p.Cb / TN;
+  const int mblocks = p.Ca / CB, nblocks = p.Cb / TN;
   int bx = blockIdx.x;
   const int nb = bx % nblocks; bx /= nblocks;
   const int mb = bx % mblocks; bx /= mblocks;
   const int k0 = bx * GK;
-  const int nk = min(GK, p.K - k0);
-  const int m0 = mb * WM, n0 = nb * TN;
-  const int mrows = min(WM, p.Ca - m0);                 // valid M rows of this block (multiple of 32)
-  const int ach = mrows / 8;
-  constexpr int BCH = TN / 8;
-  const int A_LBO = a_lbo(mrows), B_LBO = b_lbo(TN);
-  const int STAGE = stage_bytes(mrows, TN);
+  const int nk = min(GK, p.K - k0);                     // offsets of this group; the A rows of the others are zero-filled
+  const int m0 = mb * CB, n0 = nb * TN;
   const int64_t r_begin = (int64_t)blockIdx.y * p.rows_per_split;
   const int64_t r_end = min(p.n_out, r_begin + p.rows_per_split);
-  const int nsteps = r_end > r_begin ? (int)((r_end - r_begin + WK - 1) / WK) : 0;
+  const int nst = r_end > r_begin ? (int)((r_end - r_begin + RS - 1) / RS) : 0;
   const uint32_t smem_base = smem_u32(smem);
+  const uint32_t full_bar = smem_base + S::BAR_OFF;     // "B and A rows of slot s landed"
+  const uint32_t empty_bar = full_bar + 8 * NS;         // "the MMAs reading slot s have retired"
+  if (tid == 0) {
+    for (int i = 0; i < NS; ++i) {
+      mbar_init(full_bar + 8 * i, NPROD);
+      mbar_init(empty_bar + 8 * i, NCONS_WARPS);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
   pdl_wait(); pdl_trigger();
+  __syncthreads();
 
-  const int r = tid >> 4, ch = tid & 15;                // row of the step, 16-byte channel chunk
-  const bool a_on = ch < ach, b_on = ch < BCH;
-  const uint32_t a_dst = (r >> 3) * A_LBO + ch * SBO + (r & 7) * 16;
-  const uint32_t b_dst = (r >> 3) * B_LBO + ch * SBO + (r & 7) * 16;
-  const int64_t a_col = m0 + ch * 8, b_col = n0 + ch * 8;
-  const int32_t* trow = p.tbl + (int64_t)k0 * p.tbl_stride;
-  int tq[TF + PF][GK];                                  // table entries of steps issued .. issued + TF + PF - 1
-  auto fetch = [&](int (&d)[GK], int step) {
-    const int64_t row = r_begin + (int64_t)step * WK + r;
-    const bool live = step < nsteps && row < r_end;
+  // ---- stage i (RS rows from r_begin + RS i) uses slot i % NS, in its (i / NS)-th round
+  if (wgi == 0) {
+    setmaxnreg_dec<PROD_REGS>();
+    // thread: rows r + 32 q of every stage, 16-byte channel chunks c4 + 4 j of B and of each offset's A block.  A warp's copy covers
+    // 8 rows x 64 contiguous bytes in global memory and four whole 128-byte chunk columns in shared memory.
+    const int r = 8 * warp + (lane >> 2), c4 = lane & 3;
+    const uint32_t dst = (r & 7) * 16 + c4 * 128;
+    const uint32_t dst_b = dst + (r >> 3) * S::B_LBO, dst_a = S::A_OFF + dst + (r >> 3) * S::A_LBO;
+    int tq[TF + 1][NQ][GK];                              // table entries of stages i .. i + TF
+    auto fetch = [&](int (&d)[NQ][GK], int st) {
 #pragma unroll
-    for (int g = 0; g < GK; ++g) d[g] = (live && g < nk) ? __ldg(trow + g * p.tbl_stride + row) : -1;
-  };
-  // copies of step i into slot i % NS (one cp.async group per call, possibly empty); consumes tq[0] and shifts the table ring
-  int issued = 0;
-  auto load = [&]() {
-    if (issued < nsteps) {
-      const int64_t row = r_begin + (int64_t)issued * WK + r;
-      const uint32_t sb = smem_base + (issued % NS) * STAGE;
-      bool any = false;
+      for (int q = 0; q < NQ; ++q) {
+        const int64_t row = r_begin + (int64_t)st * RS + r + 32 * q;
 #pragma unroll
-      for (int g = 0; g < GK; ++g) any |= tq[0][g] >= 0;
-      if (b_on) {
-        const int64_t off = (any ? row : 0) * p.ldb + b_col;
-        cp_async16_zfill(sb + b_dst, p.Bhi + off, any ? 16u : 0u);
-        cp_async16_zfill(sb + 2 * B_LBO + b_dst, p.Blo + off, any ? 16u : 0u);
+        for (int g = 0; g < GK; ++g)
+          d[q][g] = (row < r_end && g < nk) ? __ldg(p.tbl + (int64_t)(k0 + g) * p.tbl_stride + row) : -1;
       }
-      if (a_on) {
+    };
+#pragma unroll
+    for (int f = 0; f < TF; ++f) fetch(tq[f], f);
+#pragma unroll 1
+    for (int i = 0; i < nst; ++i) {
+      fetch(tq[TF], i + TF);
+      const int s = i % NS;
+      mbar_wait(empty_bar + 8 * s, (uint32_t)(((i / NS) & 1) ^ 1));    // round 0 passes at once
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) {
+        const int64_t row = r_begin + (int64_t)i * RS + r + 32 * q;
+        const uint32_t sb = smem_base + s * S::STAGE + q * 4 * S::B_LBO, sa = smem_base + s * S::STAGE + q * 4 * S::A_LBO;
+        bool any = false;
+#pragma unroll
+        for (int g = 0; g < GK; ++g) any |= tq[0][q][g] >= 0;
+        const int64_t boff = (any ? row : 0) * p.ldb + n0 + c4 * 8;
+#pragma unroll
+        for (int j = 0; j < BCH / 4; ++j) {
+          cp_async16_zfill(sb + dst_b + j * 512, p.Bhi + boff + j * 32, any ? 16u : 0u);
+          cp_async16_zfill(sb + S::B_PLANE + dst_b + j * 512, p.Blo + boff + j * 32, any ? 16u : 0u);
+        }
 #pragma unroll
         for (int g = 0; g < GK; ++g) {
-          const int c = tq[0][g];
-          const int64_t off = (int64_t)(c >= 0 ? c : 0) * p.lda + a_col;
-          const uint32_t ab = sb + 4 * B_LBO + g * 4 * A_LBO + a_dst;
-          cp_async16_zfill(ab, p.Ahi + off, c >= 0 ? 16u : 0u);
-          cp_async16_zfill(ab + 2 * A_LBO, p.Alo + off, c >= 0 ? 16u : 0u);
+          const int c = tq[0][q][g];
+          const int64_t aoff = (int64_t)(c >= 0 ? c : 0) * p.lda + m0 + c4 * 8;
+#pragma unroll
+          for (int j = 0; j < ACH / 4; ++j) {
+            const uint32_t d = sa + dst_a + (g * ACH + 4 * j) * 128;
+            cp_async16_zfill(d, p.Ahi + aoff + j * 32, c >= 0 ? 16u : 0u);
+            cp_async16_zfill(d + S::A_PLANE, p.Alo + aoff + j * 32, c >= 0 ? 16u : 0u);
+          }
+        }
+      }
+      cp_async_mbar_arrive_noinc(full_bar + 8 * s);
+#pragma unroll
+      for (int f = 0; f < TF; ++f) {
+#pragma unroll
+        for (int q = 0; q < NQ; ++q) {
+#pragma unroll
+          for (int g = 0; g < GK; ++g) tq[f][q][g] = tq[f + 1][q][g];
         }
       }
     }
     cp_async_commit();
-#pragma unroll
-    for (int f = 0; f + 1 < TF + PF; ++f) {
-#pragma unroll
-      for (int g = 0; g < GK; ++g) tq[f][g] = tq[f + 1][g];
-    }
-    fetch(tq[TF + PF - 1], issued + TF + PF);
-    ++issued;
-  };
-
-  float acc[GK][TN / 2];
-#pragma unroll
-  for (int g = 0; g < GK; ++g) {
-#pragma unroll
-    for (int e = 0; e < TN / 2; ++e) acc[g][e] = 0.f;
+    cp_async_wait<0>();         // no copy of this thread outlives it
+    return;
   }
-  if (nsteps > 0) {
+
+  // consumers: warpgroup 1 + h owns the M64 slices h SL .. h SL + SL - 1 of the stacked tile
+  setmaxnreg_inc<CONS_REGS>();
+  const int h = wgi - 1;
+  float acc[S::SL][TN / 2];
 #pragma unroll
-    for (int f = 0; f < TF + PF; ++f) fetch(tq[f], f);
+  for (int sl = 0; sl < S::SL; ++sl) {
+#pragma unroll
+    for (int e = 0; e < TN / 2; ++e) acc[sl][e] = 0.f;
+  }
+  if (nst > 0) {
 #pragma unroll 1
-    for (int i = 0; i < PF; ++i) load();
-    for (int i = 0; i < nsteps; ++i) {
+    for (int i = 0; i < nst; ++i) {
       const int s = i % NS;
-      cp_async_wait<PF - 1>();
-      fence_proxy_async();
-      __syncthreads();
-      // issued unconditionally (branch-free, so the wgmma's stay asynchronous): the A slots of a missing second offset are
-      // zero-filled, and the fragment rows of an upper warpgroup beyond mrows are never read back
-      const uint32_t sb = smem_base + s * STAGE;
-      const uint64_t dbh = make_desc(sb, B_LBO, SBO), dbl = make_desc(sb + 2 * B_LBO, B_LBO, SBO);
+      mbar_wait(full_bar + 8 * s, (uint32_t)((i / NS) & 1));
+      fence_proxy_async();                             // generic-proxy smem writes (cp.async) -> visible to the tensor cores
+      const uint32_t sb = smem_base + s * S::STAGE;
 #pragma unroll
-      for (int g = 0; g < GK; ++g) fence_regs(acc[g]);
+      for (int sl = 0; sl < S::SL; ++sl) fence_regs(acc[sl]);
       wgmma_fence();
+      // issued unconditionally (branch-free, so the wgmma's stay asynchronous): rows past the split's end are zero-filled, and the
+      // fragment rows of offsets past K are never read back
 #pragma unroll
-      for (int g = 0; g < GK; ++g) {
-        const uint32_t ab = sb + 4 * B_LBO + g * 4 * A_LBO + wgi * 8 * SBO;
-        const uint64_t dah = make_desc(ab, A_LBO, SBO), dal = make_desc(ab + 2 * A_LBO, A_LBO, SBO);
-        wgmma<TN, false, 1, 1>(acc[g], dal, dbh, 1u);
-        wgmma<TN, false, 1, 1>(acc[g], dah, dbl, 1u);
-        wgmma<TN, false, 1, 1>(acc[g], dah, dbh, 1u);
+      for (int kk = 0; kk < RS / WK; ++kk) {
+        const uint32_t b_hi = sb + kk * 2 * S::B_LBO;
+        const uint64_t dbh = make_desc(b_hi, S::B_LBO, 128), dbl = make_desc(b_hi + S::B_PLANE, S::B_LBO, 128);
+#pragma unroll
+        for (int sl = 0; sl < S::SL; ++sl) {
+          const uint32_t a_hi = sb + S::A_OFF + kk * 2 * S::A_LBO + (h * S::SL + sl) * 8 * 128;
+          const uint64_t dah = make_desc(a_hi, S::A_LBO, 128), dal = make_desc(a_hi + S::A_PLANE, S::A_LBO, 128);
+          wgmma<TN, false, 1, 1>(acc[sl], dal, dbh, 1u);
+          wgmma<TN, false, 1, 1>(acc[sl], dah, dbl, 1u);
+          wgmma<TN, false, 1, 1>(acc[sl], dah, dbh, 1u);
+        }
       }
       wgmma_commit();
-      wgmma_wait<1>();
+      wgmma_wait<1>();                                 // the MMAs of stage i - 1 have retired: release its slot
 #pragma unroll
-      for (int g = 0; g < GK; ++g) fence_regs(acc[g]);
-      load();                 // step i + PF: its slot was last read by the MMAs of step i - 2
+      for (int sl = 0; sl < S::SL; ++sl) fence_regs(acc[sl]);
+      if (i > 0 && lane == 0) mbar_arrive(empty_bar + 8 * ((i - 1) % NS));
     }
     wgmma_wait<0>();
 #pragma unroll
-    for (int g = 0; g < GK; ++g) fence_regs(acc[g]);
+    for (int sl = 0; sl < S::SL; ++sl) fence_regs(acc[sl]);
   }
 
-  // ---- epilogue: accumulator g, fragment row m (channel of A), column n (channel of B) -> partial tile of offset k0 + g
+  // ---- epilogue: fragment row m of the stacked tile = channel m0 + m % CB of offset k0 + m / CB, column n = channel of B
 #pragma unroll
-  for (int g = 0; g < GK; ++g) {
-    if (g >= nk) break;
-    float* out = p.partial + ((int64_t)blockIdx.y * p.K + k0 + g) * (int64_t)p.Ca * p.Cb;
+  for (int sl = 0; sl < S::SL; ++sl) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = wgi * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
-      if (m >= mrows) continue;
+    for (int hh = 0; hh < 2; ++hh) {
+      const int m = (h * S::SL + sl) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * hh;
+      const int g = m / CB, ch = m0 + m % CB;
+      if (g >= nk) continue;
+      float* out = p.partial + ((int64_t)blockIdx.y * p.K + k0 + g) * (int64_t)p.Ca * p.Cb;
 #pragma unroll
       for (int c = 0; c < TN / 8; ++c) {
         const int col = n0 + c * 8 + 2 * (lane & 3);
-        const float x0 = acc[g][4 * c + 2 * h], x1 = acc[g][4 * c + 2 * h + 1];
+        const float x0 = acc[sl][4 * c + 2 * hh], x1 = acc[sl][4 * c + 2 * hh + 1];
         if (!p.transpose_out) {
-          *reinterpret_cast<float2*>(out + (int64_t)(m0 + m) * p.Cb + col) = make_float2(x0, x1);
+          *reinterpret_cast<float2*>(out + (int64_t)ch * p.Cb + col) = make_float2(x0, x1);
         } else {
-          out[(int64_t)col * p.Ca + m0 + m] = x0;
-          out[(int64_t)(col + 1) * p.Ca + m0 + m] = x1;
+          out[(int64_t)col * p.Ca + ch] = x0;
+          out[(int64_t)(col + 1) * p.Ca + ch] = x1;
         }
       }
     }
   }
 }
 
-template <int TN>
-int launch(const Args& a, int splits, cudaStream_t st) {
+template <int CB, int TN>
+int launch_cfg(const Args& a, int splits, cudaStream_t st) {
+  using S = Smem<CB, TN>;
   static bool attr_set[64] = {};          // per device: the opt-in is a per-device function attribute
-  const int mrows_max = a.Ca < WM ? a.Ca : WM;
-  // + 4 KB: the M = 64 descriptor of the upper warpgroup of a 96-channel block reads (and ignores) a few hundred bytes past the
-  // last staged chunk
-  const size_t smem = (size_t)NS * stage_bytes(mrows_max, TN) + 4096;
   const int dev_ = current_device();
   if (!attr_set[dev_]) {
-    PCB_CUDA(cudaFuncSetAttribute(wgrad_wgmma_kernel<TN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  NS * stage_bytes(WM, 128) + 4096));
+    PCB_CUDA(cudaFuncSetAttribute(wgrad_wgmma_kernel<CB, TN>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     attr_set[dev_] = true;
   }
-  const int groups = (a.K + GK - 1) / GK;
-  dim3 grid((unsigned)(groups * ((a.Ca + WM - 1) / WM) * (a.Cb / TN)), splits);
-  launch_kernel(wgrad_wgmma_kernel<TN>, grid, NTHR, smem, st, a);
+  const int groups = (a.K + S::GK - 1) / S::GK;
+  dim3 grid((unsigned)(groups * (a.Ca / CB) * (a.Cb / TN)), splits);
+  launch_kernel(wgrad_wgmma_kernel<CB, TN>, grid, NTHR, S::TOTAL, st, a);
   return check_launch("wgrad_wgmma_kernel");
+}
+
+template <int CB>
+int launch(const Args& a, int splits, int tn, cudaStream_t st) {
+  switch (tn) {
+    case 128: return launch_cfg<CB, 128>(a, splits, st);
+    case 96: return launch_cfg<CB, 96>(a, splits, st);
+    case 64: return launch_cfg<CB, 64>(a, splits, st);
+    default: return launch_cfg<CB, 32>(a, splits, st);
+  }
 }
 
 }  // namespace wg
@@ -458,11 +503,11 @@ int launch_wgrad_wgmma(const uint16_t* Ahi, const uint16_t* Alo, int lda, const 
   a.Bhi = (const __nv_bfloat16*)Bhi; a.Blo = (const __nv_bfloat16*)Blo; a.ldb = ldb;
   a.tbl = tbl; a.tbl_stride = tbl_stride; a.K = K; a.n_out = n_out; a.Ca = Ca; a.Cb = Cb; a.rows_per_split = rows_per_split;
   a.partial = partial; a.transpose_out = transpose_out;
-  switch (tn) {
-    case 128: return wg::launch<128>(a, splits, st);
-    case 96: return wg::launch<96>(a, splits, st);
-    case 64: return wg::launch<64>(a, splits, st);
-    default: return wg::launch<32>(a, splits, st);
+  switch (pick_tile(Ca)) {
+    case 128: return wg::launch<128>(a, splits, tn, st);
+    case 96: return wg::launch<96>(a, splits, tn, st);
+    case 64: return wg::launch<64>(a, splits, tn, st);
+    default: return wg::launch<32>(a, splits, tn, st);
   }
 }
 
