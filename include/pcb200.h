@@ -307,6 +307,29 @@ int pcb_nce_forward_backward(const float* q, const float* k, int64_t n, int D, f
 size_t pcb_ce_ws_bytes(int64_t n);
 int pcb_ce_forward_backward(const float* logits, const int64_t* target, int64_t n, int C, int64_t ignore_index, float grad_scale,
                             float* loss, float* dlogits, void* ws, size_t ws_bytes, void* stream);
+/* Semantic-segmentation evaluation (`downstream/semseg/lib/test.py:62-196`), accumulated on the device across calls (the caller zeroes
+ * the accumulators once); nothing synchronises.  n >= 1, 1 <= C <= 1024.
+ *
+ * pcb_seg_metrics: one pass over logits [n, C]: pred[n] = argmax, the first index among the maximal values with a NaN counting as
+ * maximal (torch `output.max(1)[1]`); prob[n, C] = exp(x - max) / sum exp(x - max), or NULL to skip it.  Then
+ *   hist[t * C + pred] += 1 (int64 [C, C]) for the rows with 0 <= t < C (`lib/utils.py:131-133` fast_hist);
+ *   stats[0] += loss * n, where loss is the mean cross-entropy over the rows with t in [0, C) and t != ignore_index -- the same bits
+ *               pcb_ce_forward_backward returns on these logits (NaN when there is no such row);
+ *   stats[1] += score * n, score = 100 * hits / rows with t != 255 in fp32 (`lib/utils.py:117-128` precision_at_one hard-codes 255);
+ *   stats[2] += n                                                            (stats: fp64 [3], the AverageMeter sums of `test.py:138-139`)
+ * ws: pcb_seg_metrics_ws_bytes(n).
+ *
+ * pcb_average_precision: per class c, sklearn's uninterpolated average precision of score[:, c] (fp32 [n, C]) against target == c (a
+ * target outside [0, C) is a negative for every class: `label_binarize` of `test.py:55-59`), sum over tie groups g of
+ * (R_g - R_{g-1}) * P_g in fp64.  A class with a positive in the batch adds its AP to ap_sum[c] (fp64) and 1 to ap_cnt[c] (int64); a
+ * class without one changes neither (its AP is NaN, left out of the reference's np.nanmean); a NaN in a column with a positive adds
+ * NaN.  n * C >= 2^31 returns PCB_ERR_ARG.  ws: pcb_average_precision_ws_bytes(n, C). */
+size_t pcb_seg_metrics_ws_bytes(int64_t n);
+int pcb_seg_metrics(const float* logits, const int64_t* target, int64_t n, int C, int64_t ignore_index, int32_t* pred, float* prob,
+                    int64_t* hist, double* stats, void* ws, size_t ws_bytes, void* stream);
+size_t pcb_average_precision_ws_bytes(int64_t n, int C);
+int pcb_average_precision(const float* score, const int64_t* target, int64_t n, int C, double* ap_sum, int64_t* ap_cnt, void* ws,
+                          size_t ws_bytes, void* stream);
 /* Row-wise L2 normalisation of the output features, y = x / ||x||_2 with no epsilon (`model/res16unet.py:262-266`), and its
  * backward dx = (dy - y (y.dy)) / ||x||.  inv_norm: [n] scratch written by forward, read by backward. */
 int pcb_l2norm_forward(const float* X, int64_t n, int C, float* Y, float* inv_norm, void* stream);

@@ -92,6 +92,10 @@ int pick_tile(int C);
 int bn_eval_stats_launch(const float* running_mean, const float* running_var, int C, float eps, float* mean, float* invstd, cudaStream_t st);
 int bn_reduce_stats_launch(const float* P, int nsplit, float* Y, int ldy, int64_t n, int64_t n0, int C, float eps, float momentum,
                            float* mean, float* invstd, float* running_mean, float* running_var, void* ws, size_t ws_bytes, cudaStream_t st);
+// loss.cu: the mean cross-entropy pass of pcb_ce_forward_backward, out[0] = sum of rowloss over the rows whose target is in [0, C) and
+// != ignore, divided by their count (fp64, fixed order, rounded to fp32), out[1] = that count.  pcb_seg_metrics (metrics.cu) runs the
+// same pass, so its evaluation loss is the training loss bit for bit.
+int ce_mean_launch(const float* rowloss, const int64_t* target, int64_t n, int C, int64_t ignore, float* out, cudaStream_t st);
 // nce_wgmma.cu: the tensor-core PointInfoNCE behind pcb_nce_forward_backward (loss.cu)
 bool nce_tc_supported(int64_t n, int D);
 size_t nce_tc_ws_bytes(int64_t n, int D);
@@ -115,6 +119,17 @@ inline void launch_kernel(void (*kernel)(Exp...), dim3 grid, dim3 block, size_t 
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
   cudaLaunchKernelEx(&cfg, kernel, static_cast<Act&&>(args)...);       // errors surface through check_launch (cudaGetLastError)
+}
+
+// One warp's row statistics of a logit row x[0, C) (lanes stride over the columns): m = the row maximum (fmaxf: NaN-free), s =
+// sum of expf(x - m).  The cross-entropy kernels (loss.cu) and the metric kernel (metrics.cu) both take lse = m + logf(s) from here.
+__device__ __forceinline__ void warp_row_max_sumexp(const float* __restrict__ x, int C, int lane, float& m, float& s) {
+  m = -INFINITY;
+  for (int c = lane; c < C; c += 32) m = fmaxf(m, x[c]);
+  for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  s = 0.f;
+  for (int c = lane; c < C; c += 32) s += expf(x[c] - m);
+  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
 }
 
 inline int current_device() { int dev = 0; cudaGetDevice(&dev); return (dev >= 0 && dev < 64) ? dev : 0; }

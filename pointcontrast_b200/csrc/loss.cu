@@ -295,12 +295,8 @@ __global__ void ce_rows_kernel(const float* __restrict__ X, const int64_t* __res
   const int64_t row = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= n) return;
   const int64_t t = target[row];
-  float m = -INFINITY;
-  for (int c = lane; c < C; c += 32) m = fmaxf(m, X[row * C + c]);
-  for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  float s = 0.f;
-  for (int c = lane; c < C; c += 32) s += expf(X[row * C + c] - m);
-  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  float m, s;
+  warp_row_max_sumexp(X + row * C, C, lane, m, s);
   if (lane == 0) {
     const float lse = m + logf(s);
     rowlse[row] = lse;
@@ -345,6 +341,11 @@ struct CeWs { float* rowloss; float* rowlse; float* stats; };
 CeWs ce_layout(Carve& c, int64_t n) { return {c.take<float>(n), c.take<float>(n), c.take<float>(2)}; }
 }  // namespace
 
+int pcb::ce_mean_launch(const float* rowloss, const int64_t* target, int64_t n, int C, int64_t ignore, float* out, cudaStream_t st) {
+  launch_kernel(ce_mean_kernel, 1, 1024, 0, st, rowloss, target, n, C, ignore, out);
+  return check_launch("ce_mean_kernel");
+}
+
 extern "C" size_t pcb_ce_ws_bytes(int64_t n) {
   return layout_bytes(ce_layout, n);
 }
@@ -358,8 +359,7 @@ extern "C" int pcb_ce_forward_backward(const float* logits, const int64_t* targe
   cudaStream_t st = (cudaStream_t)stream;
   launch_kernel(ce_rows_kernel, (unsigned)((n + 7) / 8), 256, 0, st, logits, target, n, C, ignore_index, rowloss, rowlse);
   if (int e = check_launch("ce_rows_kernel")) return e;
-  launch_kernel(ce_mean_kernel, 1, 1024, 0, st, (const float*)rowloss, target, n, C, ignore_index, stats);
-  if (int e = check_launch("ce_mean_kernel")) return e;
+  if (int e = ce_mean_launch(rowloss, target, n, C, ignore_index, stats, st)) return e;
   PCB_CUDA(cudaMemcpyAsync(loss, stats, sizeof(float), cudaMemcpyDeviceToDevice, st));
   launch_kernel(ce_grad_kernel, (unsigned)((n * C + 255) / 256), 256, 0, st, logits, target, (const float*)rowlse, (const float*)stats, n, C,
                 ignore_index, grad_scale, dlogits);

@@ -707,10 +707,32 @@ class VoxelizationLoader:
             yield [self._sub_batch() for _ in range(self.iter_size)]
 
 
+class VoxelizationPassLoader:
+    """The evaluation loader (`dataset.py:311-385` with `repeat=False`): one pass over the dataset in sampler order (a fresh permutation
+    per pass when `shuffle`), `ceil(n / batch_size)` items, the last one possibly short.  Each item is one collated (coords, feats,
+    target), colours normalised once when `normalize_color` -- what `semseg.test` takes."""
+
+    def __init__(self, dataset, batch_size, collate_fn, shuffle=False, normalize_color=False):
+        self.dataset, self.batch_size, self.collate_fn = dataset, batch_size, collate_fn
+        self.shuffle, self.normalize_color = shuffle, normalize_color
+
+    def __len__(self):
+        return (len(self.dataset) + self.batch_size - 1) // self.batch_size
+
+    def __iter__(self):
+        order = torch.randperm(len(self.dataset)).tolist() if self.shuffle else list(range(len(self.dataset)))
+        for b in range(len(self)):
+            coords, feats, target = self.collate_fn([self.dataset[i] for i in order[b * self.batch_size:(b + 1) * self.batch_size]])
+            if self.normalize_color:
+                input_transform(None, feats, normalize=True)
+            yield coords, feats, target
+
+
 def initialize_data_loader(DatasetClass, config, phase, shuffle, augment_data, batch_size, limit_numpoints, iter_size=1, normalize_color=True,
-                           input_transform=None, target_transform=None, device="cuda", draws=None, **dataset_kwargs):
-    """`dataset.py:311-385` (training, `repeat=True`): elastic distortion before voxelisation, then dropout, flip, auto-contrast,
-    colour translation and jitter (`config.augmentation.data_aug_color_trans_ratio` / `data_aug_color_jitter_std`)."""
+                           input_transform=None, target_transform=None, device="cuda", draws=None, repeat=True, **dataset_kwargs):
+    """`dataset.py:311-385`: elastic distortion before voxelisation, then dropout, flip, auto-contrast, colour translation and jitter
+    (`config.augmentation.data_aug_color_trans_ratio` / `data_aug_color_jitter_std`).  `repeat=True`: the endless training loader;
+    `repeat=False`: one pass (`VoxelizationPassLoader`, `iter_size` unused)."""
     prevoxel = [ElasticDistortion(DatasetClass.ELASTIC_DISTORT_PARAMS, draws=draws)] if augment_data else []
     transforms = list(input_transform or [])
     if augment_data:
@@ -720,5 +742,8 @@ def initialize_data_loader(DatasetClass, config, phase, shuffle, augment_data, b
     dataset = DatasetClass(config, prevoxel_transform=Compose(prevoxel) if prevoxel else None,
                            input_transform=Compose(transforms) if transforms else None, target_transform=target_transform,
                            augment_data=augment_data, phase=phase, device=device, draws=draws, **dataset_kwargs)
+    if not repeat:
+        return VoxelizationPassLoader(dataset, batch_size, cfl_collate_fn_factory(limit_numpoints), shuffle=shuffle,
+                                      normalize_color=normalize_color)
     return VoxelizationLoader(dataset, batch_size, cfl_collate_fn_factory(limit_numpoints), iter_size=iter_size, shuffle=shuffle,
                               normalize_color=normalize_color)
