@@ -330,6 +330,51 @@ int pcb_seg_metrics(const float* logits, const int64_t* target, int64_t n, int C
 size_t pcb_average_precision_ws_bytes(int64_t n, int C);
 int pcb_average_precision(const float* score, const int64_t* target, int64_t n, int C, double* ap_sum, int64_t* ap_cnt, void* ws,
                           size_t ws_bytes, void* stream);
+
+/* VoteNet detection evaluation (`downstream/votenet_det_new/models/ap_helper.py`, `lib/utils/{nms,eval_det,box_util}.py`).  Nothing
+ * synchronises.  Boxes are 8 corners fp64 [.., 8, 3] in upright-camera coordinates, built as `get_3d_box` builds them with one rounding
+ * per operation; box params fp64 [.., 8] = (center (camera), l, w, h, cos, sin).  heading_rule 0: `class2angle` returns 0 (ScanNet);
+ * 1: cls * 2 pi / H + residual, minus 2 pi above pi (SUN RGB-D).  mean_size: fp64 [S, 3] (device).
+ *
+ * pcb_det_decode_pred: per proposal of [B, K]: torch.argmax (first maximal index, NaN maximal) of heading_scores [B,K,H], size_scores
+ *   [B,K,S] and sem_cls_scores [B,K,C] (C <= 1024), the chosen residuals of heading_residuals [B,K,H] / size_residuals [B,K,S,3], the
+ *   corners and params from center [B,K,3] (depth coordinates); sem_cls int32 [B,K]; the reference's numpy fp32 softmax (fp32 exp of
+ *   x - max, numpy's pairwise row sum, one division) of sem_cls_scores -> sem_prob fp32 [B,K,C] and of objectness_scores [B,K,2] ->
+ *   obj_prob fp32 [B,K] (class 1).
+ * pcb_det_decode_gt: corners and params of labels [B, K]: center fp32 [B,K,3], heading_class int64 [B,K], heading_residual fp32 [B,K],
+ *   size_class int64 [B,K], size_residual fp32 [B,K,3].  A size class outside [0, S) (or heading class outside [0, H) under rule 1)
+ *   ORs PCB_ERR_RANGE into status (device int32, caller-zeroed) and leaves that box unwritten.
+ * pcb_det_points_in_box: counts int32 [B, K] = the points of points fp32 [B, N, ld] (xyz in the first 3 of ld channels, depth
+ *   coordinates) inside each box of box params [B, K, 8] (|local coordinate| <= half size, fp64; a point within 1e-9 of a face is
+ *   unpinned).  Zeroes counts itself.  ceil(N / 4096) > 65535 returns PCB_ERR_ARG.
+ * pcb_det_nms: pred_mask int32 [B, K] = 1 on the proposals greedy NMS keeps among those with counts >= min_points (all when counts is
+ *   NULL), scores fp32 [B, K], in the order of descending score, ties larger proposal index first.  mode 0: `nms_2d_faster` (camera x /
+ *   z extents of the corners), 1: `nms_3d_faster`, 2: `nms_3d_faster_samecls` (sem_cls int32 [B, K]); old_type: overlap over the
+ *   other box's area.  Overlaps are fp64 in the reference's expression order; a NaN overlap never suppresses.  A NaN score ranks above
+ *   every number (np.argsort sorts it last, so it is picked first); -0.0 ties +0.0.  K <= 1024.
+ * pcb_det_box_iou: iou fp64 [n] = `box3d_iou(corners1[i], corners2[i])[0]`, the IoU pcb_det_ap uses (see below), n >= 1.
+ * pcb_det_ap: VOC average precision (`eval_det_cls`, `voc_ap`) for T <= 64 IoU thresholds (host fp64 [T]) at once.  Detections d < D:
+ *   proposal row det_row (into prop_corners [P, 8, 3]), class det_cls, score det_score (fp32), scan det_scan; a class outside [0, C)
+ *   marks a slot that is not a detection.  Ground truth g < G: gt_corners [G, 8, 3], gt_scan, gt_cls (outside [0, C): ignored).  Within
+ *   a class detections rank by descending score, ties in input order (a stable sort); ground truth of one (scan, class) keeps input
+ *   order for the first-maximal-j rule.  IoU is `box3d_iou` (Sutherland-Hodgman, convex-hull area, degenerate clips area 0), a NaN IoU
+ *   never matching.  out fp64 [T, C, 4] = (AP, final recall, npos, ndet): AP and recall NaN for a class with detections but no ground
+ *   truth, 0 for one with ground truth but no detections.  D, G, P, C >= 1, C <= 1024.  ws: pcb_det_ap_ws_bytes(D, G, C, T). */
+int pcb_det_decode_pred(const float* center, const float* heading_scores, const float* heading_residuals, const float* size_scores,
+                        const float* size_residuals, const float* sem_cls_scores, const float* objectness_scores, int64_t B, int64_t K,
+                        int H, int S, int C, const double* mean_size, int heading_rule, double* corners, double* box, int32_t* sem_cls,
+                        float* obj_prob, float* sem_prob, void* stream);
+int pcb_det_decode_gt(const float* center, const int64_t* heading_class, const float* heading_residual, const int64_t* size_class,
+                      const float* size_residual, int64_t B, int64_t K, int H, int S, const double* mean_size, int heading_rule,
+                      double* corners, double* box, int32_t* status, void* stream);
+int pcb_det_points_in_box(const float* points, int64_t B, int64_t N, int ld, const double* box, int64_t K, int32_t* counts, void* stream);
+int pcb_det_nms(const double* corners, const float* score, const int32_t* sem_cls, const int32_t* counts, int min_points, int64_t B,
+                int64_t K, int mode, int old_type, double nms_iou, int32_t* pred_mask, void* stream);
+int pcb_det_box_iou(const double* corners1, const double* corners2, int64_t n, double* iou, void* stream);
+size_t pcb_det_ap_ws_bytes(int64_t D, int64_t G, int C, int T);
+int pcb_det_ap(const double* prop_corners, int64_t P, const int32_t* det_row, const int32_t* det_cls, const float* det_score,
+               const int32_t* det_scan, int64_t D, const double* gt_corners, const int32_t* gt_scan, const int32_t* gt_cls, int64_t G, int C,
+               const double* thresholds, int T, double* out, void* ws, size_t ws_bytes, void* stream);
 /* Row-wise L2 normalisation of the output features, y = x / ||x||_2 with no epsilon (`model/res16unet.py:262-266`), and its
  * backward dx = (dy - y (y.dy)) / ||x||.  inv_norm: [n] scratch written by forward, read by backward. */
 int pcb_l2norm_forward(const float* X, int64_t n, int C, float* Y, float* inv_norm, void* stream);

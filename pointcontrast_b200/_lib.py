@@ -80,6 +80,13 @@ _SIGS = {
     "pcb_seg_metrics": (_i, [_p, _p, _l, _i, _l, _p, _p, _p, _p, _p, _sz, _p]),
     "pcb_average_precision_ws_bytes": (_sz, [_l, _i]),
     "pcb_average_precision": (_i, [_p, _p, _l, _i, _p, _p, _p, _sz, _p]),
+    "pcb_det_decode_pred": (_i, [_p, _p, _p, _p, _p, _p, _p, _l, _l, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p]),
+    "pcb_det_decode_gt": (_i, [_p, _p, _p, _p, _p, _l, _l, _i, _i, _p, _i, _p, _p, _p, _p]),
+    "pcb_det_points_in_box": (_i, [_p, _l, _l, _i, _p, _l, _p, _p]),
+    "pcb_det_nms": (_i, [_p, _p, _p, _p, _i, _l, _l, _i, _i, _d, _p, _p]),
+    "pcb_det_box_iou": (_i, [_p, _p, _l, _p, _p]),
+    "pcb_det_ap_ws_bytes": (_sz, [_l, _l, _i, _i]),
+    "pcb_det_ap": (_i, [_p, _l, _p, _p, _p, _p, _l, _p, _p, _p, _l, _i, _p, _i, _p, _p, _sz, _p]),
     "pcb_profile_enable": (_i, [_i]),
     "pcb_profile_read": (_i, [_p, _p, _i, C.POINTER(C.c_int)]),
     "pcb_unit_ws_bytes": (_sz, [_i, _l, _l, _i, _i]),
