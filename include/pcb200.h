@@ -104,6 +104,34 @@ int pcb_voxelize(const float* xyz, int64_t n, float voxel_size, int32_t* out_coo
 size_t pcb_radius_pairs_ws_bytes(int64_t ns, int64_t nd);
 int pcb_radius_pairs(const float* src, int64_t ns, const float* dst, int64_t nd, float radius, int32_t* pairs, int64_t cap,
                      int64_t* n_pairs, void* ws, size_t ws_bytes, void* stream);
+/* The pretraining pair list of a scan (`pretrain/data_preprocess/scannet_pair/compute_full_overlapping.py`, SURVEY.md 8f-10).  A scene
+ * is one ragged batch of F frames, 1 <= F <= 4096: xyz fp64 [n, 3], frame f is rows [offsets[f], offsets[f+1]) (device int64 [F + 1],
+ * non-decreasing from 0 to n).
+ *
+ * pcb_voxel_down_sample: open3d `PointCloud.voxel_down_sample` of every frame (`:15-26`, `:59-63`).  Per frame lo = min(points) -
+ * voxel_size * 0.5 per axis, voxel index floor((p - lo) / voxel_size) (fp64, one rounding per operation, < 2^17 per axis); one output
+ * point per occupied voxel, the fp64 sum of its points in ascending input index divided by their number.  Rows frame-major, ascending
+ * (x, y, z) voxel index within a frame; out holds up to n rows.  out_offsets (device [F + 1]) delimit the frames of the output; SYNCHRONISES
+ * once and copies them to out_offsets_host (host, F + 1 entries).  A non-finite coordinate or a voxel index >= 2^17 returns PCB_ERR_RANGE;
+ * offsets that do not run from 0 to n return PCB_ERR_ARG (both found after the launches).  An empty frame has no output rows.
+ *
+ * pcb_frame_overlap: counts[i * F + j] (int64 [F, F], written in full, diagonal 0) = the number of points q of frame j with at least one
+ * point p of frame i != j at ((dx dx + dy dy) + dz dz) < radius * radius in fp64 without FMA contraction -- the length of
+ * `get_matching_indices(pcd_j, tree_i, radius, K=1)` (`:39-47`, `:67-74`).  One hashed grid of cell size radius (1 + 2^-20) over all
+ * frames.  status (device int32, caller-zeroed) receives bits: PCB_FRAMES_RANGE if a point's cell index lies outside +-2^20 (or it is
+ * not finite; that point matches nothing), PCB_FRAMES_OFFSETS if the offsets do not run from 0 to n without decreasing (the counts are
+ * then meaningless, though nothing outside the arrays is read).  Does not synchronise.
+ *
+ * Both: n < 0, F outside [1, 4096], voxel_size / radius not positive and finite, NULL pointers (xyz / out may be NULL when n == 0) and
+ * a short workspace return PCB_ERR_ARG before anything is launched. */
+#define PCB_FRAMES_RANGE 1
+#define PCB_FRAMES_OFFSETS 2
+size_t pcb_voxel_down_sample_ws_bytes(int64_t n, int64_t F);
+int pcb_voxel_down_sample(const double* xyz, int64_t n, const int64_t* offsets, int64_t F, double voxel_size, double* out, int64_t* out_offsets,
+                          int64_t* out_offsets_host, void* ws, size_t ws_bytes, void* stream);
+size_t pcb_frame_overlap_ws_bytes(int64_t n, int64_t F);
+int pcb_frame_overlap(const double* xyz, int64_t n, const int64_t* offsets, int64_t F, double radius, int64_t* counts, int32_t* status,
+                      void* ws, size_t ws_bytes, void* stream);
 
 /* ----------------------------------------------------------------------------------------------- semseg training data (8f-6) */
 /* Label-aware voxelisation of integer coordinates (int32 [N,3], |c| < 2^20): the M occupied voxels in ascending (x,y,z) order

@@ -106,6 +106,10 @@ _SIGS = {
     "pcb_furthest_point_sampling_ragged_ws_bytes": (_sz, [_l, _l, _l]),
     "pcb_furthest_point_sampling_ragged": (_i, [_p, _p, _l, _l, _l, _l, _p, _p, _sz, _p]),
     "pcb_gather_rows_grad": (_i, [_p, _p, _l, _l, _l, _p, _p, _sz, _p]),
+    "pcb_voxel_down_sample_ws_bytes": (_sz, [_l, _l]),
+    "pcb_voxel_down_sample": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _p, _sz, _p]),
+    "pcb_frame_overlap_ws_bytes": (_sz, [_l, _l]),
+    "pcb_frame_overlap": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _sz, _p]),
 }
 
 
@@ -138,6 +142,8 @@ class PcbUnit(C.Structure):
         ("ws", _p), ("ws_bytes", _sz),
         ("flags", C.c_int32),
     ]
+# status bits of pcb_frame_overlap (include/pcb200.h)
+FRAMES_RANGE, FRAMES_OFFSETS = 1, 2
 EXPORTS = sorted(_SIGS)
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)          # AttributeError here == the library does not export a declared symbol

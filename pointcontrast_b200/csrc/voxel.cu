@@ -18,16 +18,11 @@ using namespace pcb;
 
 namespace {
 
-constexpr int VB = 1 << 20;      // voxel / cell index bias: |index| < 2^20 per axis, 21 bits each
-
 __device__ __forceinline__ bool cell_of(float x, float y, float z, float inv_unused, float size, int& cx, int& cy, int& cz) {
   // floor(v / size) in fp32, exactly what numpy does on float32 input (IEEE division, then floor)
   const float fx = floorf(x / size), fy = floorf(y / size), fz = floorf(z / size);
   cx = (int)fx; cy = (int)fy; cz = (int)fz;
   return fabsf(fx) < (float)VB && fabsf(fy) < (float)VB && fabsf(fz) < (float)VB;
-}
-__device__ __forceinline__ uint64_t cell_key(int cx, int cy, int cz) {
-  return ((uint64_t)(cx + VB) << 42) | ((uint64_t)(cy + VB) << 21) | (uint64_t)(cz + VB);
 }
 
 __global__ void point_key_kernel(const float* __restrict__ xyz, int64_t n, float size, uint64_t* __restrict__ keys, int32_t* __restrict__ idx,
@@ -161,6 +156,26 @@ int sort_runs(int64_t n, const SortWs& w, int end_bit, cudaStream_t st) {
   return PCB_OK;
 }
 
+RunsWs runs_layout(Carve& c, int64_t n, bool hashed) {
+  RunsWs r{c.take<uint64_t>(n), c.take<int32_t>(n), c.take<int32_t>(n), 0, nullptr, nullptr};
+  if (hashed) {
+    r.tcap = 16;
+    while (r.tcap < 2 * n) r.tcap <<= 1;
+    r.tk = c.take<uint64_t>(r.tcap);
+    r.tv = c.take<int32_t>(r.tcap);
+  }
+  return r;
+}
+
+int find_runs(int64_t n, const SortWs& w, const RunsWs& r, cudaStream_t st) {
+  run_bounds_kernel<<<blocks_for(n, 256), 256, 0, st>>>(w.sk, w.rank, n, r.key, r.start, r.end, w.count);
+  if (int e = check_launch("run_bounds_kernel")) return e;
+  if (!r.tk) return PCB_OK;
+  PCB_CUDA(cudaMemsetAsync(r.tk, 0xFF, (size_t)r.tcap * 8, st));
+  run_insert_kernel<<<blocks_for(n, 256), 256, 0, st>>>(r.key, w.count, r.tk, r.tv, (uint64_t)r.tcap - 1);
+  return check_launch("run_insert_kernel");
+}
+
 }  // namespace pcb
 
 namespace {
@@ -243,17 +258,11 @@ SortWs scenes_layout(Carve& c, int64_t B, int64_t N, int64_t*& stage) {
   return w;
 }
 
-// the cell sort of the targets, their runs, the hash table of the runs (a power of two >= 2 nd slots), per-source counts / offsets
-struct PairsWs {
-  SortWs s; uint64_t* run_key; int32_t* run_start; int32_t* run_end; int64_t tcap; uint64_t* tk; int32_t* tv; int32_t* cnt; int64_t* off;
-  void* cub; size_t cub_bytes;
-};
+// the cell sort of the targets, their runs and the hash table of the runs, per-source counts / offsets
+struct PairsWs { SortWs s; RunsWs r; int32_t* cnt; int64_t* off; void* cub; size_t cub_bytes; };
 PairsWs pairs_layout(Carve& c, int64_t ns, int64_t nd) {
-  int64_t tcap = 16;
-  while (tcap < 2 * nd) tcap <<= 1;
   const size_t cub_bytes = sort_scan_bytes(ns);
-  return {sort_layout(c, nd), c.take<uint64_t>(nd), c.take<int32_t>(nd), c.take<int32_t>(nd), tcap, c.take<uint64_t>(tcap),
-          c.take<int32_t>(tcap), c.take<int32_t>(ns), c.take<int64_t>(ns), c.take<char>(cub_bytes), cub_bytes};
+  return {sort_layout(c, nd), runs_layout(c, nd, true), c.take<int32_t>(ns), c.take<int64_t>(ns), c.take<char>(cub_bytes), cub_bytes};
 }
 
 }  // namespace
@@ -361,13 +370,9 @@ extern "C" int pcb_radius_pairs(const float* src, int64_t ns, const float* dst, 
   PCB_ARG(src && dst && ws && ws_bytes >= c.used);
   cudaStream_t st = (cudaStream_t)stream;
   if (int e = sort_cells(dst, nd, radius, w.s, st)) return e;
-  const uint64_t mask = (uint64_t)w.tcap - 1;
-  run_bounds_kernel<<<blocks_for(nd, 256), 256, 0, st>>>(w.s.sk, w.s.rank, nd, w.run_key, w.run_start, w.run_end, w.s.count);
-  if (int e = check_launch("run_bounds_kernel")) return e;
-  PCB_CUDA(cudaMemsetAsync(w.tk, 0xFF, (size_t)w.tcap * 8, st));
-  run_insert_kernel<<<blocks_for(nd, 256), 256, 0, st>>>(w.run_key, w.s.count, w.tk, w.tv, mask);
-  if (int e = check_launch("run_insert_kernel")) return e;
-  radius_kernel<false><<<blocks_for(ns, 128), 128, 0, st>>>(src, ns, dst, radius, w.tk, w.tv, mask, w.run_start, w.run_end, w.s.sidx, w.cnt,
+  if (int e = find_runs(nd, w.s, w.r, st)) return e;
+  const uint64_t mask = (uint64_t)w.r.tcap - 1;
+  radius_kernel<false><<<blocks_for(ns, 128), 128, 0, st>>>(src, ns, dst, radius, w.r.tk, w.r.tv, mask, w.r.start, w.r.end, w.s.sidx, w.cnt,
                                                             nullptr, nullptr, 0);
   if (int e = check_launch("radius_kernel<count>")) return e;
   size_t cb = w.cub_bytes;
@@ -379,7 +384,7 @@ extern "C" int pcb_radius_pairs(const float* src, int64_t ns, const float* dst, 
   PCB_CUDA(cudaStreamSynchronize(st));
   *n_pairs = last_off + last_cnt;
   if (!pairs || cap <= 0) return PCB_OK;
-  radius_kernel<true><<<blocks_for(ns, 128), 128, 0, st>>>(src, ns, dst, radius, w.tk, w.tv, mask, w.run_start, w.run_end, w.s.sidx, w.cnt,
+  radius_kernel<true><<<blocks_for(ns, 128), 128, 0, st>>>(src, ns, dst, radius, w.r.tk, w.r.tv, mask, w.r.start, w.r.end, w.s.sidx, w.cnt,
                                                            w.off, pairs, cap);
   return check_launch("radius_kernel<fill>");
 }

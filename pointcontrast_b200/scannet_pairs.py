@@ -1,6 +1,7 @@
 """ScanNet frame-pair data path (SURVEY.md 8f-2 / 8f-3): the on-disk formats of the reference's preprocessing --
 `<scene>/pcd/<frame>.npz` holding `pcd` = world-frame points [N,3] (`pretrain/data_preprocess/scannet_pair/point_cloud_extractor.py:80`)
-and the pair list `overlap-30-full.txt` with lines `<file0> <file1> <overlap>` (`generate_list.py:20-28`) -- and a mirror of
+and the pair list `overlap-30-full.txt` with lines `<file0> <file1> <overlap>` (`generate_list.py:20-28`; this repository writes it
+with `pair_list.compute_full_overlapping` + `pair_list.generate_list`, or `python -m pointcontrast_b200.pair_list`) -- and a mirror of
 `ScanNetMatchPairDataset` / `default_collate_pair_fn` / the infinite samplers (`lib/ddp_data_loaders.py:52-265`,
 `lib/data_sampler.py:13-70`) whose per-sample work (voxelisation, correspondence search) runs on the GPU (`voxel.make_pair`)
 instead of `ME.utils.sparse_quantize` + one open3d KD-tree query per point on CPU workers.

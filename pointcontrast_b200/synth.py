@@ -183,6 +183,52 @@ def synth_votenet_batch(seed, batch_size, num_points, scale=1.5):
     return out
 
 
+def synth_scan_frames(seed, n_frames, points_per_frame=250_000, scale=2.0, half_angle_deg=30.0):
+    """A depth-camera walk through a `synth_room`-style room (at `scale`): n_frames fp64 [points_per_frame, 3] world-frame clouds, the
+    `pcd` of ScanNet's `<scene>/pcd/<frame>.npz` (about 250k points, like a 640x480 depth frame).  Frame k casts rays uniformly over a
+    view cone of `half_angle_deg` from pose k and keeps the nearest surface each ray hits (the room closed by its two other walls, so
+    every ray hits one), + N(0, 5 mm) noise.  The camera circles the room centre at 60 % of the wall height, looking 20 degrees down, and turns
+    10-50 degrees between frames, so consecutive frames overlap by amounts on both sides of the pair list's 0.3 threshold."""
+    rng = np.random.default_rng(seed)
+    rects = _rects() + [tuple(np.asarray(a, np.float64) for a in r) for r in (((_W, 0, 0), (0, _L, 0), (0, 0, _H)),      # wall x=W
+                                                                                ((0, _L, 0), (_W, 0, 0), (0, 0, _H)))]     # wall y=L
+    O, U, V = (np.stack([r[k] for r in rects]) * scale for k in range(3))
+    N = np.cross(U, V)
+    uu, vv = np.einsum("ij,ij->i", U, U), np.einsum("ij,ij->i", V, V)
+    centre = np.array([_W / 2, _L / 2, 0.6 * _H]) * scale
+    cos_half = np.cos(np.deg2rad(half_angle_deg))
+    yaw, phase = rng.random() * 2 * np.pi, rng.random() * 2 * np.pi
+    frames = []
+    for _ in range(n_frames):
+        pos = centre + np.array([0.2 * _W * np.cos(phase), 0.2 * _L * np.sin(phase), 0.0]) * scale
+        look = np.array([np.cos(yaw), np.sin(yaw), -np.tan(np.deg2rad(20.0))])
+        look /= np.linalg.norm(look)
+        side = np.cross(look, [0.0, 0.0, 1.0])
+        side /= np.linalg.norm(side)
+        up = np.cross(side, look)
+        got, parts, frac = 0, [], 0.5
+        while got < points_per_frame:
+            m = int(1.2 * (points_per_frame - got) / frac) + 1024
+            c = 1.0 - rng.random(m) * (1.0 - cos_half)                      # uniform over the cone's solid angle
+            s, phi = np.sqrt(1.0 - c * c), rng.random(m) * 2 * np.pi
+            d = c[:, None] * look + (s * np.cos(phi))[:, None] * side + (s * np.sin(phi))[:, None] * up
+            with np.errstate(divide="ignore", invalid="ignore"):
+                t = ((O - pos) * N).sum(1) / (d @ N.T)                      # [m, rects]: the ray's parameter at each plane
+                a = (((pos - O) * U).sum(1) + t * (d @ U.T)) / uu           # the hit point in the rectangle's (u, v) coordinates
+                b = (((pos - O) * V).sum(1) + t * (d @ V.T)) / vv
+                t = np.where((t > 0) & (a >= 0) & (a <= 1) & (b >= 0) & (b <= 1), t, np.inf)
+            tmin = t.min(1)
+            keep = np.isfinite(tmin)
+            frac = max(keep.mean(), 0.5)
+            parts.append(pos + tmin[keep, None] * d[keep])
+            got += int(keep.sum())
+        pts = np.concatenate(parts)[:points_per_frame]
+        frames.append(pts + rng.normal(0.0, 0.005, size=pts.shape))
+        yaw += np.deg2rad(rng.uniform(10.0, 50.0))
+        phase += np.deg2rad(rng.uniform(5.0, 20.0))
+    return frames
+
+
 def synth_scene(seed, scale=2.5, voxel=0.05, n_raw=1_500_000):
     """S3DIS-shaped single room for the forward-only config (C4): coords [N,4], RGB/255-0.5 features."""
     rng = np.random.default_rng(seed + 99)
