@@ -401,7 +401,8 @@ extern "C" int pcb_bn_apply_seg(const float* X, int ldx, int64_t n, int64_t n0, 
                                 const float* gamma, const float* beta, const float* residual, int ldr, int flags, float* Y, int ldy,
                                 uint16_t* Yhi, uint16_t* Ylo, int lds, uint16_t* Ybhi, uint16_t* Yblo, void* stream) {
   const int relu = flags & PCB_BN_RELU;
-  PCB_ARG(n >= 0 && n0 >= 0 && n0 <= n && C >= 4 && C % 4 == 0 && ldx % 4 == 0 && ldx >= C && (!Y || (ldy % 4 == 0 && ldy >= C)));
+  // n0 == 0 < n would normalise every row with mean[1] / invstd[1], which no statistics call writes (they require n0 >= 1)
+  PCB_ARG(n >= 0 && (n0 >= 1 || n == 0) && n0 <= n && C >= 4 && C % 4 == 0 && ldx % 4 == 0 && ldx >= C && (!Y || (ldy % 4 == 0 && ldy >= C)));
   if (n == 0) return PCB_OK;
   PCB_ARG(X && (Y || Yhi) && mean && invstd && gamma && beta && (!residual || (ldr >= C && ldr % 4 == 0)));
   PCB_ARG(!Yhi || (Ylo && lds >= C && lds % 4 == 0));
