@@ -93,6 +93,7 @@ extern "C" int pcb_unit_forward(const pcb_unit* u, void* stream) {
   PCB_ARG(u && u->K >= 1 && u->K <= PCB_MAX_KERNEL_VOLUME && u->n_out >= 1 && u->n_in >= 1 && u->n0 >= 1 && u->n0 <= u->n_out);
   PCB_ARG(u->fwd_tbl && u->z_p && u->out_hi && u->out_lo && u->mean && u->invstd && u->gamma && u->beta && u->ws);
   PCB_ARG(!(u->flags & PCB_UNIT_FP16_FORWARD) || (u->flags & PCB_UNIT_EVAL) || (u->out_bhi && u->out_blo));
+  PCB_ARG(!(u->flags & PCB_UNIT_EVAL) || (u->n0 == u->n_out && u->running_mean && u->running_var));
   Carve c{(char*)u->ws};
   const UnitWs w = unit_layout(c, u->K, u->n_in, u->n_out, u->Cin, u->Cout);
   PCB_ARG(u->ws_bytes >= c.used);
@@ -121,7 +122,6 @@ extern "C" int pcb_unit_forward(const pcb_unit* u, void* stream) {
   }
   ProfScope prof(st, 2);                     // BatchNorm forward: statistics (unless fused into the split reduction) + normalise / residual / ReLU / planes
   if (u->flags & PCB_UNIT_EVAL) {            // eval-mode BatchNorm (`downstream/semseg/lib/test.py:95-117`): normalise with the running statistics
-    PCB_ARG(u->n0 == u->n_out && u->running_mean && u->running_var);
     if (int e = bn_eval_stats_launch(u->running_mean, u->running_var, u->Cout, u->eps, u->mean, u->invstd, st)) return e;
   } else if (!partials) {
     if (int e = pcb_bn_stats_seg(u->z_p, u->z_ld, u->n_out, u->n0, u->Cout, u->eps, u->momentum, u->mean, u->invstd, u->running_mean,
@@ -142,6 +142,14 @@ extern "C" int pcb_unit_backward(const pcb_unit* u, void* stream) {
   const bool f16 = (u->flags & PCB_UNIT_FP16_FORWARD) != 0;
   PCB_ARG(tc ? (u->dz_hi && u->dz_lo && u->x_hi && u->x_lo) : (u->dz_p && u->x_p));
   PCB_ARG(tc || u->gin_mode == 0);               // only the 3-channel stem is not tensor-core shaped: its input wants no gradient
+  // the activation operand of the weight gradient as bf16 hi/lo planes (its fp16 planes serve the forward pass only): both MMA operands
+  // share one format
+  const uint16_t* xh = f16 ? u->x_bhi : u->x_hi;
+  const uint16_t* xl = f16 ? u->x_blo : u->x_lo;
+  PCB_ARG(!tc || (xh && xl));
+  PCB_ARG(tc || u->wg_gather_x);
+  PCB_ARG(u->gin_mode == 0 || (u->gin_p && u->dg_tbl && u->wt_dg));
+  // every argument is checked above: a rejected call leaves dz, dgamma / dbeta, gres, dW and gin as they were
   cudaStream_t st = (cudaStream_t)stream;
   // 1. g * (out > 0) -> BatchNorm backward -> dz (split planes), residual-gradient fan-out, dgamma / dbeta accumulated
   prof_begin(st);
@@ -151,23 +159,17 @@ extern "C" int pcb_unit_backward(const pcb_unit* u, void* stream) {
   prof_end(st, 3);
   // 2. weight gradient, accumulated into dW (the flat parameter-gradient buffer)
   if (tc) {
-    // the activation operand as bf16 hi/lo planes (its fp16 planes serve the forward pass only): both MMA operands share one format
-    const uint16_t* xh = f16 ? u->x_bhi : u->x_hi;
-    const uint16_t* xl = f16 ? u->x_blo : u->x_lo;
-    PCB_ARG(xh && xl);
     const uint16_t *Ahi, *Alo, *Bhi, *Blo; int lda, ldb, Ca, Cb, tr; int64_t rows;
     if (u->wg_gather_x) { Ahi = xh; Alo = xl; lda = u->x_lds; Bhi = u->dz_hi; Blo = u->dz_lo; ldb = u->dz_ld; Ca = u->Cin; Cb = u->Cout; tr = 0; rows = u->n_out; }
     else { Ahi = u->dz_hi; Alo = u->dz_lo; lda = u->dz_ld; Bhi = xh; Blo = xl; ldb = u->x_lds; Ca = u->Cout; Cb = u->Cin; tr = 1; rows = u->n_in; }
     if (int e = pcb_conv_wgrad_split(Ahi, Alo, lda, Bhi, Blo, ldb, u->wg_tbl, u->wg_stride, u->K, rows, Ca, Cb, u->dW, tr, w.conv, w.conv_bytes,
                                      PCB_CONV_ACCUMULATE, stream)) return e;
   } else {
-    PCB_ARG(u->wg_gather_x);
     if (int e = pcb_conv_wgrad(u->x_p, u->x_ld, u->dz_p, u->dz_ld, u->wg_tbl, u->wg_stride, u->K, u->n_out, u->Cin, u->Cout, u->dW, 0, w.conv,
                                w.conv_bytes, PCB_CONV_ACCUMULATE, stream)) return e;
   }
   // 3. data gradient: the forward kernel on the data-gradient weight tiles and the opposite-offset table
   if (u->gin_mode) {
-    PCB_ARG(u->gin_p && u->dg_tbl && u->wt_dg);
     if (int e = pcb_conv_forward_split(u->dz_hi, u->dz_lo, u->dz_ld, u->dg_tbl, u->dg_stride, u->dg_kmap, u->K, u->n_in, u->Cout, u->Cin, u->wt_dg,
                                        nullptr, u->gin_p, u->gin_ld, w.conv, w.conv_bytes, u->gin_mode == 2 ? PCB_CONV_ACCUMULATE : 0, stream)) return e;
   }
