@@ -38,16 +38,18 @@ struct Args {
   float out_scale;      // applied to the accumulators on the way out (2^-10 when the weight tiles hold fp16(W * 2^10))
 };
 
-// The ring takes every slot that fits beside the table slice in the CTA's share of shared memory.  BN = 128 and 96 run one CTA per
-// SM, with 6 and 7 slots.  BN = 64 and 32 run two CTAs per SM with 4 slots each: on an H100 that beat one CTA with 8 and 10 slots
-// at every BN <= 64 layer shape of the C1 training step (up to 22 % less kernel time, 0.65 ms less per step).
+// The ring takes every slot that fits beside the table slice in the CTA's share of shared memory.  BN = 128 runs one CTA per SM with
+// 6 slots.  BN = 96, 64 and 32 run two CTAs per SM with 3, 4 and 4 slots each: on an H100 that beat one CTA with 7, 8 and 10 slots
+// at the C1 training step's layer shapes (BN <= 64: up to 22 % less kernel time, 0.65 ms less per step; BN = 96: 1.3 ms less
+// kernel time per step, DESIGN.md section 7).  While one CTA loads its table slice, fills its ring or writes its tile out, the
+// other keeps the tensor cores busy.  BN = 128 stays at one CTA: its consumers need 90 registers, above the 85 of two CTAs.
 template <int BN>
 struct Smem {
   static constexpr int B_SBO = 128;
   static constexpr int B_LBO = (BN / 8) * 128 + 16;
   static constexpr int B_PLANE = (BK / 8) * B_LBO;
   static constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
-  static constexpr int CTAS = BN <= 64 ? 2 : 1;                                  // resident CTAs per SM
+  static constexpr int CTAS = BN <= 96 ? 2 : 1;                                  // resident CTAs per SM
   static constexpr int BUDGET = CTAS == 1 ? SMEM_OPTIN : SMEM_PER_SM / 2 - 1024;  // 1 KB per CTA is reserved by the system
   static constexpr int FIXED = PCB_MAX_KERNEL_VOLUME * BM * 4 + 72 * 4 + 16;
   static constexpr int NS = (BUDGET - FIXED) / (STAGE + 16);                      // + full and empty barrier per slot
