@@ -133,6 +133,32 @@ size_t pcb_frame_overlap_ws_bytes(int64_t n, int64_t F);
 int pcb_frame_overlap(const double* xyz, int64_t n, const int64_t* offsets, int64_t F, double radius, int64_t* counts, int32_t* status,
                       void* ws, size_t ws_bytes, void* stream);
 
+/* ----------------------------------------------------------------------------------------------- semseg on the original point cloud */
+/* The label transfer of `test_pointcloud` (`downstream/semseg/lib/datasets/scannet.py:131-172`, `stanford.py:41-84`): a scipy KD-tree
+ * query of every original point against the predicted voxel centres, then `fast_hist` (`lib/utils.py:131-133`).
+ *
+ * pcb_nearest: idx[i] (int32 [n]) = the smallest j in [0, m) whose d2 = ((dx dx + dy dy) + dz dz) (fp64, no FMA contraction) between
+ * ref[j] and query[i] (fp64 [m, 3], [n, 3]) is the minimum over all j.  A hashed grid of cell size cell_size over the references, searched
+ * in Chebyshev shells around the query's cell with an exact stop rule; a query not settled within 8 shells is compared with every
+ * reference.  The result does not depend on cell_size (which only sets the speed), the launch shape or ws_bytes.  status (device int32,
+ * caller-zeroed) receives PCB_NEAREST_RANGE if a coordinate is not finite or its cell lies outside +-2^20 (that query gets idx -1; the
+ * other results are then meaningless).  Does not synchronise.  n == 0 returns at once; m == 0 < n, m or n >= 2^31 - 1, cell_size not
+ * positive and finite, NULL pointers and a short workspace return PCB_ERR_ARG before anything is launched.
+ *
+ * pcb_label_transfer: point_label[i] = ref_label[idx[i]] (int32 [n]; ref_label int32 [m]).  With query_label (int32 [n], may be NULL): gt = lut[query_label[i]],
+ * pred = lut[point_label[i]] (lut: device int32 [lut_n], original -> masked label, -1 for no entry), and for 0 <= gt < C
+ * hist[gt * C + pred] += 1 (int64 [C, C], accumulated; the caller zeroes it).  status receives PCB_LABEL_RANGE if a label lies outside
+ * the table, has no entry, or a counted pred lies outside [0, C) (the reference's KeyError / IndexError), PCB_NEAREST_RANGE if an idx
+ * lies outside [0, m) (that row gets point_label -1 and is not counted).  Does not synchronise.  m or n outside [0, 2^31 - 1), and with
+ * query_label C outside [1, 46340], lut_n < 1 or NULL lut / hist, return PCB_ERR_ARG before the launch. */
+#define PCB_NEAREST_RANGE 1
+#define PCB_LABEL_RANGE 2
+size_t pcb_nearest_ws_bytes(int64_t m, int64_t n);
+int pcb_nearest(const double* ref, int64_t m, const double* query, int64_t n, double cell_size, int32_t* idx, int32_t* status, void* ws,
+                size_t ws_bytes, void* stream);
+int pcb_label_transfer(const int32_t* idx, const int32_t* ref_label, int64_t m, const int32_t* query_label, int64_t n, const int32_t* lut,
+                       int lut_n, int C, int32_t* point_label, int64_t* hist, int32_t* status, void* stream);
+
 /* ----------------------------------------------------------------------------------------------- semseg training data (8f-6) */
 /* Label-aware voxelisation of integer coordinates (int32 [N,3], |c| < 2^20): the M occupied voxels in ascending (x,y,z) order
  * (out_coords int32 [M,3]), sel[M] = the smallest index of a point in the voxel, out_labels[M] = the label all of the voxel's points

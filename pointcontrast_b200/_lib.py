@@ -110,6 +110,9 @@ _SIGS = {
     "pcb_voxel_down_sample": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _p, _sz, _p]),
     "pcb_frame_overlap_ws_bytes": (_sz, [_l, _l]),
     "pcb_frame_overlap": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _sz, _p]),
+    "pcb_nearest_ws_bytes": (_sz, [_l, _l]),
+    "pcb_nearest": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _sz, _p]),
+    "pcb_label_transfer": (_i, [_p, _p, _l, _p, _l, _p, _i, _i, _p, _p, _p, _p]),
 }
 
 
@@ -144,6 +147,8 @@ class PcbUnit(C.Structure):
     ]
 # status bits of pcb_frame_overlap (include/pcb200.h)
 FRAMES_RANGE, FRAMES_OFFSETS = 1, 2
+# status bits of pcb_nearest / pcb_label_transfer (include/pcb200.h)
+NEAREST_RANGE, LABEL_RANGE = 1, 2
 EXPORTS = sorted(_SIGS)
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)          # AttributeError here == the library does not export a declared symbol

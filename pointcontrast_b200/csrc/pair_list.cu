@@ -125,20 +125,12 @@ DownWs down_layout(Carve& c, int64_t n, int64_t F) {
   return w;
 }
 
-// cell = floor(p / cell_size) per axis in fp64; false outside +-2^20 (also for a non-finite coordinate)
-__device__ __forceinline__ bool cell_of(const double* __restrict__ p, double cell_size, int& cx, int& cy, int& cz) {
-  const double fx = floor(__ddiv_rn(p[0], cell_size)), fy = floor(__ddiv_rn(p[1], cell_size)), fz = floor(__ddiv_rn(p[2], cell_size));
-  if (!(fabs(fx) < (double)VB && fabs(fy) < (double)VB && fabs(fz) < (double)VB)) { cx = cy = cz = 0; return false; }
-  cx = (int)fx; cy = (int)fy; cz = (int)fz;
-  return true;
-}
-
 __global__ void overlap_key_kernel(const double* __restrict__ xyz, int64_t n, double cell_size, uint64_t* __restrict__ keys,
                                    int32_t* __restrict__ idx, int32_t* status) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
   int cx, cy, cz;
-  if (!cell_of(xyz + 3 * i, cell_size, cx, cy, cz)) atomicOr(status, PCB_FRAMES_RANGE);
+  if (!grid_cell(xyz + 3 * i, cell_size, cx, cy, cz)) atomicOr(status, PCB_FRAMES_RANGE);
   keys[i] = cell_key(cx, cy, cz);
   idx[i] = (int32_t)i;
 }
@@ -176,7 +168,7 @@ __global__ void __launch_bounds__(OV_WARPS * 32, 4) overlap_kernel(
     for (int64_t q = lo + warp; q < hi; q += OV_WARPS) {
       const double px = xyz[3 * q], py = xyz[3 * q + 1], pz = xyz[3 * q + 2];
       int cx, cy, cz;
-      if (!cell_of(xyz + 3 * q, cell_size, cx, cy, cz)) continue;
+      if (!grid_cell(xyz + 3 * q, cell_size, cx, cy, cz)) continue;
       for (int d = 0; d < 27; ++d) {
         const int qx = cx + d / 9 - 1, qy = cy + (d / 3) % 3 - 1, qz = cz + d % 3 - 1;
         if (abs(qx) >= VB || abs(qy) >= VB || abs(qz) >= VB) continue;

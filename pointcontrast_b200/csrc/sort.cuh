@@ -30,4 +30,13 @@ __host__ __device__ __forceinline__ uint64_t cell_key(int cx, int cy, int cz) {
   return ((uint64_t)(cx + VB) << 42) | ((uint64_t)(cy + VB) << 21) | (uint64_t)(cz + VB);
 }
 
+// The cell of an fp64 point p[0..2]: floor(p / cell_size) per axis, one rounded division each; false outside +-2^20 (also for a
+// non-finite coordinate), the cell then (0, 0, 0).  pcb_frame_overlap (pair_list.cu) and pcb_nearest (fulleval.cu).
+__device__ __forceinline__ bool grid_cell(const double* __restrict__ p, double cell_size, int& cx, int& cy, int& cz) {
+  const double fx = floor(__ddiv_rn(p[0], cell_size)), fy = floor(__ddiv_rn(p[1], cell_size)), fz = floor(__ddiv_rn(p[2], cell_size));
+  if (!(fabs(fx) < (double)VB && fabs(fy) < (double)VB && fabs(fz) < (double)VB)) { cx = cy = cz = 0; return false; }
+  cx = (int)fx; cy = (int)fy; cz = (int)fz;
+  return true;
+}
+
 }  // namespace pcb

@@ -17,20 +17,29 @@ Evaluation (`lib/test.py:62-196`) and the training loop around the step (`lib/tr
     r = metrics.result()                                    # one device -> host read: r.loss, r.score, r.mAP, r.mIoU, r.iou, ...
     loss, score, mAP, mIoU = test(model, val_loader, config)
     trainer.train(train_loader, val_loader)                 # stat / save / val frequencies, best_val checkpoint, resume
+
+On the original point cloud (`lib/utils.py:304-349`, `lib/datasets/scannet.py:131-172`, `stanford.py:41-84`; `pcb_nearest`,
+`pcb_label_transfer`):
+
+    test(model, val_loader, config)        # data.return_transformation + test.save_prediction / test.test_original_pointcloud
+    r = test_pointcloud(dataset, pred_dir)  # the same from saved `pred_%04d_%02d.npy` files: r.hist, r.iou, r.mIoU
 """
 import dataclasses
 import logging
 import os
+import tempfile
 import time
 import warnings
 
 import numpy as np
 import torch
 
-from . import losses, me as ME
+from . import _lib, losses, me as ME
 from ._lib import check, lib, ptr, stream
 from .me import workspace
 from .optim import FlatSGD, PolyLR
+
+_FULLEVAL_SLOT = 9
 
 
 def load_state_with_same_shape(model, weights):
@@ -302,19 +311,47 @@ def print_info(iteration, max_iteration, data_time, iter_time, has_gt=False, r=N
     logging.info(s)
 
 
-def test(model, data_loader, config, has_gt=True):
+class TransformationRequired(ValueError, NotImplementedError):
+    """`test.save_prediction` / `test.test_original_pointcloud` without `data.return_transformation`.  Also a NotImplementedError,
+    which is what `test` raised for these keys before it supported them."""
+
+
+def test(model, data_loader, config, has_gt=True, evaluator=None):
     """`lib/test.py:62-196`: `model.eval()` under `torch.no_grad()` (the fused eval-mode forward) over one pass of `data_loader` (e.g.
-    `semseg_data.initialize_data_loader(..., repeat=False)`: items (coords, feats, target) with colours already normalised), the
-    metrics accumulated on the device and logged every `config.test.test_stat_freq` batches.  Returns (loss, precision@1, mAP, mIoU).
-    Saving predictions, evaluation on the original point cloud and returned transformations are not supported."""
-    for key in ("save_prediction", "test_original_pointcloud", "evaluate_original_pointcloud"):
-        if config.test.get(key):
-            raise NotImplementedError(f"test.{key}")
-    if config.data.get("return_transformation"):
-        raise NotImplementedError("data.return_transformation")
+    `semseg_data.initialize_data_loader(..., repeat=False)`: items (coords, feats, target[, transformation]) with colours already
+    normalised), the metrics accumulated on the device and logged every `config.test.test_stat_freq` batches.  Returns (loss,
+    precision@1, mAP, mIoU).
+
+    `config.test.save_prediction`: `save_predictions` of every batch into `config.test.save_pred_dir` (new or empty).
+    `config.test.test_original_pointcloud`: the predictions go, on the device, into a `PointCloudEvaluator` (`evaluator`, else a new
+    one writing ScanNet's submission files under `<save_pred_dir>/fulleval`, or under a new temporary directory without
+    `save_prediction`; the directory is logged), which logs the full-resolution IoU.  Both need `data.return_transformation` and a
+    loader in dataset order."""
+    if config.test.get("evaluate_original_pointcloud"):
+        raise NotImplementedError("test.evaluate_original_pointcloud")          # the reference raises it too (`test.py:126-127`)
     dataset = data_loader.dataset
+    save, full = bool(config.test.get("save_prediction")), bool(config.test.get("test_original_pointcloud"))
+    save_pred_dir = None
+    if save or full:
+        if not getattr(dataset, "IS_FULL_POINTCLOUD_EVAL", False):
+            raise ValueError("This dataset does not support full pointcloud evaluation.")
+        if not config.data.get("return_transformation"):
+            raise TransformationRequired("saving predictions / full pointcloud evaluation needs data.return_transformation")
+        if getattr(data_loader, "shuffle", False):
+            raise ValueError("saving predictions / full pointcloud evaluation needs an unshuffled loader (pieces map to items by position)")
+        if save:
+            save_pred_dir = config.test.save_pred_dir
+            os.makedirs(save_pred_dir, exist_ok=True)
+            if os.listdir(save_pred_dir):
+                raise ValueError(f"Directory {save_pred_dir} not empty. Please remove the existing prediction.")
     device = next(model.parameters()).device
     metrics = SegmentationMetrics(dataset.NUM_LABELS, config.data.ignore_label, device)
+    # without ground truth the predictions still come from pcb_seg_metrics (torch's argmax rule), of a second accumulator never read
+    argmax = SegmentationMetrics(dataset.NUM_LABELS, config.data.ignore_label, device) if (save or full) and not has_gt else None
+    if full and evaluator is None:
+        eval_path = os.path.join(save_pred_dir if save else tempfile.mkdtemp(prefix="fulleval_"), "fulleval")
+        logging.info(f"Full pointcloud evaluation: submission files go to {eval_path}")
+        evaluator = PointCloudEvaluator(dataset, device, eval_path=eval_path)
     class_names = getattr(dataset, "CLASS_LABELS", None)
     logging.info("===> Start testing")
     t_start = time.time()
@@ -322,20 +359,258 @@ def test(model, data_loader, config, has_gt=True):
     model.eval()
     data_time = iter_time = 0.0
     iteration = -1
+    first = 0                                          # the dataset index of the batch's first item
     with torch.no_grad():
         data_iter = iter(data_loader)
         for iteration in range(max_iter):
             t0 = time.time()
-            coords, feats, target = next(data_iter)
+            item = next(data_iter)
+            coords, feats, target = item[:3]
             data_time = time.time() - t0
             t0 = time.time()
             soutput = model(ME.SparseTensor(feats, coords).to(device))
+            pred = None
             if has_gt:
-                metrics.update(soutput.F, target)
+                pred, _ = metrics.update(soutput.F, target)
             iter_time = time.time() - t0
+            if save or full:
+                if pred is None:
+                    pred, _ = argmax.update(soutput.F, torch.full((len(soutput.F),), config.data.ignore_label, device=device),
+                                            average_precision=False)
+                pieces = prediction_pieces(coords.to(device), pred, item[3], dataset)
+                if save:
+                    save_predictions(coords, pred, item[3], dataset, iteration, save_pred_dir, pieces=pieces)
+                if full:
+                    for b, (centres, labels) in enumerate(pieces):
+                        evaluator.add(first + b, centres, labels)
+                first += getattr(data_loader, "batch_size", len(pieces))
             if iteration % config.test.test_stat_freq == 0 and iteration > 0:
                 print_info(iteration, max_iter, data_time, iter_time, has_gt, metrics.result(), class_names)
     r = metrics.result()
     print_info(iteration, max_iter, data_time, iter_time, has_gt, r, class_names)
     logging.info("Finished test. Elapsed time: {:.4f}".format(time.time() - t_start))
+    if full:
+        evaluator.finish()
     return r.tuple()
+
+
+# ---------------------------------------------------------------------------------------------------------------- original point cloud
+
+def nearest(ref, query, cell_size):
+    """`pcb_nearest`: idx int32 CUDA [n], the nearest row of ref (fp64 CUDA [m, 3]) to each row of query (fp64 CUDA [n, 3]) by
+    d2 = ((dx dx + dy dy) + dz dz), ties to the smallest index.  cell_size (the grid's) only sets the speed.  Synchronises once, to read
+    the status."""
+    _lib.require_cuda(ref); _lib.require_cuda(query)
+    ref, query = ref.contiguous().double(), query.to(ref.device).contiguous().double()
+    if ref.dim() != 2 or ref.shape[1] != 3 or query.dim() != 2 or query.shape[1] != 3:
+        raise _lib.PcbError(f"ref and query must be [m, 3] / [n, 3], got {tuple(ref.shape)} / {tuple(query.shape)}")
+    m, n = ref.shape[0], query.shape[0]
+    idx = torch.empty(n, dtype=torch.int32, device=ref.device)
+    status = torch.zeros(1, dtype=torch.int32, device=ref.device)
+    with torch.cuda.device(ref.device):
+        wsb = lib.pcb_nearest_ws_bytes(m, n)
+        ws = workspace(wsb, ref.device, slot=_FULLEVAL_SLOT)
+        check(lib.pcb_nearest(ptr(ref), m, ptr(query), n, float(cell_size), ptr(idx), ptr(status), ptr(ws), wsb, stream()))
+    if int(status.item()) & _lib.NEAREST_RANGE:
+        raise _lib.PcbError("nearest: a coordinate is not finite or lies outside +-2^20 cells")
+    return idx
+
+
+def label_transfer(idx, ref_label, query_label=None, lut=None, C=0, hist=None):
+    """`pcb_label_transfer`: point_label int32 CUDA [n] = ref_label[idx]; with query_label, hist (int64 CUDA [C, C], accumulated) +=
+    fast_hist(lut[point_label], lut[query_label], C).  Does not synchronise; returns (point_label, status int32 CUDA [1])."""
+    dev = idx.device
+    idx = idx.contiguous().int()
+    ref_label = ref_label.to(dev).contiguous().int()
+    n = idx.shape[0]
+    point_label = torch.empty(n, dtype=torch.int32, device=dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    if query_label is not None:
+        query_label = query_label.to(dev).contiguous().int()
+        lut = lut.to(dev).contiguous().int()
+        assert hist is not None and hist.dtype == torch.int64 and hist.is_contiguous() and hist.numel() == C * C
+    with torch.cuda.device(dev):
+        check(lib.pcb_label_transfer(ptr(idx), ptr(ref_label), ref_label.shape[0], ptr(query_label), n, ptr(lut), 0 if lut is None else lut.shape[0], int(C),
+                                     ptr(point_label), ptr(hist), ptr(status), stream()))
+    return point_label, status
+
+
+def _decode_lut(dataset, device):
+    """`utils.py:336-339`: masked prediction -> original id, as a device table."""
+    dec = {}
+    for k, v in dataset.label_map.items():
+        dec[v] = k
+    return torch.tensor([dec[v] for v in range(dataset.NUM_LABELS)], dtype=torch.int32, device=device)
+
+
+def prediction_pieces(coords, pred, transformation, dataset):
+    """`utils.py:304-349` up to the file: per batch item of batch-first coords (int CUDA [N, 4]) and pred (masked, int CUDA [N]) the
+    voxel centres in the original frame, inv(T) @ (c + 0.5, 1) (inv: the float32 `np.linalg.inv` of the item's float32 4x4 in
+    transformation [B, 17]; the product in fp64 on the device), and the predictions decoded to original ids.  A list of (centres
+    fp64 CUDA [M, 3], labels int32 CUDA [M])."""
+    dev = coords.device
+    dec = _decode_lut(dataset, dev)
+    T = torch.as_tensor(transformation).cpu().numpy()
+    out = []
+    for i in range(len(T)):
+        mask = coords[:, 0] == int(T[i, 16])
+        c = coords[mask, 1:4].double() + 0.5
+        inv = torch.from_numpy(np.linalg.inv(T[i, :16].reshape(4, 4).astype(np.float32)).astype(np.float64)).to(dev)
+        centres = torch.stack([((inv[k, 0] * c[:, 0] + inv[k, 1] * c[:, 1]) + inv[k, 2] * c[:, 2]) + inv[k, 3] for k in range(3)], 1)
+        out.append((centres.contiguous(), dec[pred[mask].long()]))
+    return out
+
+
+def save_predictions(coords, pred, transformation, dataset, iteration, save_pred_dir, pieces=None):
+    """`utils.py:304-349`: `<save_pred_dir>/pred_%04d_%02d.npy` (iteration, batch item) = fp64 [M, 4] of the item's voxel centres in
+    the original frame and its predictions as original ids (`prediction_pieces`; batch-first coords)."""
+    if pieces is None:
+        pieces = prediction_pieces(coords.to(pred.device), pred, transformation, dataset)
+    for i, (centres, labels) in enumerate(pieces):
+        full = torch.cat([centres, labels.double()[:, None]], 1).cpu().numpy()
+        np.save(os.path.join(save_pred_dir, "pred_%04d_%02d.npy" % (iteration, i)), full)
+
+
+@dataclasses.dataclass
+class PointCloudResult:
+    """The confusion histogram hist[gt, pred] (int64) of the original points, the per-class IoU (in %) and their nanmean."""
+    hist: np.ndarray
+    iou: np.ndarray
+    mIoU: float
+
+
+class PointCloudEvaluator:
+    """`test_pointcloud` (`lib/datasets/scannet.py:131-172`, `stanford.py:41-84`) fed one dataset item at a time with its voxel centres
+    and decoded predictions on the device.  When an evaluation group is complete -- a ScanNet scene; for S3DIS every room of one type
+    in an area (DESIGN.md section 5) -- it reads the group's PLYs, finds each original point's nearest centre (`pcb_nearest`),
+    transfers the labels and bins them (`pcb_label_transfer`).  ScanNet: `<eval_path>/<scene>.txt` of the per-point original ids when
+    eval_path is set.  `finish()` logs and returns the `PointCloudResult`."""
+
+    def __init__(self, dataset, device=None, eval_path=None, cell_size=None):
+        from . import semseg_data as D
+        self.dataset = dataset
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.C = int(dataset.NUM_LABELS)
+        self.cell_size = float(cell_size if cell_size is not None else dataset.VOXEL_SIZE)
+        self.eval_path = eval_path                                 # made when the first submission file is written
+        self.stanford = isinstance(dataset, D.StanfordDataset)
+        if not self.stanford and not isinstance(dataset, D.ScannetVoxelizationDataset):
+            raise ValueError(f"{type(dataset).__name__}: full pointcloud evaluation knows ScanNet and S3DIS")
+        paths = dataset.data_paths
+        if self.stanford:
+            groups = {}
+            for i, p in enumerate(paths):
+                area, room = p.split(os.sep)
+                room = os.path.splitext(room)[0]
+                groups.setdefault((area, "_".join(room.split("_")[:-1])), []).append(i)
+            self.groups = list(groups.values())
+        else:
+            self.groups = [[i] for i in range(len(paths))]
+        self.group_of = {i: g for g, rooms in enumerate(self.groups) for i in rooms}
+        self.pieces = {}
+        self.done = 0
+        self.hist = torch.zeros(self.C * self.C, dtype=torch.int64, device=self.device)
+        self.status = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self.lut = dataset._lut.to(self.device).int()
+
+    def add(self, index, centres, labels):
+        """Item `index`'s voxel centres (fp64 [M, 3]) and predicted original ids (int [M]), on any device."""
+        if index in self.pieces or index not in self.group_of:
+            raise ValueError(f"item {index}: already added or not in the dataset")
+        self.pieces[index] = (centres.to(self.device).double(), labels.to(self.device).int())
+        rooms = self.groups[self.group_of[index]]
+        if all(i in self.pieces for i in rooms):
+            self._evaluate(self.group_of[index], [self.pieces.pop(i) for i in rooms])
+
+    def _cloud(self, i):
+        from .semseg_data import read_ply
+        v = read_ply(os.path.join(self.dataset.data_root, self.dataset.data_paths[i]))
+        cols = ["x", "y", "z", "red", "green", "blue"] + (["label"] if "label" in v.dtype.names else [])
+        return torch.from_numpy(np.stack([np.asarray(v[k], np.float64) for k in cols], 1)).to(self.device), "label" in v.dtype.names
+
+    def _evaluate(self, g, pieces):
+        rooms = self.groups[g]
+        ref = torch.cat([c for c, _ in pieces]).contiguous()
+        ref_label = torch.cat([l for _, l in pieces])
+        clouds = [self._cloud(i) for i in rooms]
+        has = all(h for _, h in clouds)
+        cloud = torch.cat([c for c, _ in clouds])
+        if self.stanford:
+            if not has:
+                raise ValueError(f"S3DIS room group {g}: a PLY without a label property")
+            cloud = torch.unique(cloud, dim=0)                      # `set(tuple(l) ...)`: exact 7-column equality
+        idx = nearest(ref, cloud[:, :3].contiguous(), self.cell_size)
+        point_label, status = label_transfer(idx, ref_label, cloud[:, 6].int() if has else None, self.lut, self.C, self.hist)
+        self.status |= status
+        if not self.stanford and self.eval_path is not None:
+            room_id = "_".join(os.path.splitext(os.path.basename(self.dataset.data_paths[rooms[0]]))[0].split("_")[:2])
+            text = "\n".join(map(str, point_label.cpu().tolist()))
+            os.makedirs(self.eval_path, exist_ok=True)
+            with open(os.path.join(self.eval_path, room_id + ".txt"), "w") as f:
+                f.write(text + "\n" if text else "")                # np.savetxt(..., fmt='%i')
+        self.done += 1
+        if self.stanford:
+            self._check()
+            logging.info(f"Evaluating room {g} / {len(self.groups)}.")
+            hist = self.hist.cpu().numpy().reshape(self.C, self.C)
+            ious = []
+            lines = ["Per class IoU:"]
+            for c, iou in enumerate(_per_class_iu(hist) * 100):
+                if hist.sum(1)[c]:
+                    lines.append(f"{iou}")
+                    ious.append(iou)
+                else:
+                    lines.append("N/A")
+            lines.append(f"Average IoU: {np.nanmean(ious) if ious else float('nan')}")
+            logging.info("\n".join(lines))
+
+    def _check(self):
+        bits = int(self.status.item())
+        if bits & _lib.LABEL_RANGE:
+            raise KeyError("full pointcloud evaluation: a label lies outside the dataset's label map")
+        if bits & _lib.NEAREST_RANGE:
+            raise _lib.PcbError("full pointcloud evaluation: a prediction index is invalid")
+
+    def result(self):
+        self._check()
+        hist = self.hist.cpu().numpy().reshape(self.C, self.C)
+        iou = _per_class_iu(hist) * 100
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore", category=RuntimeWarning)
+            return PointCloudResult(hist, iou, float(np.nanmean(iou)))
+
+    def finish(self):
+        """Checks that every group was evaluated, logs the reference's summary and returns `result()`."""
+        if self.done != len(self.groups):
+            raise ValueError(f"full pointcloud evaluation: {len(self.groups) - self.done} of {len(self.groups)} groups have no complete "
+                             f"prediction (items pending: {sorted(self.pieces)})")
+        r = self.result()
+        if not self.stanford:
+            names = getattr(self.dataset, "CLASS_LABELS", None)
+            logging.info("mIoU: " + str(r.mIoU) + "\n" + ("Class names: " + ", ".join(names) + "\n" if names else "") +
+                         "IoU: " + ", ".join(np.round(r.iou, 2).astype(str)))
+        return r
+
+
+def _per_class_iu(hist):
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.diag(hist) / (hist.sum(1) + hist.sum(0) - np.diag(hist))
+
+
+def test_pointcloud(dataset, pred_dir, device=None, cell_size=None):
+    """`dataset.test_pointcloud(pred_dir)` for a directory of `save_predictions` files written with batch size 1: ScanNet item i is
+    `pred_%04d_00.npy` % i and its submission file goes to `<pred_dir>/fulleval/<scene>.txt`; S3DIS item i is the i-th `.npy` file in
+    sorted order.  The same `PointCloudEvaluator` as `test`; returns its `PointCloudResult`."""
+    from . import semseg_data as D
+    device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    if isinstance(dataset, D.StanfordDataset):
+        files = sorted(f for f in os.listdir(pred_dir) if f.endswith(".npy"))
+        ev = PointCloudEvaluator(dataset, device, cell_size=cell_size)
+    else:
+        files = ["pred_%04d_%02d.npy" % (i, 0) for i in range(len(dataset))]
+        ev = PointCloudEvaluator(dataset, device, eval_path=os.path.join(pred_dir, "fulleval"), cell_size=cell_size)
+    logging.info("Running full pointcloud evaluation.")
+    for i in range(len(dataset)):
+        pred = torch.from_numpy(np.load(os.path.join(pred_dir, files[i]))).to(device)
+        ev.add(i, pred[:, :3].contiguous(), pred[:, 3].long().int())
+    return ev.finish()

@@ -540,11 +540,15 @@ class VoxelizationDataset:
         self._lut = torch.from_numpy(lut).to(self.device)
 
     def load_ply(self, index):
-        """`dataset.py:180-187`: float32 xyz, float32 rgb, int32 labels (numpy)."""
+        """`dataset.py:180-187`: float32 xyz, float32 rgb, int32 labels (numpy).  A scene without a `label` property (the ScanNet
+        test split) gets the ignore label everywhere."""
         data = read_ply(os.path.join(self.data_root, self.data_paths[index]))
         coords = np.array([data["x"], data["y"], data["z"]], dtype=np.float32).T
         feats = np.array([data["red"], data["green"], data["blue"]], dtype=np.float32).T
-        labels = np.array(data["label"], dtype=np.int32)
+        if "label" in data.dtype.names:
+            labels = np.array(data["label"], dtype=np.int32)
+        else:
+            labels = np.full(len(data), self.ignore_mask, np.int32)
         return coords, feats, labels, None
 
     def map_labels(self, labels):
@@ -682,6 +686,27 @@ class cfl_collate_fn_factory:
         return torch.cat(coords_batch, 0).int(), torch.cat(feats_batch, 0).float(), torch.cat(labels_batch, 0).int()
 
 
+class cflt_collate_fn_factory:
+    """`transforms.py:286-316`: the `cfl` collate plus the items' transformations as float32 CPU rows [B, 17] -- the 16 entries of the
+    4x4, then the batch index -- for the scenes the `limit_numpoints` truncation keeps.  (The reference concatenates a 1-D matrix with
+    a 2-D column and an empty point-cloud list; this is what it means to build, DESIGN.md section 5.)"""
+
+    def __init__(self, limit_numpoints):
+        self.limit_numpoints = limit_numpoints
+
+    def __call__(self, list_data):
+        coords, feats, labels, transformations = list(zip(*list_data))[:4]
+        coords_batch, feats_batch, labels_batch = cfl_collate_fn_factory(self.limit_numpoints)(list(zip(coords, feats, labels)))
+        kept, total = len(coords), 0
+        for b, c in enumerate(coords):               # the scenes cfl keeps: those before the one that would exceed the limit
+            total += len(c)
+            if self.limit_numpoints and total > self.limit_numpoints:
+                kept = b
+                break
+        rows = [np.concatenate([np.asarray(t, np.float32).reshape(16), np.float32([b])]) for b, t in enumerate(transformations[:kept])]
+        return coords_batch, feats_batch, labels_batch, torch.from_numpy(np.stack(rows).astype(np.float32))
+
+
 class VoxelizationLoader:
     """The training loader (`dataset.py:311-385` with `repeat=True`): endless; each item is a list of `iter_size` collated sub-batches
     (coords, feats, target) -- what `semseg.SegmentationTrainer.train_step` takes.  `normalize_color` applies `lib/train.py:114`
@@ -710,7 +735,8 @@ class VoxelizationLoader:
 class VoxelizationPassLoader:
     """The evaluation loader (`dataset.py:311-385` with `repeat=False`): one pass over the dataset in sampler order (a fresh permutation
     per pass when `shuffle`), `ceil(n / batch_size)` items, the last one possibly short.  Each item is one collated (coords, feats,
-    target), colours normalised once when `normalize_color` -- what `semseg.test` takes."""
+    target), colours normalised once when `normalize_color` -- what `semseg.test` takes.  With `cflt_collate_fn_factory` the items are
+    (coords, feats, target, transformation)."""
 
     def __init__(self, dataset, batch_size, collate_fn, shuffle=False, normalize_color=False):
         self.dataset, self.batch_size, self.collate_fn = dataset, batch_size, collate_fn
@@ -722,17 +748,18 @@ class VoxelizationPassLoader:
     def __iter__(self):
         order = torch.randperm(len(self.dataset)).tolist() if self.shuffle else list(range(len(self.dataset)))
         for b in range(len(self)):
-            coords, feats, target = self.collate_fn([self.dataset[i] for i in order[b * self.batch_size:(b + 1) * self.batch_size]])
+            item = self.collate_fn([self.dataset[i] for i in order[b * self.batch_size:(b + 1) * self.batch_size]])
             if self.normalize_color:
-                input_transform(None, feats, normalize=True)
-            yield coords, feats, target
+                input_transform(None, item[1], normalize=True)
+            yield tuple(item)
 
 
 def initialize_data_loader(DatasetClass, config, phase, shuffle, augment_data, batch_size, limit_numpoints, iter_size=1, normalize_color=True,
                            input_transform=None, target_transform=None, device="cuda", draws=None, repeat=True, **dataset_kwargs):
     """`dataset.py:311-385`: elastic distortion before voxelisation, then dropout, flip, auto-contrast, colour translation and jitter
     (`config.augmentation.data_aug_color_trans_ratio` / `data_aug_color_jitter_std`).  `repeat=True`: the endless training loader;
-    `repeat=False`: one pass (`VoxelizationPassLoader`, `iter_size` unused)."""
+    `repeat=False`: one pass (`VoxelizationPassLoader`, `iter_size` unused), whose items carry the transformations
+    (`cflt_collate_fn_factory`) when `config.data.return_transformation` is set."""
     prevoxel = [ElasticDistortion(DatasetClass.ELASTIC_DISTORT_PARAMS, draws=draws)] if augment_data else []
     transforms = list(input_transform or [])
     if augment_data:
@@ -743,7 +770,7 @@ def initialize_data_loader(DatasetClass, config, phase, shuffle, augment_data, b
                            input_transform=Compose(transforms) if transforms else None, target_transform=target_transform,
                            augment_data=augment_data, phase=phase, device=device, draws=draws, **dataset_kwargs)
     if not repeat:
-        return VoxelizationPassLoader(dataset, batch_size, cfl_collate_fn_factory(limit_numpoints), shuffle=shuffle,
-                                      normalize_color=normalize_color)
+        collate = cflt_collate_fn_factory if config.data.get("return_transformation") else cfl_collate_fn_factory
+        return VoxelizationPassLoader(dataset, batch_size, collate(limit_numpoints), shuffle=shuffle, normalize_color=normalize_color)
     return VoxelizationLoader(dataset, batch_size, cfl_collate_fn_factory(limit_numpoints), iter_size=iter_size, shuffle=shuffle,
                               normalize_color=normalize_color)
