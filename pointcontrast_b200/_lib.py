@@ -145,10 +145,16 @@ class PcbUnit(C.Structure):
         ("ws", _p), ("ws_bytes", _sz),
         ("flags", C.c_int32),
     ]
-# status bits of pcb_frame_overlap (include/pcb200.h)
-FRAMES_RANGE, FRAMES_OFFSETS = 1, 2
-# status bits of pcb_nearest / pcb_label_transfer (include/pcb200.h)
-NEAREST_RANGE, LABEL_RANGE = 1, 2
+# Every integer `#define PCB_<NAME>` of include/pcb200.h as <NAME> (tests/test_host_abi.py holds this table to the header).
+OK, ERR_CUDA, ERR_ARG = 0, 1, 2                       # return codes
+ERR_RANGE, ERR_DUPLICATE = 3, 4                       # return codes, and the status bits of pcb_coords_pack / pcb_hash_build
+MAX_KERNEL_VOLUME = 27
+FRAMES_RANGE, FRAMES_OFFSETS = 1, 2                   # status bits of pcb_frame_overlap
+NEAREST_RANGE, LABEL_RANGE = 1, 2                     # status bits of pcb_nearest / pcb_label_transfer
+CONV_FORCE_SIMT, CONV_ACCUMULATE = 1, 4               # flags of the convolution and weight-gradient entry points
+PLANES_A_FP16, PLANES_B_FP16 = 8, 16                  # flags: 16-bit plane formats of the split-operand calls
+BN_RELU = 1                                           # flag of pcb_bn_apply_seg
+UNIT_SEPARATE_STATS, UNIT_FP16_FORWARD, UNIT_EVAL = 1, 2, 4     # pcb_unit.flags
 EXPORTS = sorted(_SIGS)
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)          # AttributeError here == the library does not export a declared symbol
@@ -179,6 +185,20 @@ def stream():
         check(lib.pcb_set_device(d))
         _cur_dev[0] = d
     return torch.cuda.current_stream().cuda_stream
+
+
+_WS = {}
+
+
+def workspace(nbytes, device):
+    """Stream-ordered scratch owned by torch's allocator, one per (device, stream) and shared by every call on it (no entry point reads
+    what an earlier call left in `ws`); grows, never shrinks.  Hold the tensor while its pointer is in use: a larger request replaces it."""
+    key = (device.index, torch.cuda.current_stream(device).cuda_stream)
+    t = _WS.get(key)
+    if t is None or t.numel() < nbytes:
+        t = torch.empty(max(int(nbytes), 1 << 20), dtype=torch.uint8, device=device)
+        _WS[key] = t
+    return t
 
 
 def require_cuda(t):

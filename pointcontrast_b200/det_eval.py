@@ -17,7 +17,7 @@ import types
 import numpy as np
 import torch
 
-from ._lib import PcbError, check, lib, ptr, require_cuda, stream
+from ._lib import PcbError, check, lib, ptr, require_cuda, stream, workspace
 
 NMS_MODES = {"2d": 0, "3d": 1, "3d_samecls": 2}
 MIN_POINTS = 5                                          # ap_helper.py:98: a box with fewer points is empty
@@ -276,7 +276,7 @@ class _Accumulator:
         D, G, P = cls.numel(), gcls.numel(), prop.shape[0]
         out = torch.empty(T, C, 4, dtype=torch.float64, device=dev)
         wsb = lib.pcb_det_ap_ws_bytes(D, G, C, T)
-        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        ws = workspace(wsb, dev)
         thr = (ctypes.c_double * T)(*[float(x) for x in thresholds])           # host array: the entry point copies it
         check(lib.pcb_det_ap(ptr(prop), P, ptr(row), ptr(cls), ptr(score), ptr(scan), D, ptr(gtc), ptr(gscan), ptr(gcls), G, C,
                              ctypes.addressof(thr), T, ptr(out), ptr(ws), wsb, stream()))

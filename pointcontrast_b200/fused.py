@@ -328,7 +328,8 @@ class Runner:
             assert residual.p, "a residual input needs its fp32 plane"
             u.res_p, u.res_ld = residual.p, residual.ld
         u.ws, u.ws_bytes = self.ws.data_ptr(), self.ws.numel()
-        u.flags = (1 if SEPARATE_STATS else 0) | (2 if me.FWD_FP16 else 0) | (4 if self.eval_mode else 0)
+        u.flags = ((_lib.UNIT_SEPARATE_STATS if SEPARATE_STATS else 0) | (_lib.UNIT_FP16_FORWARD if me.FWD_FP16 else 0)
+                   | (_lib.UNIT_EVAL if self.eval_mode else 0))
         me.record_profile("fwd", plan, K, Cin, Cout, tc)
         check(lib.pcb_unit_forward(ctypes.byref(u), self.st))
         if CAPTURE_RELU is not None and relu:
@@ -361,7 +362,7 @@ class Runner:
                 d = buf[off:off + sizes_d[i]]; off += al(sizes_d[i])
                 K, Cin, Cout = c.kernel.shape
                 check(lib.pcb_tile_desc_fill(ctypes.byref(descs[i]), c.kernel.data_ptr(), K, Cin, Cout, f.data_ptr(), d.data_ptr(),
-                                             me.PLANES_B_FP16 if me.FWD_FP16 else 0, start))
+                                             _lib.PLANES_B_FP16 if me.FWD_FP16 else 0, start))
                 start += K * Cin * Cout
                 views.append((f, d))
             host = torch.frombuffer(bytearray(bytes(descs)), dtype=torch.uint8)
@@ -441,7 +442,7 @@ class Runner:
             self.stats = torch.empty(4 * sum(mod.bn.num_features for mod in m.modules() if isinstance(mod, me.MinkowskiBatchNorm)),
                                      dtype=torch.float32, device=dev)
             self.stat_off = 0
-            self.ws = me.workspace(self._ws_bytes(g), dev, slot=5)
+            self.ws = _lib.workspace(self._ws_bytes(g), dev)
             self._refresh_tiles()
             self.arena = arena = Arena(dev, self._fwd_hint)
             P = m.PLANES
@@ -482,6 +483,7 @@ class Runner:
             self.units = self.arena = self.stats = None
             return out_t, None
         tape = _Tape()
+        # the units' u.ws is used again by the backward sweep, and a later, larger request replaces the cached buffer: the tape holds it
         tape.units, tape.arena, tape.x_last, tape.p_final, tape.stats, tape.geom, tape.ws = self.units, arena, x, p1[0], self.stats, g, self.ws
         self.units = self.arena = self.stats = None
         return out_t, tape

@@ -8,8 +8,7 @@ Nothing in this file synchronises the host with the device.
 import torch
 
 from . import _lib
-from ._lib import check, lib, ptr, stream
-from .me import workspace
+from ._lib import check, lib, ptr, stream, workspace
 
 
 class _PointNCEFunction(torch.autograd.Function):
@@ -22,7 +21,7 @@ class _PointNCEFunction(torch.autograd.Function):
         dq, dk = torch.empty_like(q), torch.empty_like(k)
         with torch.cuda.device(q.device):
             wsb = lib.pcb_nce_ws_bytes(n)
-            ws = workspace(wsb, q.device, slot=1)
+            ws = workspace(wsb, q.device)
             check(lib.pcb_nce_forward_backward(ptr(q), ptr(k), n, D, inv_T, ptr(loss), ptr(dq), ptr(dk), ptr(ws), wsb, stream()))
         ctx.save_for_backward(dq, dk)
         return loss
@@ -72,7 +71,7 @@ class _CrossEntropyFunction(torch.autograd.Function):
         dlogits = torch.empty_like(logits)
         with torch.cuda.device(logits.device):
             wsb = lib.pcb_ce_ws_bytes(n)
-            ws = workspace(wsb, logits.device, slot=1)
+            ws = workspace(wsb, logits.device)
             check(lib.pcb_ce_forward_backward(ptr(logits), ptr(target), n, C, int(ignore_index), 1.0, ptr(loss), ptr(dlogits), ptr(ws), wsb,
                                               stream()))
         ctx.save_for_backward(dlogits)

@@ -22,7 +22,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import check, lib, ptr, stream
+from ._lib import check, lib, ptr, stream, workspace
 
 
 class RegionType(Enum):
@@ -86,7 +86,7 @@ class KernelGenerator:
         else:
             raise NotImplementedError(f"{region_type} is not on the hot path")
         self.kernel_volume = len(self.offsets)
-        if self.kernel_volume > 27:
+        if self.kernel_volume > _lib.MAX_KERNEL_VOLUME:
             raise NotImplementedError("kernel volume > 27")
         self.cache_key = (tuple(self.kernel_size), tuple(map(tuple, self.offsets.tolist())))
 
@@ -110,20 +110,6 @@ class CoordsKey:
 
     def __repr__(self):
         return f"CoordsKey(ts={self.ts})"
-
-
-# ------------------------------------------------------------------------------------------------ workspace
-_WS = {}
-
-
-def workspace(nbytes, device, slot=0):
-    """Stream-ordered scratch owned by torch's allocator, one per (device, slot, stream); grows, never shrinks."""
-    key = (device.index, slot, torch.cuda.current_stream(device).cuda_stream)
-    t = _WS.get(key)
-    if t is None or t.numel() < nbytes:
-        t = torch.empty(max(int(nbytes), 1 << 20), dtype=torch.uint8, device=device)
-        _WS[key] = t
-    return t
 
 
 class _Level:
@@ -209,9 +195,9 @@ class CoordsManager:
             lvl._coords = c
             self._hash(lvl, status)
             st = int(status.item())
-        if st & 3:
+        if st & _lib.ERR_RANGE:
             raise _lib.PcbError("coordinate out of the packable range (batch < 65535, |x|,|y|,|z| < 32768)")
-        if st & 4:
+        if st & _lib.ERR_DUPLICATE:
             raise _lib.PcbError("duplicate coordinates in SparseTensor")
         self.levels[ts] = lvl
 
@@ -255,7 +241,7 @@ class CoordsManager:
             with torch.cuda.device(self.device):
                 out_keys = torch.empty(src.n, dtype=torch.int64, device=self.device)
                 wsb = lib.pcb_coords_stride_ws_bytes(src.n)
-                ws = workspace(wsb, self.device, slot=4)
+                ws = workspace(wsb, self.device)
                 n_out = ctypes.c_int64(0)
                 check(lib.pcb_coords_stride(ptr(src.keys), src.n, new_ts[0], ptr(out_keys), None, ctypes.byref(n_out),
                                             ptr(ws), wsb, stream()))
@@ -398,7 +384,6 @@ PROFILE = None
 # bf16 hi/lo's 16): the forward pass is what sets the whole-network gradient error.  Test hook: False runs bf16 everywhere (the
 # modular path's numerics), the reference side of tests/test_gpu_model.py and profiles/grad_precision_ab.py.
 FWD_FP16 = True
-CONV_FORCE_SIMT, CONV_ACCUMULATE, PLANES_A_FP16, PLANES_B_FP16 = 1, 4, 8, 16
 
 
 def record_profile(kind, plan, K, Cin, Cout, tc):
@@ -424,9 +409,9 @@ def conv(kind, plan, Cin, Cout, x, ldx, y, ldy, tiles=None, w=None, bias=None, a
     else:
         tbl, kmap, n_out, Cin, Cout = plan.dg_tbl, plan.c_kmap("dg_kmap"), plan.n_in, Cout, Cin
     if tiles is not None:
-        flags = (CONV_ACCUMULATE if accumulate else 0) | ((PLANES_A_FP16 | PLANES_B_FP16) if fp16 else 0)
+        flags = (_lib.CONV_ACCUMULATE if accumulate else 0) | ((_lib.PLANES_A_FP16 | _lib.PLANES_B_FP16) if fp16 else 0)
         wsb = lib.pcb_conv_forward_split_ws_bytes(K, n_out, Cin, Cout)
-        ws = workspace(wsb, _device(), slot=2)
+        ws = workspace(wsb, _device())
         check(lib.pcb_conv_forward_split(x[0], x[1], ldx, ptr(tbl), tbl.shape[1], kmap, K, n_out, Cin, Cout, tiles, bias, y, ldy,
                                          ptr(ws), wsb, flags, stream()))
     else:
@@ -445,7 +430,7 @@ def wgrad(plan, Cin, Cout, x, ldx, dy, lddy, dw, split, accumulate=False, force_
         A, lda, B, ldb, Ca, Cb, tr, rows = x, ldx, dy, lddy, Cin, Cout, 0, plan.n_out
     else:
         A, lda, B, ldb, Ca, Cb, tr, rows = dy, lddy, x, ldx, Cout, Cin, 1, plan.n_in
-    flags = CONV_ACCUMULATE if accumulate else 0
+    flags = _lib.CONV_ACCUMULATE if accumulate else 0
     tbl = plan.wg_tbl
     if split:
         wsb = lib.pcb_conv_wgrad_split_ws_bytes(K, rows, Ca, Cb)
@@ -456,7 +441,7 @@ def wgrad(plan, Cin, Cout, x, ldx, dy, lddy, dw, split, accumulate=False, force_
         wsb = lib.pcb_conv_wgrad_ws_bytes(K, rows, Ca, Cb)
         ws = workspace(wsb, _device())
         check(lib.pcb_conv_wgrad(A, lda, B, ldb, ptr(tbl), tbl.shape[1], K, rows, Ca, Cb, dw, tr, ptr(ws), wsb,
-                                 flags | (CONV_FORCE_SIMT if force_simt else 0), stream()))
+                                 flags | (_lib.CONV_FORCE_SIMT if force_simt else 0), stream()))
 
 
 _WEIGHTS_EPOCH = [0]
@@ -487,7 +472,7 @@ class _PreparedWeights:
             K, Cin, Cout = kernel.shape
             f = torch.empty(lib.pcb_weight_tile_bytes(K, Cin, Cout, 0), dtype=torch.uint8, device=kernel.device)
             d = torch.empty(lib.pcb_weight_tile_bytes(K, Cin, Cout, 1), dtype=torch.uint8, device=kernel.device)
-            check(lib.pcb_weight_tile(ptr(kernel.detach()), K, Cin, Cout, ptr(f), ptr(d), PLANES_B_FP16 if fp16 else 0, stream()))
+            check(lib.pcb_weight_tile(ptr(kernel.detach()), K, Cin, Cout, ptr(f), ptr(d), _lib.PLANES_B_FP16 if fp16 else 0, stream()))
             self._tiles, self.tile_tag = (f, d), tag
         return self._tiles
 

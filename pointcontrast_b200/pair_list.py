@@ -26,8 +26,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import check, lib, ptr, stream
-from .me import workspace
+from ._lib import check, lib, ptr, stream, workspace
 
 MAX_FRAMES = 4096
 
@@ -51,7 +50,7 @@ def voxel_down_sample(xyz, offsets, voxel_size):
     host = (ctypes.c_int64 * max(F + 1, 1))()
     with torch.cuda.device(xyz.device):
         wsb = lib.pcb_voxel_down_sample_ws_bytes(n, F)
-        ws = workspace(wsb, xyz.device, slot=6)
+        ws = workspace(wsb, xyz.device)
         check(lib.pcb_voxel_down_sample(ptr(xyz), n, ptr(offsets), F, float(voxel_size), ptr(out), ptr(out_off), host, ptr(ws), wsb,
                                         stream()))
     return out[:host[F]], out_off, list(host)
@@ -66,7 +65,7 @@ def overlap_counts(points, offsets, radius):
     status = torch.zeros(1, dtype=torch.int32, device=points.device)
     with torch.cuda.device(points.device):
         wsb = lib.pcb_frame_overlap_ws_bytes(n, F)
-        ws = workspace(wsb, points.device, slot=6)
+        ws = workspace(wsb, points.device)
         check(lib.pcb_frame_overlap(ptr(points), n, ptr(offsets), F, float(radius), ptr(counts), ptr(status), ptr(ws), wsb, stream()))
     bits = int(status.item())
     if bits & _lib.FRAMES_OFFSETS:

@@ -18,10 +18,7 @@ import torch.nn as nn
 from torch.autograd import Function
 
 from . import _lib
-from ._lib import PcbError, check, lib, ptr, stream
-from .me import workspace
-
-_WS_SLOT = 7
+from ._lib import PcbError, check, lib, ptr, stream, workspace
 
 
 def _check(t, dtype, name, device=None):
@@ -48,7 +45,7 @@ def furthest_point_sampling(points, nsamples):
     out = torch.empty(B, int(nsamples), dtype=torch.int32, device=points.device)
     with torch.cuda.device(points.device):
         wsb = lib.pcb_furthest_point_sampling_ws_bytes(B, N)
-        ws = workspace(wsb, points.device, slot=_WS_SLOT) if wsb else None
+        ws = workspace(wsb, points.device) if wsb else None
         check(lib.pcb_furthest_point_sampling(ptr(points), B, N, int(nsamples), ptr(out), ptr(ws), wsb, stream()))
     return out
 
@@ -63,7 +60,7 @@ def furthest_point_sampling_ragged(points, offsets, max_n, nsamples):
     out = torch.empty(B, int(nsamples), dtype=torch.int32, device=points.device)
     with torch.cuda.device(points.device):
         wsb = lib.pcb_furthest_point_sampling_ragged_ws_bytes(B, M, int(max_n))
-        ws = workspace(wsb, points.device, slot=_WS_SLOT) if wsb else None
+        ws = workspace(wsb, points.device) if wsb else None
         check(lib.pcb_furthest_point_sampling_ragged(ptr(points), ptr(offsets), B, M, int(max_n), int(nsamples), ptr(out), ptr(ws), wsb,
                                                      stream()))
     return out
@@ -80,7 +77,7 @@ def gather_rows_grad(grad_out, idx, m):
     out = torch.empty(int(m), C, dtype=torch.float32, device=grad_out.device)
     with torch.cuda.device(grad_out.device):
         wsb = lib.pcb_points_grad_ws_bytes(1, int(m), L)
-        ws = workspace(wsb, grad_out.device, slot=_WS_SLOT)
+        ws = workspace(wsb, grad_out.device)
         check(lib.pcb_gather_rows_grad(ptr(grad_out), ptr(idx), L, C, int(m), ptr(out), ptr(ws), wsb, stream()))
     return out
 
@@ -100,7 +97,7 @@ def _points_grad(grad_out, idx, weight, B, C, n_src, L):
     out = torch.empty(B, C, int(n_src), dtype=torch.float32, device=grad_out.device)
     with torch.cuda.device(grad_out.device):
         wsb = lib.pcb_points_grad_ws_bytes(B, int(n_src), L)
-        ws = workspace(wsb, grad_out.device, slot=_WS_SLOT)
+        ws = workspace(wsb, grad_out.device)
         if weight is None:
             check(lib.pcb_gather_points_grad(ptr(grad_out), ptr(idx), B, C, int(n_src), L, ptr(out), ptr(ws), wsb, stream()))
         else:

@@ -35,11 +35,8 @@ import numpy as np
 import torch
 
 from . import _lib, losses, me as ME
-from ._lib import check, lib, ptr, stream
-from .me import workspace
+from ._lib import check, lib, ptr, stream, workspace
 from .optim import FlatSGD, PolyLR
-
-_FULLEVAL_SLOT = 9
 
 
 def load_state_with_same_shape(model, weights):
@@ -275,7 +272,7 @@ class SegmentationMetrics:
         with torch.cuda.device(self.device):
             st = stream()
             wsb = max(lib.pcb_seg_metrics_ws_bytes(n), lib.pcb_average_precision_ws_bytes(n, C) if average_precision else 0)
-            ws = workspace(wsb, self.device, slot=7)
+            ws = workspace(wsb, self.device)
             check(lib.pcb_seg_metrics(ptr(logits), ptr(target), n, C, self.ignore_label, ptr(pred), ptr(prob), ptr(self.hist), ptr(self.stats),
                                       ptr(ws), wsb, st))
             if average_precision:
@@ -409,7 +406,7 @@ def nearest(ref, query, cell_size):
     status = torch.zeros(1, dtype=torch.int32, device=ref.device)
     with torch.cuda.device(ref.device):
         wsb = lib.pcb_nearest_ws_bytes(m, n)
-        ws = workspace(wsb, ref.device, slot=_FULLEVAL_SLOT)
+        ws = workspace(wsb, ref.device)
         check(lib.pcb_nearest(ptr(ref), m, ptr(query), n, float(cell_size), ptr(idx), ptr(status), ptr(ws), wsb, stream()))
     if int(status.item()) & _lib.NEAREST_RANGE:
         raise _lib.PcbError("nearest: a coordinate is not finite or lies outside +-2^20 cells")

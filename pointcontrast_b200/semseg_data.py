@@ -22,10 +22,7 @@ import numpy as np
 import torch
 
 from . import _lib, voxel
-from ._lib import check, lib, ptr, stream
-from .me import workspace
-
-_WS_SLOT = 8
+from ._lib import check, lib, ptr, stream, workspace
 
 # ---------------------------------------------------------------------------------------------------------------- PLY
 
@@ -174,7 +171,7 @@ def point_bounds(xyz):
     lo, hi = (ctypes.c_float * 3)(), (ctypes.c_float * 3)()
     with torch.cuda.device(xyz.device):
         wsb = lib.pcb_point_bounds_ws_bytes()
-        ws = workspace(wsb, xyz.device, slot=_WS_SLOT)
+        ws = workspace(wsb, xyz.device)
         check(lib.pcb_point_bounds(ptr(xyz), xyz.shape[0], lo, hi, ptr(ws), wsb, stream()))
     return np.array(lo[:], np.float32), np.array(hi[:], np.float32)
 
@@ -189,7 +186,7 @@ def elastic_distort(xyz, noise, axes, magnitude):
     ax = torch.from_numpy(np.concatenate([np.asarray(a, np.float64) for a in axes])).to(xyz.device)
     with torch.cuda.device(xyz.device):
         wsb = lib.pcb_elastic_distort_ws_bytes(gx, gy, gz)
-        ws = workspace(wsb, xyz.device, slot=_WS_SLOT)
+        ws = workspace(wsb, xyz.device)
         check(lib.pcb_elastic_distort(ptr(xyz), xyz.shape[0], ptr(noise), gx, gy, gz, ptr(ax), float(magnitude), ptr(ws), wsb, stream()))
     return xyz
 
@@ -204,7 +201,7 @@ def affine_floor(xyz, T):
     mn = (ctypes.c_int32 * 3)()
     with torch.cuda.device(xyz.device):
         wsb = lib.pcb_affine_floor_ws_bytes()
-        ws = workspace(wsb, xyz.device, slot=_WS_SLOT)
+        ws = workspace(wsb, xyz.device)
         check(lib.pcb_affine_floor(ptr(xyz), xyz.shape[0], Tc.ctypes.data, ptr(out), mn, ptr(ws), wsb, stream()))
     return out, np.array(mn[:], np.int64)
 
@@ -222,7 +219,7 @@ def voxelize_labels(coords, labels, ignore_label):
     m = ctypes.c_int64(0)
     with torch.cuda.device(coords.device):
         wsb = lib.pcb_voxelize_labels_ws_bytes(n)
-        ws = workspace(wsb, coords.device, slot=_WS_SLOT)
+        ws = workspace(wsb, coords.device)
         check(lib.pcb_voxelize_labels(ptr(coords), ptr(labels), n, int(ignore_label), ptr(out), ptr(sel), ptr(lab), ctypes.byref(m), ptr(ws),
                                       wsb, stream()))
     return out[:m.value], sel[:m.value].long(), lab[:m.value]
@@ -247,7 +244,7 @@ def input_transform(coords, feats, flip_mask=0, contrast=False, blend=0.0, trans
         jitter_noise = jitter_noise.contiguous()
     with torch.cuda.device(feats.device):
         wsb = lib.pcb_semseg_input_transform_ws_bytes()
-        ws = workspace(wsb, feats.device, slot=_WS_SLOT)
+        ws = workspace(wsb, feats.device)
         check(lib.pcb_semseg_input_transform(ptr(coords), ptr(feats), n, int(flip_mask), int(bool(contrast)), float(blend), tr, ptr(jitter_noise),
                                              float(jitter_scale), int(bool(normalize)), ptr(ws), wsb, stream()))
     return coords, feats

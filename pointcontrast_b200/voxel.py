@@ -12,8 +12,7 @@ import ctypes
 import torch
 
 from . import _lib
-from ._lib import check, lib, ptr, stream
-from .me import workspace
+from ._lib import check, lib, ptr, stream, workspace
 
 
 def voxelize(xyz, voxel_size):
@@ -26,7 +25,7 @@ def voxelize(xyz, voxel_size):
     m = ctypes.c_int64(0)
     with torch.cuda.device(xyz.device):
         wsb = lib.pcb_voxelize_ws_bytes(n)
-        ws = workspace(wsb, xyz.device, slot=6)
+        ws = workspace(wsb, xyz.device)
         check(lib.pcb_voxelize(ptr(xyz), n, float(voxel_size), ptr(coords), ptr(sel), ctypes.byref(m), ptr(ws), wsb, stream()))
     return coords[:m.value], sel[:m.value].long()
 
@@ -46,7 +45,7 @@ def voxelize_scenes(xyz, voxel_size):
     host = (ctypes.c_int64 * (B + 1))()
     with torch.cuda.device(xyz.device):
         wsb = lib.pcb_voxelize_scenes_ws_bytes(B, N)
-        ws = workspace(wsb, xyz.device, slot=6)
+        ws = workspace(wsb, xyz.device)
         check(lib.pcb_voxelize_scenes(ptr(xyz), B, N, float(voxel_size), ptr(coords), ptr(inds), ptr(offsets), host, ptr(ws), wsb, stream()))
     m = host[B]
     return coords[:m], inds[:m], offsets, list(host)
@@ -60,7 +59,7 @@ def radius_pairs(src, dst, radius):
     total = ctypes.c_int64(0)
     with torch.cuda.device(src.device):
         wsb = lib.pcb_radius_pairs_ws_bytes(ns, nd)
-        ws = workspace(wsb, src.device, slot=6)
+        ws = workspace(wsb, src.device)
         cap = max(4 * ns, 1024)                                     # usually enough for one pass (about 1-3 matches per point)
         pairs = torch.empty(cap, 2, dtype=torch.int32, device=src.device)
         check(lib.pcb_radius_pairs(ptr(src), ns, ptr(dst), nd, float(radius), ptr(pairs), cap, ctypes.byref(total), ptr(ws), wsb, stream()))

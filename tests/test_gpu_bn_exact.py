@@ -39,6 +39,7 @@ import numpy as np
 import pytest
 import torch
 
+from pointcontrast_b200._lib import BN_RELU, ERR_ARG, PLANES_A_FP16, UNIT_EVAL, UNIT_FP16_FORWARD, UNIT_SEPARATE_STATS
 from tests import exact_bn as X
 from tests import exact_conv as XC
 
@@ -49,8 +50,6 @@ REF = 2.0 ** -40
 F64 = torch.float64
 SENT = -7777.25              # fp32 output sentinel
 SENT16 = 0x5A5A              # 16-bit plane sentinel
-PCB_ERR_ARG = 2
-RELU, FP16 = 1, 8            # PCB_BN_RELU, PCB_PLANES_A_FP16
 EPS32 = float(np.float32(X.EPS))
 MOM32 = float(np.float32(X.MOMENTUM))
 A32 = float(np.float32(1.0) - np.float32(X.MOMENTUM))        # fl32(1 - momentum), as the kernel forms it
@@ -299,7 +298,7 @@ def _apply_call(x, n0, mean, invstd, gamma_, beta, res, v, what):
     g, b = gamma_.cuda(), beta.cuda()
     lds = planes["hi"].ld
     rc = L.lib.pcb_bn_apply_seg(xp, ldx, n, n0, C, mb.data_ptr(), ib.data_ptr(), g.data_ptr(), b.data_ptr(), rp, ldr,
-                                (RELU if relu else 0) | (FP16 if fp16 else 0), Y.ptr if Y else None, Y.ld if Y else 0,
+                                (BN_RELU if relu else 0) | (PLANES_A_FP16 if fp16 else 0), Y.ptr if Y else None, Y.ld if Y else 0,
                                 planes["hi"].ptr, planes["lo"].ptr, lds, planes["bhi"].ptr if dual else None,
                                 planes["blo"].ptr if dual else None, L.stream())
     L.check(rc)
@@ -367,7 +366,7 @@ def test_bn_apply_rejects_a_missing_first_view():
     Y = _Out(n, C, False)
     hi, lo = _Out(n, C, False, torch.int16), _Out(n, C, False, torch.int16)
     assert L.lib.pcb_bn_apply_seg(x.data_ptr(), C, n, 0, C, st.data_ptr(), st.data_ptr(), st.data_ptr(), st.data_ptr(), None, 0, 0,
-                                  Y.ptr, C, hi.ptr, lo.ptr, C, None, None, L.stream()) == PCB_ERR_ARG
+                                  Y.ptr, C, hi.ptr, lo.ptr, C, None, None, L.stream()) == ERR_ARG
     assert b"bad argument" in L.lib.pcb_last_error()
     assert L.lib.pcb_bn_apply_seg(x.data_ptr(), C, 0, 0, C, st.data_ptr(), st.data_ptr(), st.data_ptr(), st.data_ptr(), None, 0, 0,
                                   Y.ptr, C, hi.ptr, lo.ptr, C, None, None, L.stream()) == 0
@@ -483,7 +482,7 @@ def test_split_rows_bit_exact(fp16):
         x = X.plane_palette(n, C, seed=n + C).cuda()
         xb, xp, ldx, _ = _in(x, True)
         hi, lo = _Out(n, C, True, torch.int16), _Out(n, C, True, torch.int16)
-        L.check(L.lib.pcb_split_rows(xp, ldx, n, C, hi.ptr, lo.ptr, hi.ld, FP16 if fp16 else 0, L.stream()))
+        L.check(L.lib.pcb_split_rows(xp, ldx, n, C, hi.ptr, lo.ptr, hi.ld, PLANES_A_FP16 if fp16 else 0, L.stream()))
         torch.cuda.synchronize()
         what = f"split_rows n={n} C={C} fp16={fp16}"
         hi.assert_padding(what)
@@ -495,7 +494,6 @@ def test_split_rows_bit_exact(fp16):
 
 
 # ----------------------------------------------------------------------------------------------- through pcb_unit_forward
-UNIT_SEPARATE_STATS, UNIT_FP16_FORWARD, UNIT_EVAL = 1, 2, 4
 
 
 def _unit_forward(n, n0, flags, seed):

@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 import torch
 
+from pointcontrast_b200._lib import CONV_ACCUMULATE, ERR_ARG, PLANES_B_FP16, UNIT_EVAL, UNIT_FP16_FORWARD
 from tests import exact_bn as XB
 from tests import exact_conv as XC
 from tests import exact_unit as XU
@@ -27,8 +28,6 @@ from tests.test_gpu_conv_exact import _assert_exact, _gather, _kmap_arg, _ref_fo
 pytestmark = pytest.mark.gpu
 SENT = -7777.25
 SENT16 = 0x5A5A
-PCB_ERR_ARG = 2
-FP16F, EVAL = 2, 4              # PCB_UNIT_FP16_FORWARD, PCB_UNIT_EVAL
 
 
 def _L():
@@ -117,7 +116,7 @@ class _Case:
         wsb = L.lib.pcb_unit_ws_bytes(self.K, self.n_in, self.n_out, Cin, Cout)
         self.ws = _ws(wsb)
         u.ws, u.ws_bytes = self.ws.data_ptr(), wsb
-        u.flags = (FP16F if sig.fp16 else 0) | (EVAL if sig.eval else 0)
+        u.flags = (UNIT_FP16_FORWARD if sig.fp16 else 0) | (UNIT_EVAL if sig.eval else 0)
 
     def _buf(self, name, n, C, strided, dtype, fill, c0=8, extra=16):
         """[n + 1, ld] framed by `fill`; the operand is columns [c0, c0 + C) of the first n rows.  Sets the struct's pointer."""
@@ -139,7 +138,7 @@ class _Case:
             return
         self.ft = torch.empty(L.lib.pcb_weight_tile_bytes(K, Cin, Cout, 0), dtype=torch.uint8, device="cuda")
         self.dt = torch.empty(L.lib.pcb_weight_tile_bytes(K, Cin, Cout, 1), dtype=torch.uint8, device="cuda")
-        L.check(L.lib.pcb_weight_tile(self.W.data_ptr(), K, Cin, Cout, self.ft.data_ptr(), self.dt.data_ptr(), 16 if self.sig.fp16 else 0,
+        L.check(L.lib.pcb_weight_tile(self.W.data_ptr(), K, Cin, Cout, self.ft.data_ptr(), self.dt.data_ptr(), PLANES_B_FP16 if self.sig.fp16 else 0,
                                       L.stream()))
         self.u.wt_fwd, self.u.wt_dg = self.ft.data_ptr(), self.dt.data_ptr()
 
@@ -514,7 +513,7 @@ def test_unit_chain_matches_primitives(plans, sig):
     if sig.gin_mode:
         L.check(L.lib.pcb_conv_forward_split(P("dz_hi"), P("dz_lo"), u.dz_ld, plan.dg_tbl.data_ptr(), plan.dg_tbl.shape[1],
                                              _kmap_arg(plan.dg_kmap), K, n_in, Cout, Cin, case.dt.data_ptr(), None, P("gin_p"), u.gin_ld,
-                                             ws.data_ptr(), wsb, 4 if sig.gin_mode == 2 else 0, st))
+                                             ws.data_ptr(), wsb, CONV_ACCUMULATE if sig.gin_mode == 2 else 0, st))
     torch.cuda.synchronize()
     what = sig.name() + " chained"
     for k in ["dgamma", "dbeta", "dW"] + (["dz_hi", "dz_lo"] if tc else ["dz_p"]) + ["gin_p"] * (sig.gin_mode > 0) + ["gres_p"] * (sig.gres_mode > 0):
@@ -566,7 +565,7 @@ class _Recorder:
         else:
             kind = "down" if u.n_out < u.n_in else "up"
         s = XU.Sig(kind, u.K, u.Cin, u.Cout, bool(u.relu), bool(u.res_p), bool(u.out_p), u.gres_mode if backward else 0,
-                   u.gin_mode if backward else 0, bool(u.flags & FP16F), bool(u.flags & EVAL), u.n0 < u.n_out,
+                   u.gin_mode if backward else 0, bool(u.flags & UNIT_FP16_FORWARD), bool(u.flags & UNIT_EVAL), u.n0 < u.n_out,
                    (u.x_lds if tc else u.x_ld) != u.Cin, u.out_lds != u.Cout, backward and u.g_ld != u.Cout,
                    backward and u.gin_mode > 0 and u.gin_ld != u.Cin, backward and u.gres_mode > 0 and u.gres_ld != u.Cout)
         return s
@@ -620,9 +619,9 @@ def test_every_executor_signature_is_in_the_matrix(monkeypatch, name):
 
 # ----------------------------------------------------------------------------------------------- e. arguments before writes
 def _violations_forward(u):
-    yield "eval with two views", dict(flags=u.flags | EVAL, n0=u.n_out - 1)
-    yield "eval without running_mean", dict(flags=u.flags | EVAL, n0=u.n_out, running_mean=None)
-    yield "eval without running_var", dict(flags=u.flags | EVAL, n0=u.n_out, running_var=None)
+    yield "eval with two views", dict(flags=u.flags | UNIT_EVAL, n0=u.n_out - 1)
+    yield "eval without running_mean", dict(flags=u.flags | UNIT_EVAL, n0=u.n_out, running_mean=None)
+    yield "eval without running_var", dict(flags=u.flags | UNIT_EVAL, n0=u.n_out, running_var=None)
     yield "fp16 forward without out_bhi", dict(out_bhi=None)
     yield "no x_lo", dict(x_lo=None)
     yield "no weight tiles", dict(wt_fwd=None)
@@ -674,7 +673,7 @@ def test_rejected_struct_writes_nothing(plans, stem):
         v = _copy(case.u, **kw)
         rc = getattr(L.lib, f"pcb_unit_{fn}")(ctypes.byref(v), L.stream())
         torch.cuda.synchronize()
-        assert rc == PCB_ERR_ARG, (fn, name, rc)
+        assert rc == ERR_ARG, (fn, name, rc)
         for k, t in before.items():
             _assert_bits(case.b[k][0], t, f"{fn} rejected ({name}): {k} written")
     # the unchanged struct is accepted by both

@@ -45,7 +45,7 @@ def test_library_has_sm90a_code_and_tensor_core_instructions():
 def test_argument_errors_do_not_need_a_gpu():
     from pointcontrast_b200 import _lib
     rc = _lib.lib.pcb_hash_build(None, 10, None, None, 24, None, None)      # capacity not a power of two
-    assert rc == 2 and b"bad argument" in _lib.lib.pcb_last_error()
+    assert rc == _lib.ERR_ARG and b"bad argument" in _lib.lib.pcb_last_error()
     with pytest.raises(_lib.PcbError):
         _lib.check(rc)
     assert _lib.lib.pcb_conv_wgrad_ws_bytes(27, 100000, 96, 96) > 27 * 96 * 96 * 4
@@ -59,9 +59,10 @@ def test_split_weight_gradient_rejects_fp16_planes():
     fake = 256                                   # never dereferenced
     def wgrad(flags):
         return _lib.lib.pcb_conv_wgrad_split(fake, fake, 32, fake, fake, 32, fake, 0, 27, 0, 32, 32, fake, 0, fake, 256, flags, None)
-    assert wgrad(4) == 0
-    for flags in (4 | 8, 4 | 16, 4 | 8 | 16):
-        assert wgrad(flags) == 2 and b"bad argument" in _lib.lib.pcb_last_error()
+    acc, a16, b16 = _lib.CONV_ACCUMULATE, _lib.PLANES_A_FP16, _lib.PLANES_B_FP16
+    assert wgrad(acc) == _lib.OK
+    for flags in (acc | a16, acc | b16, acc | a16 | b16):
+        assert wgrad(flags) == _lib.ERR_ARG and b"bad argument" in _lib.lib.pcb_last_error()
 
 
 def test_offset_tables_match_oracle():

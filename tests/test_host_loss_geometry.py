@@ -6,7 +6,6 @@ import torch
 
 from tests import exact_loss as X
 
-PCB_ERR_ARG = 2            # include/pcb200.h
 REQUIRED = {"partial last tile", "single split of several tiles", "several splits", "short last split",
             "diagonal in half 0 of a split's last tile", "diagonal in half 1 of a split's last tile"}
 
@@ -114,6 +113,6 @@ def test_pdist_rejects_more_than_64_channels():
     """D = 65 is an argument error, returned before anything touches the (fake) pointers."""
     from pointcontrast_b200 import _lib
     fake = 256
-    assert _lib.lib.pcb_pdist_rowmin(fake, 1, fake, 1, 65, fake, fake, fake, None) == PCB_ERR_ARG
+    assert _lib.lib.pcb_pdist_rowmin(fake, 1, fake, 1, 65, fake, fake, fake, None) == _lib.ERR_ARG
     assert b"bad argument" in _lib.lib.pcb_last_error()
-    assert _lib.lib.pcb_pdist_rowmin(fake, 1, fake, 1, 0, fake, fake, fake, None) == PCB_ERR_ARG
+    assert _lib.lib.pcb_pdist_rowmin(fake, 1, fake, 1, 0, fake, fake, fake, None) == _lib.ERR_ARG

@@ -322,6 +322,18 @@ def test_short_workspace_is_an_argument_error(case, args):
 
 
 @pytest.mark.gpu
+def test_python_workspace_is_one_growing_buffer_per_stream():
+    """_lib.workspace: every caller on a stream shares one buffer, replaced by a larger one on demand; another stream (the side
+    stream of fused.prepare_pair) gets its own."""
+    a = _lib.workspace(1000, DEV)
+    assert _lib.workspace(10, DEV).data_ptr() == a.data_ptr()
+    big = _lib.workspace(a.numel() + 1, DEV)
+    assert big.numel() > a.numel() and _lib.workspace(10, DEV).data_ptr() == big.data_ptr()
+    with torch.cuda.stream(torch.cuda.Stream()):
+        assert _lib.workspace(10, DEV).data_ptr() != big.data_ptr()
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("case,args", CASES, ids=IDS)
 def test_workspace_tail_untouched_and_size_independent(case, args):
     q, call, outputs = case(*args)
