@@ -16,9 +16,11 @@ This module runs the SAME graph (`pretrain/pointcontrast/model/res16unet.py:206-
     device->host reads) is built on a SIDE stream (`prepare_pair`), so those reads never wait for the previous step's
     backward pass and the integer kernels overlap it.
 
-The executor reads the graph from the attribute names (`matches`), so it serves this package's model class and the
-reference's own, unmodified `model/res16unet.py` alike.
+The executor reads the graph once per model from the attribute names into its unit schedule (`schedule`), so it serves this
+package's model class and the reference's own, unmodified `model/res16unet.py` alike; everything else -- issue order,
+buffers, gradient modes, workspace size, neighbour tables -- reads the schedule.
 """
+import collections
 import ctypes
 
 import torch
@@ -40,6 +42,127 @@ SEPARATE_STATS = False
 # the fp64 oracle: a pre-activation within rounding distance of zero is a coin flip in ANY finite precision, and one flipped
 # entry on a deep level moves every upstream gradient by ~1/sqrt(rows x channels) of its norm.
 CAPTURE_RELU = None
+
+
+# ------------------------------------------------------------------------------------------------ the unit schedule
+INPUT = "input"
+
+
+class Unit:
+    """One entry of a model's unit schedule: out = [relu]( BN(conv(x)) [+ res] ), one pcb_unit_forward and one pcb_unit_backward
+    call.  (The schedule's `final` entry is the 1x1 output layer: no BatchNorm, issued as plain convolutions.)
+
+    Buffers are named: INPUT (the network's input), "cat5".."cat8" (the decoder's concatenations, read whole) or the index of the
+    unit that wrote it.  `out` is None for a fresh buffer, with an fp32 plane if `need_f32`, or (concatenation, first column) for a
+    column slice.  `plan` indexes the neighbour-table plans of a `Geometry` (one per distinct `plan_key`).  `gin_mode` / `gres_mode`
+    are the backward call's data- and residual-gradient modes (0: none, 1: write, 2: accumulate)."""
+    __slots__ = ("conv", "bn", "level_in", "level_out", "transpose", "relu", "x", "res", "out", "need_f32", "K", "Cin", "Cout", "tc",
+                 "plan_key", "plan", "gin_mode", "gres_mode")
+
+    def __init__(self, conv, bn, x, level_in, level_out, relu=True, res=None, out=None, need_f32=False):
+        self.conv, self.bn, self.x, self.res, self.out, self.relu = conv, bn, x, res, out, relu
+        self.level_in, self.level_out, self.transpose = level_in, level_out, conv.is_transpose
+        self.need_f32 = need_f32 and out is None
+        self.K, self.Cin, self.Cout = (int(v) for v in conv.kernel.shape)
+        self.tc = me.tensor_core_shape(self.Cin, self.Cout)
+        self.plan_key = (level_in, level_out, conv.kernel_generator.cache_key, self.transpose)
+        self.gin_mode = self.gres_mode = 0
+
+
+# a model's units in issue order, its concatenation buffers as (name, level, width) in allocation order, its final layer, and one
+# entry per neighbour-table plan in build order
+Schedule = collections.namedtuple("Schedule", "units cats final plans")
+
+
+class _NotWired(Exception):
+    pass
+
+
+def schedule(model):
+    """`model`'s unit schedule -- the one description of the graph the executor runs -- or None if it is not wired like
+    `pretrain/pointcontrast/model/res16unet.py:36-268` (Res16UNet with BasicBlock stages) with the widths the tensor-core tiling
+    needs (every hidden width % 32).  Read from the attribute names, so ANY class with this wiring -- this package's model file
+    or the reference's own, unmodified -- runs fused.  Built once per model (cached on it) from module attributes and kernel
+    shapes only: a model on the meta device has one too."""
+    d = model.__dict__
+    if "_fused_schedule" not in d:
+        try:
+            d["_fused_schedule"] = _build_schedule(model)
+        except (AttributeError, TypeError, IndexError, _NotWired):
+            d["_fused_schedule"] = None
+    return d["_fused_schedule"]
+
+
+def matches(model):
+    return schedule(model) is not None
+
+
+def _build_schedule(m):
+    P, I = m.PLANES, m.INIT_DIM
+    final = m.final
+    if not isinstance(final, me.MinkowskiConvolution) or final.kernel_volume != 1:
+        raise _NotWired
+    units = []
+
+    def unit(conv, bn, x, level_in, level_out, **kw):
+        if not isinstance(conv, me._ConvolutionBase) or not isinstance(bn, me.MinkowskiBatchNorm) \
+                or conv.is_transpose != (level_out < level_in):
+            raise _NotWired
+        units.append(Unit(conv, bn, x, level_in, level_out, **kw))
+        return len(units) - 1
+
+    def stage(blocks, x, level, out=None, need_f32=False):
+        """A stage of BasicBlocks.  A block's output needs its fp32 plane only if the NEXT block adds it back as the identity
+        residual (`resnet_block.py:51-57`: no downsample branch); `need_f32` says so for the stage's own output."""
+        for i, blk in enumerate(blocks):
+            if not isinstance(blk.conv1, me.MinkowskiConvolution) or not isinstance(blk.conv2, me.MinkowskiConvolution) \
+                    or hasattr(blk, "conv3") or (blk.downsample is not None and len(blk.downsample) != 2):
+                raise _NotWired
+            last = i == len(blocks) - 1
+            h = unit(blk.conv1, blk.norm1, x, level, level)
+            res = x if blk.downsample is None else unit(blk.downsample[0], blk.downsample[1], x, level, level, relu=False, need_f32=True)
+            x = unit(blk.conv2, blk.norm2, h, level, level, res=res, out=out if last else None,
+                     need_f32=need_f32 if last else blocks[i + 1].downsample is None)
+        return x
+
+    # the concatenations: decoder branch in the left columns, encoder skip in the right ones
+    cats = (("cat8", 0, P[7] + I), ("cat7", 1, P[6] + P[0]), ("cat6", 2, P[5] + P[1]), ("cat5", 3, P[4] + P[2]))
+    x = unit(m.conv0p1s1, m.bn0, INPUT, 0, 0, out=("cat8", P[7]))
+    for i, (c, b) in enumerate((("conv1p1s2", "bn1"), ("conv2p2s2", "bn2"), ("conv3p4s2", "bn3"), ("conv4p8s2", "bn4"))):
+        blocks = list(getattr(m, f"block{i + 1}"))
+        x = unit(getattr(m, c), getattr(m, b), x, i, i + 1, need_f32=blocks[0].downsample is None)
+        x = stage(blocks, x, i + 1, out=(f"cat{7 - i}", P[6 - i]) if i < 3 else None)
+    fin_tc = me.tensor_core_shape(final.in_channels, final.out_channels)
+    for i, (c, b) in enumerate((("convtr4p16s2", "bntr4"), ("convtr5p8s2", "bntr5"), ("convtr6p4s2", "bntr6"), ("convtr7p2s2", "bntr7"))):
+        unit(getattr(m, c), getattr(m, b), x, 4 - i, 3 - i, out=(f"cat{5 + i}", 0))
+        x = stage(list(getattr(m, f"block{5 + i}")), f"cat{5 + i}", 3 - i, need_f32=i == 3 and not fin_tc)
+    fin = Unit(final, None, x, 0, 0, relu=False)
+    # the exact fp32 stem (3 input channels), tensor-core widths everywhere else
+    if units[0].Cout != I or fin.Cin != P[7] or units[0].tc or not all(u.tc for u in units[1:]) or any(w % 32 for w in (I, *P)):
+        raise _NotWired
+
+    # gradient modes: the reverse sweep writes a buffer's gradient first, then accumulates into it (a column slice shares its
+    # concatenation's gradient buffer); the final layer's data gradient is the first write
+    root = lambda b: units[b].out[0] if isinstance(b, int) and units[b].out is not None else b
+    has_grad = {root(fin.x)}
+    for i in reversed(range(len(units))):
+        u = units[i]
+        assert root(i) in has_grad, f"unit {i}: its output gets no gradient before its own backward call"
+        for b, mode in ((u.res, "gres_mode"), (u.x, "gin_mode")):
+            if b is not None and b != INPUT:
+                setattr(u, mode, 2 if root(b) in has_grad else 1)
+                has_grad.add(root(b))
+
+    # plans in a fixed build order: tensor-core layers before the exact fp32 stem, stride-1 before strided, larger kernels first,
+    # level by level.  The caching allocator splits its blocks by allocation order; schedule order cost a C1 step on an H100
+    # 250 KB more peak memory.
+    index, plans = {}, []
+    for u in sorted(units + [fin], key=lambda u: (not u.tc, u.level_in != u.level_out, -u.K, u.level_in)):
+        if u.plan_key not in index:
+            index[u.plan_key] = len(plans)
+            plans.append(u)
+        u.plan = index[u.plan_key]
+    return Schedule(tuple(units), cats, fin, tuple(plans))
 
 
 # ------------------------------------------------------------------------------------------------ side-stream preparation
@@ -116,11 +239,12 @@ def prepare_pair(model, feats0, coords0, feats1, coords1, device):
 
 class Geometry:
     """Levels, row counts, per-view row splits and kernel maps of one input: everything the executor needs from the
-    coordinate manager (`SparseTensor` -> 4 strided levels -> 5 + 5 + 4 + 4 + 1 neighbour tables), built in one go with a
-    single device->host read at the end for the per-level view split."""
+    coordinate manager (`SparseTensor` -> 4 strided levels -> one plan per distinct `Unit.plan_key` of the model's schedule,
+    each on the tables of its own units' kernel generator: 19 plans on 19 neighbour tables for Res16UNet), built in one go
+    with a single device->host read at the end for the per-level view split."""
 
     def __init__(self, model, sinput, view0_rows=None):
-        m = model
+        sched = schedule(model)
         cm = sinput.coords_man
         self.sinput = sinput
         with torch.cuda.device(sinput.F.device):
@@ -128,14 +252,7 @@ class Geometry:
             for _ in range(4):
                 keys.append(cm.stride(keys[-1], [2, 2, 2]))
             n = [cm.num_rows(k) for k in keys]
-            kg3 = m.block1[0].conv1.kernel_generator
-            kg1 = m.final.kernel_generator
-            kg2 = m.conv1p1s2.kernel_generator
-            self.p3 = [cm.conv_plan(k, k, kg3, False) for k in keys]
-            self.p1 = [cm.conv_plan(k, k, kg1, False) for k in keys]
-            self.down = [cm.conv_plan(keys[i], keys[i + 1], kg2, False) for i in range(4)]
-            self.up = [cm.conv_plan(keys[i + 1], keys[i], kg2, True) for i in range(4)]
-            self.p0 = cm.conv_plan(keys[0], keys[0], m.conv0p1s1.kernel_generator, False)
+            self.plans = [cm.conv_plan(keys[u.level_in], keys[u.level_out], u.conv.kernel_generator, u.transpose) for u in sched.plans]
             if view0_rows is None or view0_rows >= n[0]:
                 seg = list(n)
             else:                                # rows of view 0 per level: strided levels are sorted by key, batch most significant
@@ -194,14 +311,13 @@ def _grow_hint(old, used):
 class Buf:
     """Matrix [n, C] with row stride ld.  `p`: fp32 storage (or 0), `hi`/`lo`: the same values as bf16 split planes (or 0)
     -- the operand format of the tensor-core kernels.  Storage belongs to an Arena (or `owner` keeps a tensor alive)."""
-    __slots__ = ("owner", "p", "hi", "lo", "bh", "bl", "n", "C", "ld", "slot", "_grad", "parent", "col", "device")
+    __slots__ = ("owner", "p", "hi", "lo", "bh", "bl", "n", "C", "ld", "_grad", "parent", "col", "device")
 
     def __init__(self, owner, p, n, C, ld, device, hi=0, lo=0, parent=None, col=0, bh=0, bl=0):
         self.owner, self.p, self.hi, self.lo, self.n, self.C, self.ld, self.device = owner, p, hi, lo, n, C, ld, device
         self.bh, self.bl = bh, bl             # me.FWD_FP16: hi/lo are fp16 planes (forward gathers), bh/bl the bf16 planes (weight gradient)
         self.parent, self.col = parent, col
         self._grad = None
-        self.slot = parent.slot if parent is not None else [False]     # [gradient buffer initialised?]
 
     @staticmethod
     def new(arena, n, C, fp32=True, split=False, dual=False):
@@ -243,25 +359,26 @@ def _plane_i16(p, n, C, ld, device):
         return torch.as_tensor(_Plane(p, n, C, ld), device=device)
 
 
-class _Tape:
-    __slots__ = ("units", "arena", "x_last", "p_final", "stats", "geom", "ws")
+_Tape = collections.namedtuple("_Tape", "structs bufs arena stats geom ws")
 
 
 class Runner:
     def __init__(self, model):
         self.model = model
+        self.schedule = schedule(model)
         self.anchor = torch.zeros(1, requires_grad=True)
         self._fwd_hint = 0
         self._bwd_hint = 0
+        self._ws_cache = {}
+        self._tile_batch = None
 
     # ------------------------------------------------------------------------------------------ single launches (final layer)
-    def _conv(self, kind, plan, conv, x, out, bias=None):
+    def _conv(self, kind, plan, fin, x, out, bias=None):
         """The final layer's forward ("fwd") or data gradient ("dgrad") into `out`."""
-        kern = conv.kernel
-        Cin, Cout = kern.shape[1:]
-        if Cin % 32 == 0 and Cout % 32 == 0:
+        kern, Cin, Cout = fin.conv.kernel, fin.Cin, fin.Cout
+        if fin.tc:
             assert x.hi, "tensor-core conv needs the split planes of its input"
-            tiles = conv._prepared.tiles(kern, me.FWD_FP16)[0 if kind == "fwd" else 1]
+            tiles = fin.conv._prepared.tiles(kern, me.FWD_FP16)[0 if kind == "fwd" else 1]
             fp16 = me.FWD_FP16 and kind == "fwd"          # forward roles: fp16 activation planes x fp16 weight tiles
             me.conv(kind, plan, Cin, Cout, (x.hi, x.lo), x.ld, out.p, out.ld, tiles=ptr(tiles), bias=ptr(bias), fp16=fp16)
         else:
@@ -271,83 +388,25 @@ class Runner:
             w = kern.detach() if kind == "fwd" else kern.detach().transpose(1, 2).contiguous()
             me.conv(kind, plan, Cin, Cout, x.p, x.ld, out.p, out.ld, w=ptr(w), bias=ptr(bias))
 
-    def _wgrad(self, conv, plan, a_in, dz):
-        kern = conv.kernel
-        Cin, Cout = kern.shape[1:]
+    def _wgrad(self, fin, plan, a_in, dz):
+        kern = fin.conv.kernel
         if kern.grad is None:
             kern.grad = torch.zeros_like(kern)
-        if Cin % 32 == 0 and Cout % 32 == 0:
+        if fin.tc:
             pl = lambda b: (b.bh, b.bl) if b.bh else (b.hi, b.lo)          # activations: their bf16 planes (gradients only have those)
-            me.wgrad(plan, Cin, Cout, pl(a_in), a_in.ld, pl(dz), dz.ld, kern.grad.data_ptr(), True, accumulate=True)
+            me.wgrad(plan, fin.Cin, fin.Cout, pl(a_in), a_in.ld, pl(dz), dz.ld, kern.grad.data_ptr(), True, accumulate=True)
         else:
-            me.wgrad(plan, Cin, Cout, a_in.p, a_in.ld, dz.p, dz.ld, kern.grad.data_ptr(), False, accumulate=True)
-
-    # ------------------------------------------------------------------------------------------ forward
-    def _unit(self, conv, bnm, a_in, plan, relu, residual=None, out=None, need_f32=False):
-        """out = [relu]( BN(conv(a_in)) [+ residual] )   -- one pcb_unit_forward call"""
-        bn = bnm.bn
-        kern = conv.kernel
-        K, Cin, Cout = kern.shape
-        n = plan.n_out
-        n0 = self.seg_of[id(plan)]                       # rows of view 0 at the output level (== n: a single view)
-        nseg = 2 if n0 < n else 1
-        arena = self.arena
-        tc = Cin % 32 == 0 and Cout % 32 == 0
-        z = Buf.new(arena, n, Cout)
-        if out is None:
-            out = Buf.new(arena, n, Cout, fp32=need_f32, split=True, dual=self.dual)
-        u = PcbUnit()
-        u.n_in, u.n_out, u.n0 = plan.n_in, n, n0
-        u.K, u.Cin, u.Cout, u.relu = K, Cin, Cout, 1 if relu else 0
-        u.fwd_tbl, u.fwd_stride = plan.fwd_tbl.data_ptr(), plan.fwd_tbl.shape[1]
-        km = plan.c_kmap("fwd_kmap")
-        u.fwd_kmap = ctypes.cast(km, ctypes.c_void_p) if km is not None else None
-        u.W = kern.data_ptr()
-        if tc:
-            tiles = conv._prepared.tiles(kern, me.FWD_FP16)
-            u.wt_fwd, u.wt_dg = tiles[0].data_ptr(), tiles[1].data_ptr()
-            u.x_hi, u.x_lo, u.x_lds = a_in.hi, a_in.lo, a_in.ld
-            if a_in.bh:
-                u.x_bhi, u.x_blo = a_in.bh, a_in.bl
-        if a_in.p:
-            u.x_p, u.x_ld = a_in.p, a_in.ld
-        u.gamma, u.beta = bn.weight.data_ptr(), bn.bias.data_ptr()
-        u.running_mean, u.running_var = bn.running_mean.data_ptr(), bn.running_var.data_ptr()
-        if bn.momentum is None:
-            raise NotImplementedError("BatchNorm with momentum=None (cumulative average) is not on the hot path")
-        u.eps, u.momentum = bn.eps, bn.momentum
-        u.mean = self._stat(nseg * Cout)
-        u.invstd = self._stat(nseg * Cout)
-        u.z_p, u.z_ld = z.p, z.ld
-        if out.p:
-            u.out_p, u.out_ld = out.p, out.ld
-        u.out_hi, u.out_lo, u.out_lds = out.hi, out.lo, out.ld
-        if out.bh:
-            u.out_bhi, u.out_blo = out.bh, out.bl
-        if residual is not None:
-            assert residual.p, "a residual input needs its fp32 plane"
-            u.res_p, u.res_ld = residual.p, residual.ld
-        u.ws, u.ws_bytes = self.ws.data_ptr(), self.ws.numel()
-        u.flags = ((_lib.UNIT_SEPARATE_STATS if SEPARATE_STATS else 0) | (_lib.UNIT_FP16_FORWARD if me.FWD_FP16 else 0)
-                   | (_lib.UNIT_EVAL if self.eval_mode else 0))
-        me.record_profile("fwd", plan, K, Cin, Cout, tc)
-        check(lib.pcb_unit_forward(ctypes.byref(u), self.st))
-        if CAPTURE_RELU is not None and relu:
-            CAPTURE_RELU.append((n0, _plane_i16(out.hi, n, Cout, out.ld, self.device) > 0))
-        if not self.eval_mode:
-            self.bns.append(bn)
-            self.units.append((u, conv, bn, a_in, out, plan, residual))
-        return out
+            me.wgrad(plan, fin.Cin, fin.Cout, a_in.p, a_in.ld, dz.p, dz.ld, kern.grad.data_ptr(), False, accumulate=True)
 
     def _refresh_tiles(self):
         """Re-tile the weights of every tensor-core convolution in ONE launch when the parameters changed (after each optimiser
         step) and hand the results to the per-layer caches (`me._PreparedWeights`), instead of one small launch per layer."""
         m = self.model
-        convs = [c for c in m.modules() if isinstance(c, me._ConvolutionBase) and c.in_channels % 32 == 0 and c.out_channels % 32 == 0]
+        convs = [c for c in m.modules() if isinstance(c, me._ConvolutionBase) and me.tensor_core_shape(c.in_channels, c.out_channels)]
         tags = [me._PreparedWeights.tag(c.kernel, me.FWD_FP16) for c in convs]
         if all(c._prepared.tile_tag == t for c, t in zip(convs, tags)):
             return
-        cache = self.__dict__.get("_tile_batch")
+        cache = self._tile_batch
         key = tuple((c.kernel.data_ptr(), tuple(c.kernel.shape)) for c in convs) + (me.FWD_FP16,)
         if cache is None or cache[0] != key:
             dev = convs[0].kernel.device
@@ -372,181 +431,158 @@ class Runner:
         for c, t, v in zip(convs, tags, views):
             c._prepared._tiles, c._prepared.tile_tag = v, t
 
-    def _stat(self, C):
-        p = self.stats.data_ptr() + 4 * self.stat_off
-        self.stat_off += C
-        return p
-
-    def _block(self, blk, x, plan3, plan1, out=None, need_f32=False):
-        h = self._unit(blk.conv1, blk.norm1, x, plan3, True)
-        res = x if blk.downsample is None else self._unit(blk.downsample[0], blk.downsample[1], x, plan1, False, need_f32=True)
-        return self._unit(blk.conv2, blk.norm2, h, plan3, True, residual=res, out=out, need_f32=need_f32)
-
-    def _stage(self, seq, x, plan3, plan1, out=None, need_f32=False):
-        """A stage of BasicBlocks.  A block's output needs its fp32 plane only if the NEXT block adds it back as the identity
-        residual (`resnet_block.py:51-57`: no downsample branch); `need_f32` says so for the stage's own output."""
-        blocks = list(seq)
-        for i, blk in enumerate(blocks):
-            last = i == len(blocks) - 1
-            x = self._block(blk, x, plan3, plan1, out if last else None, need_f32 if last else blocks[i + 1].downsample is None)
-        return x
-
-    def _ws_bytes(self, g):
-        """Scratch for the largest unit of this geometry (the units run back to back on one stream and share it)."""
-        m = self.model
-        n, best = g.n, 0
-        cached = self.__dict__.setdefault("_ws_cache", {})
-        if tuple(n) in cached:
-            return cached[tuple(n)]
-        shapes = {(27, n[0], n[0], m.conv0p1s1.in_channels, m.INIT_DIM)}
-        for name, lvl in (("block1", 1), ("block2", 2), ("block3", 3), ("block4", 4), ("block5", 3), ("block6", 2), ("block7", 1), ("block8", 0)):
-            for blk in getattr(m, name):
-                shapes.add((27, n[lvl], n[lvl], blk.conv1.in_channels, blk.conv1.out_channels))
-                shapes.add((27, n[lvl], n[lvl], blk.conv2.in_channels, blk.conv2.out_channels))
-                if blk.downsample is not None:
-                    shapes.add((1, n[lvl], n[lvl], blk.downsample[0].in_channels, blk.downsample[0].out_channels))
-        for i, (dn, upn) in enumerate((("conv1p1s2", "convtr7p2s2"), ("conv2p2s2", "convtr6p4s2"), ("conv3p4s2", "convtr5p8s2"),
-                                       ("conv4p8s2", "convtr4p16s2"))):
-            d, u = getattr(m, dn), getattr(m, upn)
-            shapes.add((8, n[i], n[i + 1], d.in_channels, d.out_channels))
-            shapes.add((8, n[i + 1], n[i], u.in_channels, u.out_channels))
-        for (K, n_in, n_out, ci, co) in shapes:
-            best = max(best, lib.pcb_unit_ws_bytes(K, n_in, n_out, ci, co))
-        if len(cached) > 64:
-            cached.clear()
-        cached[tuple(n)] = best
+    def _ws_bytes(self, n):
+        """Scratch for the largest unit at `n` rows per level (the units run back to back on one stream and share it)."""
+        n = tuple(n)
+        best = self._ws_cache.get(n)
+        if best is None:
+            if len(self._ws_cache) > 64:
+                self._ws_cache.clear()
+            best = self._ws_cache[n] = max(lib.pcb_unit_ws_bytes(u.K, n[u.level_in], n[u.level_out], u.Cin, u.Cout)
+                                           for u in self.schedule.units)
         return best
 
+    # ------------------------------------------------------------------------------------------ forward
     def forward(self, sinput, view0_rows=None, geom=None, eval_mode=False):
         """`view0_rows`: the input is a `stack_views` tensor whose first `view0_rows` rows are view 0.
-        `eval_mode`: forward only with eval-mode BatchNorm (running statistics); nothing is kept for a backward pass."""
-        m = self.model
-        self.eval_mode = eval_mode
-        self.dual = me.FWD_FP16 and not eval_mode          # bf16 copies of the activations are only needed by the weight gradient
+        `eval_mode`: forward only with eval-mode BatchNorm (running statistics); nothing is kept for a backward pass.
+        Each unit: out = [relu]( BN(conv(x)) [+ residual] ), one pcb_unit_forward call."""
+        m, sched = self.model, self.schedule
+        dual = me.FWD_FP16 and not eval_mode          # bf16 copies of the activations are only needed by the weight gradient
         feats = sinput.F
         _lib.require_cuda(feats)
-        self.device = dev = feats.device
+        dev = feats.device
         g = geom if geom is not None else Geometry(m, sinput, view0_rows)
-        self.units, self.bns = [], []
+        n = g.n
+        flags = ((_lib.UNIT_SEPARATE_STATS if SEPARATE_STATS else 0) | (_lib.UNIT_FP16_FORWARD if me.FWD_FP16 else 0)
+                 | (_lib.UNIT_EVAL if eval_mode else 0))
         with torch.cuda.device(dev):
-            self.st = stream()
-            n, seg = g.n, g.seg
-            p3, p1, down, up, p0 = g.p3, g.p1, g.down, g.up, g.p0
-            self.seg_of = {id(p0): seg[0]}
-            for l in range(5):
-                self.seg_of[id(p3[l])] = seg[l]
-                self.seg_of[id(p1[l])] = seg[l]
-            for i in range(4):
-                self.seg_of[id(down[i])] = seg[i + 1]
-                self.seg_of[id(up[i])] = seg[i]
-            self.stats = torch.empty(4 * sum(mod.bn.num_features for mod in m.modules() if isinstance(mod, me.MinkowskiBatchNorm)),
-                                     dtype=torch.float32, device=dev)
-            self.stat_off = 0
-            self.ws = _lib.workspace(self._ws_bytes(g), dev)
+            st = stream()
+            stats = torch.empty(4 * sum(mod.bn.num_features for mod in m.modules() if isinstance(mod, me.MinkowskiBatchNorm)),
+                                dtype=torch.float32, device=dev)
+            stat_p = stats.data_ptr()
+            ws = _lib.workspace(self._ws_bytes(n), dev)
             self._refresh_tiles()
-            self.arena = arena = Arena(dev, self._fwd_hint)
-            P = m.PLANES
+            arena = Arena(dev, self._fwd_hint)
             x_in = feats.detach().contiguous().float()
-            a0 = Buf(x_in, x_in.data_ptr(), n[0], x_in.shape[1], x_in.shape[1], dev)
-            a0.slot[0] = None                    # network input: no gradient wanted
-            fin = m.final
-            fin_tc = fin.in_channels % 32 == 0 and fin.out_channels % 32 == 0
-            # concatenation buffers (left = decoder branch, right = encoder skip); consumed by convolutions only: split planes
-            cat8 = Buf.new(arena, n[0], P[7] + m.INIT_DIM, fp32=False, split=True, dual=self.dual)
-            cat7 = Buf.new(arena, n[1], P[6] + P[0], fp32=False, split=True, dual=self.dual)
-            cat6 = Buf.new(arena, n[2], P[5] + P[1], fp32=False, split=True, dual=self.dual)
-            cat5 = Buf.new(arena, n[3], P[4] + P[2], fp32=False, split=True, dual=self.dual)
-            out_p1 = self._unit(m.conv0p1s1, m.bn0, a0, p0, True, out=cat8.cols(P[7], m.INIT_DIM))
-            x = self._unit(m.conv1p1s2, m.bn1, out_p1, down[0], True, need_f32=m.block1[0].downsample is None)
-            b1 = self._stage(m.block1, x, p3[1], p1[1], out=cat7.cols(P[6], P[0]))
-            x = self._unit(m.conv2p2s2, m.bn2, b1, down[1], True, need_f32=m.block2[0].downsample is None)
-            b2 = self._stage(m.block2, x, p3[2], p1[2], out=cat6.cols(P[5], P[1]))
-            x = self._unit(m.conv3p4s2, m.bn3, b2, down[2], True, need_f32=m.block3[0].downsample is None)
-            b3 = self._stage(m.block3, x, p3[3], p1[3], out=cat5.cols(P[4], P[2]))
-            x = self._unit(m.conv4p8s2, m.bn4, b3, down[3], True, need_f32=m.block4[0].downsample is None)
-            x = self._stage(m.block4, x, p3[4], p1[4])
-            self._unit(m.convtr4p16s2, m.bntr4, x, up[3], True, out=cat5.cols(0, P[4]))
-            x = self._stage(m.block5, cat5, p3[3], p1[3])
-            self._unit(m.convtr5p8s2, m.bntr5, x, up[2], True, out=cat6.cols(0, P[5]))
-            x = self._stage(m.block6, cat6, p3[2], p1[2])
-            self._unit(m.convtr6p4s2, m.bntr6, x, up[1], True, out=cat7.cols(0, P[6]))
-            x = self._stage(m.block7, cat7, p3[1], p1[1])
-            self._unit(m.convtr7p2s2, m.bntr7, x, up[0], True, out=cat8.cols(0, P[7]))
-            x = self._stage(m.block8, cat8, p3[0], p1[0], need_f32=not fin_tc)
-            out_t = torch.empty(n[0], fin.out_channels, dtype=torch.float32, device=dev)
-            out = Buf(out_t, out_t.data_ptr(), n[0], fin.out_channels, fin.out_channels, dev)
-            self._conv("fwd", p1[0], fin, x, out, bias=fin.bias.detach().reshape(-1) if fin.bias is not None else None)
-            if self.bns:
-                torch._foreach_add_([bn.num_batches_tracked for bn in self.bns], g.calls)       # one multi-tensor launch, not 62
+            bufs = {INPUT: Buf(x_in, x_in.data_ptr(), n[0], x_in.shape[1], x_in.shape[1], dev)}
+            for name, level, C in sched.cats:             # consumed by convolutions only: split planes
+                bufs[name] = Buf.new(arena, n[level], C, fp32=False, split=True, dual=dual)
+            structs = []
+            for i, s in enumerate(sched.units):
+                bn, kern, plan, a_in = s.bn.bn, s.conv.kernel, g.plans[s.plan], bufs[s.x]
+                n_out, n0 = plan.n_out, g.seg[s.level_out]      # n0: rows of view 0 at the output level (== n_out: a single view)
+                nseg = 2 if n0 < n_out else 1
+                z = Buf.new(arena, n_out, s.Cout)
+                if s.out is None:
+                    out = Buf.new(arena, n_out, s.Cout, fp32=s.need_f32, split=True, dual=dual)
+                else:
+                    out = bufs[s.out[0]].cols(s.out[1], s.Cout)
+                u = PcbUnit()
+                u.n_in, u.n_out, u.n0 = plan.n_in, n_out, n0
+                u.K, u.Cin, u.Cout, u.relu = s.K, s.Cin, s.Cout, 1 if s.relu else 0
+                u.fwd_tbl, u.fwd_stride = plan.fwd_tbl.data_ptr(), plan.fwd_tbl.shape[1]
+                km = plan.c_kmap("fwd_kmap")
+                u.fwd_kmap = ctypes.cast(km, ctypes.c_void_p) if km is not None else None
+                u.W = kern.data_ptr()
+                if s.tc:
+                    tiles = s.conv._prepared.tiles(kern, me.FWD_FP16)
+                    u.wt_fwd, u.wt_dg = tiles[0].data_ptr(), tiles[1].data_ptr()
+                    u.x_hi, u.x_lo, u.x_lds = a_in.hi, a_in.lo, a_in.ld
+                    if a_in.bh:
+                        u.x_bhi, u.x_blo = a_in.bh, a_in.bl
+                if a_in.p:
+                    u.x_p, u.x_ld = a_in.p, a_in.ld
+                u.gamma, u.beta = bn.weight.data_ptr(), bn.bias.data_ptr()
+                u.running_mean, u.running_var = bn.running_mean.data_ptr(), bn.running_var.data_ptr()
+                if bn.momentum is None:
+                    raise NotImplementedError("BatchNorm with momentum=None (cumulative average) is not on the hot path")
+                u.eps, u.momentum = bn.eps, bn.momentum
+                u.mean, u.invstd = stat_p, stat_p + 4 * nseg * s.Cout
+                stat_p += 8 * nseg * s.Cout
+                u.z_p, u.z_ld = z.p, z.ld
+                if out.p:
+                    u.out_p, u.out_ld = out.p, out.ld
+                u.out_hi, u.out_lo, u.out_lds = out.hi, out.lo, out.ld
+                if out.bh:
+                    u.out_bhi, u.out_blo = out.bh, out.bl
+                if s.res is not None:
+                    res = bufs[s.res]
+                    assert res.p, "a residual input needs its fp32 plane"
+                    u.res_p, u.res_ld = res.p, res.ld
+                u.ws, u.ws_bytes = ws.data_ptr(), ws.numel()
+                u.flags = flags
+                me.record_profile("fwd", plan, s.K, s.Cin, s.Cout, s.tc)
+                check(lib.pcb_unit_forward(ctypes.byref(u), st))
+                if CAPTURE_RELU is not None and s.relu:
+                    CAPTURE_RELU.append((n0, _plane_i16(out.hi, n_out, s.Cout, out.ld, dev) > 0))
+                bufs[i] = out
+                structs.append(u)
+            fin = sched.final
+            out_t = torch.empty(n[0], fin.Cout, dtype=torch.float32, device=dev)
+            out = Buf(out_t, out_t.data_ptr(), n[0], fin.Cout, fin.Cout, dev)
+            bias = fin.conv.bias
+            self._conv("fwd", g.plans[fin.plan], fin, bufs[fin.x], out, bias=bias.detach().reshape(-1) if bias is not None else None)
+            if not eval_mode:
+                torch._foreach_add_([s.bn.bn.num_batches_tracked for s in sched.units], g.calls)       # one multi-tensor launch, not 62
         self._fwd_hint = _grow_hint(self._fwd_hint, arena.total)
         if eval_mode:
-            self.units = self.arena = self.stats = None
             return out_t, None
-        tape = _Tape()
         # the units' u.ws is used again by the backward sweep, and a later, larger request replaces the cached buffer: the tape holds it
-        tape.units, tape.arena, tape.x_last, tape.p_final, tape.stats, tape.geom, tape.ws = self.units, arena, x, p1[0], self.stats, g, self.ws
-        self.units = self.arena = self.stats = None
-        return out_t, tape
+        return out_t, _Tape(structs, bufs, arena, stats, g, ws)
 
     # ------------------------------------------------------------------------------------------ backward
     def backward(self, tape, d_out):
-        m = self.model
+        sched, g, bufs = self.schedule, tape.geom, tape.bufs
+        fin = sched.final
         d_out = d_out.contiguous()
         dev = d_out.device
-        self.device = dev
-        x_last, p_final = tape.x_last, tape.p_final
         with torch.cuda.device(dev):
             st = stream()
             arena = Arena(dev, self._bwd_hint)
-            fin = m.final
-            if fin.out_channels % 32 == 0:
+            if fin.tc:
                 dfin = Buf.new(arena, d_out.shape[0], d_out.shape[1], fp32=False, split=True)
                 check(lib.pcb_split_rows(d_out.data_ptr(), d_out.shape[1], d_out.shape[0], d_out.shape[1], dfin.hi, dfin.lo, dfin.ld, 0, st))
             else:                                # e.g. 13 / 20 classes: the final layer's backward runs on the exact fp32 kernels
                 dfin = Buf(d_out, d_out.data_ptr(), d_out.shape[0], d_out.shape[1], d_out.shape[1], dev)
-            if fin.bias is not None:
-                if fin.bias.grad is None:
-                    fin.bias.grad = torch.zeros_like(fin.bias)
-                fin.bias.grad += d_out.sum(0, keepdim=True)
+            bias = fin.conv.bias
+            if bias is not None:
+                if bias.grad is None:
+                    bias.grad = torch.zeros_like(bias)
+                bias.grad += d_out.sum(0, keepdim=True)
+            p_final, x_last = g.plans[fin.plan], bufs[fin.x]
             self._wgrad(fin, p_final, x_last, dfin)
-            gx = x_last.grad(arena)
-            self._conv("dgrad", p_final, fin, dfin, gx)
-            x_last.slot[0] = True
-            after_unit = m.__dict__.get("_fused_after_unit")       # trainer hook: gradient all-reduce of the chunk this unit completes
-            for (u, conv, bn, a_in, out, plan, residual) in reversed(tape.units):
-                kern = conv.kernel
-                g = out.grad(arena)
-                assert out.slot[0], "gradient of a unit output was never produced"
-                tc = u.Cin % 32 == 0 and u.Cout % 32 == 0
-                n, Cout = u.n_out, u.Cout
-                u.g_p, u.g_ld = g.p, g.ld
-                dz = Buf.new(arena, n, Cout, fp32=not tc, split=tc)       # consumed only by the conv kernels: split planes suffice
+            self._conv("dgrad", p_final, fin, dfin, x_last.grad(arena))
+            after_unit = self.model.__dict__.get("_fused_after_unit")       # trainer hook: gradient all-reduce of the chunk this unit completes
+            for i in reversed(range(len(sched.units))):
+                s, u = sched.units[i], tape.structs[i]
+                bn, kern, plan = s.bn.bn, s.conv.kernel, g.plans[s.plan]
+                gb = bufs[i].grad(arena)
+                u.g_p, u.g_ld = gb.p, gb.ld
+                dz = Buf.new(arena, u.n_out, s.Cout, fp32=not s.tc, split=s.tc)       # consumed only by the conv kernels: split planes suffice
                 u.dz_p, u.dz_hi, u.dz_lo, u.dz_ld = dz.p or None, dz.hi or None, dz.lo or None, dz.ld
-                u.gres_p, u.gres_ld, u.gres_mode = None, 0, 0
-                if residual is not None and residual.slot[0] is not None:
-                    rg = residual.grad(arena)
+                u.gres_p, u.gres_ld, u.gres_mode = None, 0, s.gres_mode
+                if s.gres_mode:
+                    rg = bufs[s.res].grad(arena)
                     u.gres_p, u.gres_ld = rg.p, rg.ld
-                    u.gres_mode = 2 if residual.slot[0] else 1
-                    residual.slot[0] = True
                 for prm in (bn.weight, bn.bias, kern):
                     if prm.grad is None:
                         prm.grad = torch.zeros_like(prm)
                 u.dgamma, u.dbeta, u.dW = bn.weight.grad.data_ptr(), bn.bias.grad.data_ptr(), kern.grad.data_ptr()
                 u.wg_tbl, u.wg_stride, u.wg_gather_x = plan.wg_tbl.data_ptr(), plan.wg_tbl.shape[1], 1 if plan.wg_gather_x else 0
-                u.gin_p, u.gin_ld, u.gin_mode = None, 0, 0
-                if a_in.slot[0] is not None:
-                    ga = a_in.grad(arena)
-                    u.gin_p, u.gin_ld, u.gin_mode = ga.p, ga.ld, 2 if a_in.slot[0] else 1
-                    a_in.slot[0] = True
+                u.gin_p, u.gin_ld, u.gin_mode = None, 0, s.gin_mode
+                if s.gin_mode:
+                    ga = bufs[s.x].grad(arena)
+                    u.gin_p, u.gin_ld = ga.p, ga.ld
                     u.dg_tbl, u.dg_stride = plan.dg_tbl.data_ptr(), plan.dg_tbl.shape[1]
                     km = plan.c_kmap("dg_kmap")
                     u.dg_kmap = ctypes.cast(km, ctypes.c_void_p) if km is not None else None
-                me.record_profile("wgrad", plan, u.K, u.Cin, u.Cout, tc)
-                if u.gin_mode:
-                    me.record_profile("dgrad", plan, u.K, u.Cin, u.Cout, tc)
+                me.record_profile("wgrad", plan, s.K, s.Cin, s.Cout, s.tc)
+                if s.gin_mode:
+                    me.record_profile("dgrad", plan, s.K, s.Cin, s.Cout, s.tc)
                 check(lib.pcb_unit_backward(ctypes.byref(u), st))
                 if after_unit is not None:
-                    after_unit(conv)
+                    after_unit(s.conv)
             self._bwd_hint = _grow_hint(self._bwd_hint, arena.total)
             # the arenas (and the geometry's tables) are released here, in stream order after the last kernel that reads them
 
@@ -563,45 +599,6 @@ class _FusedFunction(torch.autograd.Function):
         ctx.runner.backward(ctx.tape, d_out)
         ctx.tape = None
         return None, None, None, None, None
-
-
-_STAGES = ("block1", "block2", "block3", "block4", "block5", "block6", "block7", "block8")
-_UNITS = (("conv0p1s1", "bn0"), ("conv1p1s2", "bn1"), ("conv2p2s2", "bn2"), ("conv3p4s2", "bn3"), ("conv4p8s2", "bn4"),
-          ("convtr4p16s2", "bntr4"), ("convtr5p8s2", "bntr5"), ("convtr6p4s2", "bntr6"), ("convtr7p2s2", "bntr7"))
-
-
-def matches(model):
-    """Is `model` wired like `pretrain/pointcontrast/model/res16unet.py:36-268` (Res16UNet with BasicBlock stages)?  The
-    executor reads the graph from the attribute names, so ANY class with this wiring -- this package's model file or the
-    reference's own, unmodified -- runs fused.  Also checks what the tensor-core tiling needs (all hidden widths % 32)."""
-    ok = model.__dict__.get("_fused_ok")
-    if ok is None:
-        ok = _matches(model)
-        model.__dict__["_fused_ok"] = ok
-    return ok
-
-
-def _matches(m):
-    try:
-        for c, b in _UNITS:
-            if not isinstance(getattr(m, c), me._ConvolutionBase) or not isinstance(getattr(m, b), me.MinkowskiBatchNorm):
-                return False
-        if not isinstance(m.final, me.MinkowskiConvolution) or m.final.kernel_volume != 1:
-            return False
-        widths = [m.INIT_DIM] + list(m.PLANES)
-        for name in _STAGES:
-            for blk in getattr(m, name):
-                if not all(isinstance(getattr(blk, a), t) for a, t in (("conv1", me.MinkowskiConvolution), ("conv2", me.MinkowskiConvolution),
-                                                                       ("norm1", me.MinkowskiBatchNorm), ("norm2", me.MinkowskiBatchNorm))):
-                    return False
-                if hasattr(blk, "conv3") or (blk.downsample is not None and len(blk.downsample) != 2):
-                    return False
-                widths += [blk.conv1.in_channels, blk.conv1.out_channels, blk.conv2.out_channels]
-        if m.conv0p1s1.out_channels != m.INIT_DIM or m.final.in_channels != m.PLANES[7]:
-            return False
-        return all(w % 32 == 0 for w in widths) and m.conv0p1s1.in_channels % 32 != 0      # exact fp32 stem (3 input channels)
-    except (AttributeError, TypeError):
-        return False
 
 
 def applicable_on(model, device):

@@ -481,8 +481,13 @@ def _simt(op):
     return FORCE_SIMT or op in SIMT_OPS
 
 
+def tensor_core_shape(Cin, Cout):
+    """Widths the split-operand tensor-core kernels tile (both multiples of 32); other convolutions run the exact fp32 kernels."""
+    return Cin % 32 == 0 and Cout % 32 == 0
+
+
 def _use_tc(Cin, Cout, op="fwd"):
-    return (not _simt(op)) and Cin % 32 == 0 and Cout % 32 == 0
+    return (not _simt(op)) and tensor_core_shape(Cin, Cout)
 
 
 def _split_rows(t):
