@@ -88,6 +88,14 @@ int pcb_kernel_map(const uint64_t* out_keys, int64_t n_out, const uint64_t* tabl
                    void* stream);
 /* counts[k] = number of non-negative entries of row k (device int64 [K]). */
 int pcb_kernel_map_count(const int32_t* tbl, int K, int64_t n_out, int64_t* counts, void* stream);
+/* Tile order of a neighbour table for pcb_conv_forward_split_ordered: perm[i] (device int32 [n_out]) = the output row at tile
+ * position i.  Rows are stably sorted by (row / window, mask), bit k of mask = (tbl[k][row] >= 0): rows with the same neighbour
+ * offsets share the kernel's 128-row tiles, so a tile stages fewer offsets, while every tile stays inside one window of `window`
+ * consecutive rows (a multiple of 128; >= n_out: one window), which bounds how far apart in the input a tile's gathers land.
+ * The order depends on the table only, so it serves every kmap over the table.  n_out < 2^31.  ws: pcb_conv_tile_order_ws_bytes. */
+size_t pcb_conv_tile_order_ws_bytes(int64_t n_out);
+int pcb_conv_tile_order(const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int64_t window, int32_t* perm, void* ws,
+                        size_t ws_bytes, void* stream);
 
 /* ----------------------------------------------------------------------------------------------- data preparation (SURVEY.md 8f-2) */
 /* One point per occupied voxel: voxel index = floor(xyz / voxel_size) per axis (fp32, |index| < 2^20).  Writes the M occupied voxels'
@@ -251,6 +259,12 @@ size_t pcb_conv_forward_split_ws_bytes(int K, int64_t n_out, int Cin, int Cout);
 int pcb_conv_forward_split(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride,
                            const int32_t* kmap, int K, int64_t n_out, int Cin, int Cout, const void* w_tiles,
                            const float* bias, float* Y, int ldy, void* ws, size_t ws_bytes, int flags, void* stream);
+/* The same with the output rows taken in the tile order `perm` of pcb_conv_tile_order on `tbl` (NULL: identity, which is
+ * pcb_conv_forward_split).  Same bits as the identity order; an offset-split launch (small levels) runs in the identity order. */
+int pcb_conv_forward_split_ordered(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride,
+                                   const int32_t* kmap, int K, const int32_t* perm, int64_t n_out, int Cin, int Cout,
+                                   const void* w_tiles, const float* bias, float* Y, int ldy, void* ws, size_t ws_bytes, int flags,
+                                   void* stream);
 /* pcb_conv_wgrad_split: both operands as bf16 hi/lo planes; flags: PCB_CONV_ACCUMULATE only (PCB_ERR_ARG if a PCB_PLANES_* flag
  * is set). */
 size_t pcb_conv_wgrad_split_ws_bytes(int K, int64_t n_out, int Ca, int Cb);
@@ -317,6 +331,7 @@ typedef struct pcb_unit {
   int32_t K, Cin, Cout, relu;
   const int32_t* fwd_tbl; int64_t fwd_stride; const int32_t* fwd_kmap;
   const int32_t* dg_tbl; int64_t dg_stride; const int32_t* dg_kmap;
+  const int32_t* fwd_perm;                          /* tile order (pcb_conv_tile_order) of fwd_tbl, or NULL (identity) */
   const int32_t* wg_tbl; int64_t wg_stride; int32_t wg_gather_x;
   const float* W; const void* wt_fwd; const void* wt_dg; float* dW;
   const float* gamma; const float* beta; float* running_mean; float* running_var; float* dgamma; float* dbeta;

@@ -50,6 +50,8 @@ _SIGS = {
     "pcb_semseg_input_transform": (_i, [_p, _p, _l, _i, _i, _d, _p, _p, _d, _i, _p, _sz, _p]),
     "pcb_kernel_map": (_i, [_p, _l, _p, _p, _l, _p, _i, _p, _p]),
     "pcb_kernel_map_count": (_i, [_p, _i, _l, _p, _p]),
+    "pcb_conv_tile_order_ws_bytes": (_sz, [_l]),
+    "pcb_conv_tile_order": (_i, [_p, _l, _i, _l, _l, _p, _p, _sz, _p]),
     "pcb_conv_forward": (_i, [_p, _i, _p, _l, _p, _i, _l, _i, _i, _p, _p, _p, _i, _p]),
     "pcb_gather_sum": (_i, [_p, _i, _p, _l, _p, _i, _l, _i, _p, _i, _p, _p]),
     "pcb_conv_wgrad_ws_bytes": (_sz, [_i, _l, _i, _i]),
@@ -60,6 +62,7 @@ _SIGS = {
     "pcb_weight_tile_batch": (_i, [_p, _i, _l, _p]),
     "pcb_conv_forward_split_ws_bytes": (_sz, [_i, _l, _i, _i]),
     "pcb_conv_forward_split": (_i, [_p, _p, _i, _p, _l, _p, _i, _l, _i, _i, _p, _p, _p, _i, _p, _sz, _i, _p]),
+    "pcb_conv_forward_split_ordered": (_i, [_p, _p, _i, _p, _l, _p, _i, _p, _l, _i, _i, _p, _p, _p, _i, _p, _sz, _i, _p]),
     "pcb_conv_wgrad_split_ws_bytes": (_sz, [_i, _l, _i, _i]),
     "pcb_conv_wgrad_split": (_i, [_p, _p, _i, _p, _p, _i, _p, _l, _i, _l, _i, _i, _p, _i, _p, _sz, _i, _p]),
     "pcb_bn_ws_bytes": (_sz, [_l, _i]),
@@ -129,6 +132,7 @@ class PcbUnit(C.Structure):
         ("K", C.c_int32), ("Cin", C.c_int32), ("Cout", C.c_int32), ("relu", C.c_int32),
         ("fwd_tbl", _p), ("fwd_stride", _l), ("fwd_kmap", _p),
         ("dg_tbl", _p), ("dg_stride", _l), ("dg_kmap", _p),
+        ("fwd_perm", _p),
         ("wg_tbl", _p), ("wg_stride", _l), ("wg_gather_x", C.c_int32),
         ("W", _p), ("wt_fwd", _p), ("wt_dg", _p), ("dW", _p),
         ("gamma", _p), ("beta", _p), ("running_mean", _p), ("running_var", _p), ("dgamma", _p), ("dbeta", _p),

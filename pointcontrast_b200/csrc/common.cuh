@@ -73,15 +73,15 @@ struct ProfScope {
 };
 
 // ---- functions one .cu file defines and another calls.  Declared only here, so each definition is checked against its callers.
-// conv.cu: the tensor-core forward / data gradient of pcb_conv_forward_split, without its profile scope.  partials != NULL: the caller
-// runs the reduction of an offset-split launch itself (bias and PCB_CONV_ACCUMULATE are then rejected: that pass applies them);
+// conv.cu: the tensor-core forward / data gradient of pcb_conv_forward_split_ordered, without its profile scope.  partials != NULL: the
+// caller runs the reduction of an offset-split launch itself (bias and PCB_CONV_ACCUMULATE are then rejected: that pass applies them);
 // *partials receives the planes P[*nsplit][n_out][Cout] in ws, or NULL when the convolution ran unsplit and wrote Y.
 int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap,
-                            int K, int64_t n_out, int Cin, int Cout, const void* w_tiles, const float* bias, float* Y, int ldy, void* ws,
+                            int K, const int32_t* perm, int64_t n_out, int Cin, int Cout, const void* w_tiles, const float* bias, float* Y, int ldy, void* ws,
                             size_t ws_bytes, int flags, cudaStream_t st, const float** partials, int* nsplit);
 // conv_wgmma.cu: the wgmma kernels behind conv.cu's split-operand entry points
 int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl, int64_t tbl_stride,
-                      const int* kmap, int K, int64_t n_out, int Cin, int Cout, const float* bias, float* Y, int ldy,
+                      const int* kmap, int K, const int32_t* perm, int64_t n_out, int Cin, int Cout, const float* bias, float* Y, int ldy,
                       float* partial, int nsplit, int bn, int accumulate, cudaStream_t st, int x_fp16, int w_fp16);
 int launch_wgrad_wgmma(const uint16_t* Ahi, const uint16_t* Alo, int lda, const uint16_t* Bhi, const uint16_t* Blo, int ldb,
                        const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int Ca, int Cb, int rows_per_split, int splits,

@@ -476,7 +476,7 @@ namespace pcb {
 float* conv_split_layout(Carve& c, int nsplit, int64_t n_out, int Cout) { return nsplit > 1 ? c.take<float>(nsplit * n_out * Cout) : nullptr; }
 
 int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride, const int32_t* kmap,
-                            int K, int64_t n_out, int Cin, int Cout, const void* w_tiles, const float* bias, float* Y, int ldy, void* ws,
+                            int K, const int32_t* perm, int64_t n_out, int Cin, int Cout, const void* w_tiles, const float* bias, float* Y, int ldy, void* ws,
                             size_t ws_bytes, int flags, cudaStream_t st, const float** partials, int* nsplit_out) {
   PCB_ARG(K >= 1 && K <= PCB_MAX_KERNEL_VOLUME && n_out >= 0 && Cin % 32 == 0 && Cout % 32 == 0 && Cin >= 32 && Cout >= 32);
   PCB_ARG(lds >= Cin && lds % 8 == 0 && ldy >= Cout && ldy % 4 == 0);
@@ -491,7 +491,10 @@ int conv_forward_split_impl(const uint16_t* Xhi, const uint16_t* Xlo, int lds, c
   for (int k = 0; k < K; ++k) { km[k] = kmap ? kmap[k] : k; PCB_ARG(km[k] >= 0 && km[k] < PCB_MAX_KERNEL_VOLUME); }
   const int accumulate = (flags & PCB_CONV_ACCUMULATE) ? 1 : 0;
   PCB_ARG(!partials || (nsplit_out && !bias && !accumulate));
-  if (int e = launch_conv_wgmma(Xhi, Xlo, lds, w_tiles, tbl, tbl_stride, km, K, n_out, Cin, Cout, bias, Y, ldy,
+  PCB_ARG(n_out < (1ll << 31) || !perm);
+  // An offset-split launch keeps the identity order: a tile's split boundaries fall within its own list of offsets, so another tile
+  // composition would regroup each row's fp32 partial sums.
+  if (int e = launch_conv_wgmma(Xhi, Xlo, lds, w_tiles, tbl, tbl_stride, km, K, nsplit == 1 ? perm : nullptr, n_out, Cin, Cout, bias, Y, ldy,
                                 partial, nsplit, pick_tile(Cout), accumulate, st,
                                 (flags & PCB_PLANES_A_FP16) ? 1 : 0, (flags & PCB_PLANES_B_FP16) ? 1 : 0)) return e;
   if (nsplit == 1) return PCB_OK;
@@ -511,14 +514,22 @@ extern "C" size_t pcb_conv_forward_split_ws_bytes(int K, int64_t n_out, int Cin,
   return layout_bytes(conv_split_layout, conv_splits(K, n_out, Cin, Cout), n_out, Cout);
 }
 
+extern "C" int pcb_conv_forward_split_ordered(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride,
+                                              const int32_t* kmap, int K, const int32_t* perm, int64_t n_out, int Cin, int Cout,
+                                              const void* w_tiles, const float* bias, float* Y, int ldy, void* ws, size_t ws_bytes,
+                                              int flags, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  ProfScope prof(st, 0);
+  return pcb::conv_forward_split_impl(Xhi, Xlo, lds, tbl, tbl_stride, kmap, K, perm, n_out, Cin, Cout, w_tiles, bias, Y, ldy, ws, ws_bytes,
+                                      flags, st, nullptr, nullptr);
+}
+
 extern "C" int pcb_conv_forward_split(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const int32_t* tbl, int64_t tbl_stride,
                                       const int32_t* kmap, int K, int64_t n_out, int Cin, int Cout, const void* w_tiles,
                                       const float* bias, float* Y, int ldy, void* ws, size_t ws_bytes,
                                       int flags, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  ProfScope prof(st, 0);
-  return pcb::conv_forward_split_impl(Xhi, Xlo, lds, tbl, tbl_stride, kmap, K, n_out, Cin, Cout, w_tiles, bias, Y, ldy, ws, ws_bytes, flags,
-                                      st, nullptr, nullptr);
+  return pcb_conv_forward_split_ordered(Xhi, Xlo, lds, tbl, tbl_stride, kmap, K, nullptr, n_out, Cin, Cout, w_tiles, bias, Y, ldy, ws,
+                                        ws_bytes, flags, stream);
 }
 
 namespace {

@@ -4,7 +4,9 @@
 // neighbour) into the K-major no-swizzle core-matrix layout, and fetches the weights, pre-tiled as shared-memory images, by one TMA
 // bulk copy per stage; both complete on the stage's mbarrier.  Per 32-channel step each consumer warpgroup issues 2 k16-steps x 3
 // products (lo.hi + hi.lo + hi.hi).  Offsets without a neighbour in the tile are skipped; small levels split the steps over
-// gridDim.z (partial planes + fixed-order reduce).
+// gridDim.z (partial planes + fixed-order reduce).  With a tile order `perm` (pcb_conv_tile_order), tile position i is output row
+// perm[i]: rows with the same neighbour offsets share tiles, so the skip drops whole pipeline steps; every row still takes its own
+// offsets in ascending order, and the steps it skips would have added exact zeros, so a direct launch computes the same bits.
 #include "common.cuh"
 #include "wgmma_ptx.cuh"
 
@@ -29,6 +31,7 @@ struct Args {
   const __nv_bfloat16* Xhi; const __nv_bfloat16* Xlo; int lds;      // the input as 16-bit hi/lo planes
   const int32_t* tbl; int64_t tbl_stride;
   int kmap[PCB_MAX_KERNEL_VOLUME]; int K;
+  const int32_t* perm;  // output row of each tile position, or NULL (identity)
   int64_t n_out; int Cin; int Cout;
   const unsigned char* wt;                                      // weights pre-tiled as shared-memory images
   const float* bias;
@@ -85,18 +88,18 @@ __global__ void __launch_bounds__(NTHR, Smem<BN>::CTAS) conv_wgmma_kernel(const 
   }
   pdl_wait(); pdl_trigger();        // no global memory touched before this
   {
-    // this tile's slice of the neighbour table -> shared memory; all loads of a thread are issued before the first store
+    // this tile's slice of the neighbour table -> shared memory; all loads of a thread are issued before the first store.  A thread
+    // loads the entries of one tile row (NTHR is a multiple of BM): offsets tid / BM, + NTHR / BM, ...
+    static_assert(NTHR % BM == 0, "one tile row per thread");
     constexpr int FILL = (PCB_MAX_KERNEL_VOLUME * BM + NTHR - 1) / NTHR;
+    const int64_t row = row0 + tid % BM;
+    const int64_t orow = row < p.n_out ? (p.perm ? (int64_t)__ldg(p.perm + row) : row) : -1;
     int vals[FILL];
 #pragma unroll
     for (int f = 0; f < FILL; ++f) {
       const int e = tid + f * NTHR;
       int v = -1;
-      if (e < p.K * BM) {
-        const int k = e / BM, r = e - k * BM;
-        const int64_t row = row0 + r;
-        if (row < p.n_out) v = __ldg(p.tbl + (int64_t)p.kmap[k] * p.tbl_stride + row);
-      }
+      if (e < p.K * BM && orow >= 0) v = __ldg(p.tbl + (int64_t)p.kmap[e / BM] * p.tbl_stride + orow);
       vals[f] = v;
     }
 #pragma unroll
@@ -197,22 +200,36 @@ __global__ void __launch_bounds__(NTHR, Smem<BN>::CTAS) conv_wgmma_kernel(const 
   float* outp = p.partial ? p.partial + (int64_t)blockIdx.z * p.n_out * p.Cout : p.Y;
   const int ldo = p.partial ? p.Cout : p.ldy;
   const float* bias = p.partial ? nullptr : p.bias;
+  // Every read of Y (PCB_CONV_ACCUMULATE) is issued before the first write: a store to dst followed by a load from dst would make each
+  // load wait for the one before it, one memory round trip per 8 columns.
+  float* dst[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int64_t row = row0 + h64 * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
-    if (row >= p.n_out) continue;
-    float* dst = outp + row * ldo + n0;
+    dst[h] = row < p.n_out ? outp + (p.perm ? (int64_t)__ldg(p.perm + row) : row) * ldo + n0 : nullptr;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (!dst[h]) continue;
 #pragma unroll
     for (int c = 0; c < BN / 8; ++c) {
       const int col = c * 8 + 2 * (lane & 3);
-      float2 o = make_float2(acc[4 * c + 2 * h] * p.out_scale, acc[4 * c + 2 * h + 1] * p.out_scale);
-      if (bias) { o.x += bias[n0 + col]; o.y += bias[n0 + col + 1]; }
+      float& x = acc[4 * c + 2 * h];
+      float& y = acc[4 * c + 2 * h + 1];
+      x *= p.out_scale; y *= p.out_scale;
+      if (bias) { x += bias[n0 + col]; y += bias[n0 + col + 1]; }
       if (p.accumulate && !p.partial) {
-        const float2 old = *reinterpret_cast<const float2*>(dst + col);
-        o.x += old.x; o.y += old.y;
+        const float2 old = *reinterpret_cast<const float2*>(dst[h] + col);
+        x += old.x; y += old.y;
       }
-      *reinterpret_cast<float2*>(dst + col) = o;
     }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (!dst[h]) continue;
+#pragma unroll
+    for (int c = 0; c < BN / 8; ++c)
+      *reinterpret_cast<float2*>(dst[h] + c * 8 + 2 * (lane & 3)) = make_float2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]);
   }
 }
 
@@ -239,7 +256,7 @@ int launch(const Args& a, int nsplit, cudaStream_t st, int f16) {
 
 // Called by conv_forward_split_impl (conv.cu).  wt: the weights of this call's roles pre-tiled by pcb_weight_tile[_batch].
 int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const void* wt, const int32_t* tbl, int64_t tbl_stride,
-                      const int* kmap, int K, int64_t n_out, int Cin, int Cout, const float* bias, float* Y, int ldy,
+                      const int* kmap, int K, const int32_t* perm, int64_t n_out, int Cin, int Cout, const float* bias, float* Y, int ldy,
                       float* partial, int nsplit, int bn, int accumulate, cudaStream_t st, int x_fp16, int w_fp16) {
   // wgmma takes ONE 16-bit format for both operands
   if (x_fp16 != w_fp16) { set_error("conv: fp16 and bf16 operand planes cannot be mixed"); return PCB_ERR_ARG; }
@@ -250,6 +267,7 @@ int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const v
   a.wt = (const unsigned char*)wt;
   a.tbl = tbl; a.tbl_stride = tbl_stride; a.K = K; a.n_out = n_out; a.Cin = Cin; a.Cout = Cout;
   for (int k = 0; k < K; ++k) a.kmap[k] = kmap[k];
+  a.perm = perm;
   a.bias = bias; a.Y = Y; a.ldy = ldy;
   a.partial = partial;
   switch (bn) {

@@ -117,6 +117,17 @@ __global__ void map_count_kernel(const int32_t* __restrict__ tbl, int64_t n_out,
   if ((threadIdx.x & 31) == 0 && b) atomicAdd(counts + k, (unsigned long long)__popc(b));
 }
 
+// key[row] = (row / window) << 32 | mask, bit k of mask = (tbl[k][row] >= 0); payload = row
+__global__ void tile_order_key_kernel(const int32_t* __restrict__ tbl, int64_t tbl_stride, int K, int64_t n_out, int64_t window,
+                                      uint64_t* __restrict__ keys, int32_t* __restrict__ idx) {
+  const int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (j >= n_out) return;
+  uint32_t mask = 0;
+  for (int k = 0; k < K; ++k) mask |= (tbl[(int64_t)k * tbl_stride + j] >= 0 ? 1u : 0u) << k;
+  keys[j] = ((uint64_t)(j / window) << 32) | mask;
+  idx[j] = (int32_t)j;
+}
+
 }  // namespace
 
 extern "C" int pcb_coords_pack(const int32_t* coords, int64_t n, uint64_t* keys, int32_t* status, void* stream) {
@@ -190,4 +201,24 @@ extern "C" int pcb_kernel_map_count(const int32_t* tbl, int K, int64_t n_out, in
   dim3 grid(blocks_for(n_out, 256), K);
   map_count_kernel<<<grid, 256, 0, st>>>(tbl, n_out, (unsigned long long*)counts);
   return check_launch("map_count_kernel");
+}
+
+extern "C" size_t pcb_conv_tile_order_ws_bytes(int64_t n_out) {
+  return layout_bytes(sort_layout, n_out < 1 ? 1 : n_out);
+}
+
+extern "C" int pcb_conv_tile_order(const int32_t* tbl, int64_t tbl_stride, int K, int64_t n_out, int64_t window, int32_t* perm, void* ws,
+                                   size_t ws_bytes, void* stream) {
+  PCB_ARG(K >= 1 && K <= PCB_MAX_KERNEL_VOLUME && n_out >= 0 && n_out < (1ll << 31) && window >= 128 && window % 128 == 0);
+  if (n_out == 0) return PCB_OK;
+  Carve c{(char*)ws};
+  SortWs w = sort_layout(c, n_out);
+  PCB_ARG(tbl && perm && tbl_stride >= n_out && ws && ws_bytes >= c.used);
+  w.sidx = perm;                                   // the sorted payloads are the order
+  cudaStream_t st = (cudaStream_t)stream;
+  tile_order_key_kernel<<<blocks_for(n_out, 256), 256, 0, st>>>(tbl, tbl_stride, K, n_out, window, w.k, w.idx);
+  if (int e = check_launch("tile_order_key_kernel")) return e;
+  int end_bit = 32;                                // the mask bits and as many window bits as there are windows
+  while (end_bit < 64 && ((n_out - 1) / window) >> (end_bit - 32)) ++end_bit;
+  return sort_keys(n_out, w, end_bit, st);
 }

@@ -108,7 +108,7 @@ extern "C" int pcb_unit_forward(const pcb_unit* u, void* stream) {
     PCB_ARG(u->x_hi && u->x_lo && u->wt_fwd);
     const bool fuse = !(u->flags & (PCB_UNIT_SEPARATE_STATS | PCB_UNIT_EVAL));
     ProfScope prof(st, 0);                   // the convolution, and the reduction + statistics pass when it has one
-    if (int e = conv_forward_split_impl(u->x_hi, u->x_lo, u->x_lds, u->fwd_tbl, u->fwd_stride, u->fwd_kmap, u->K, u->n_out, u->Cin, u->Cout,
+    if (int e = conv_forward_split_impl(u->x_hi, u->x_lo, u->x_lds, u->fwd_tbl, u->fwd_stride, u->fwd_kmap, u->K, u->fwd_perm, u->n_out, u->Cin, u->Cout,
                                         u->wt_fwd, nullptr, u->z_p, u->z_ld, w.conv, w.conv_bytes, f16 ? (PCB_PLANES_A_FP16 | PCB_PLANES_B_FP16) : 0,
                                         st, fuse ? &partials : nullptr, &nsplit)) return e;
     if (partials) {

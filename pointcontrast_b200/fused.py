@@ -228,7 +228,7 @@ def prepare_pair(model, feats0, coords0, feats1, coords1, device):
             _await_input(t, side)
         with torch.cuda.stream(side):
             p.sinput, p.n0 = stack_views(feats0, coords0, feats1, coords1, device)
-            p.geom = Geometry(model, p.sinput, p.n0)
+            p.geom = Geometry(model, p.sinput, p.n0, tile_orders=True)
             done = torch.cuda.Event()
             done.record(side)
         main.wait_event(done)
@@ -243,7 +243,7 @@ class Geometry:
     each on the tables of its own units' kernel generator: 19 plans on 19 neighbour tables for Res16UNet), built in one go
     with a single device->host read at the end for the per-level view split."""
 
-    def __init__(self, model, sinput, view0_rows=None):
+    def __init__(self, model, sinput, view0_rows=None, tile_orders=False):
         sched = schedule(model)
         cm = sinput.coords_man
         self.sinput = sinput
@@ -252,7 +252,13 @@ class Geometry:
             for _ in range(4):
                 keys.append(cm.stride(keys[-1], [2, 2, 2]))
             n = [cm.num_rows(k) for k in keys]
-            self.plans = [cm.conv_plan(keys[u.level_in], keys[u.level_out], u.conv.kernel_generator, u.transpose) for u in sched.plans]
+            # With `tile_orders` (prepare_pair, whose side stream keeps the sorts off the critical path), tile orders for the forward
+            # launches of the transposed convolutions only.  Their tables give each fine row exactly one coarse neighbour, so a
+            # window-sorted tile stages about 1 of the 8 offsets instead of 5-8, and those launches ran 1.7-2.9x faster on an H100.
+            # Ordering every other table too (3x3x3: 20-22 of 27 offsets per tile instead of 27) sped some launches up by up to 15 %
+            # and slowed others by up to 26 %, 0.35 ms more per C1 step than this choice: DESIGN.md section 7.
+            self.plans = [cm.conv_plan(keys[u.level_in], keys[u.level_out], u.conv.kernel_generator, u.transpose,
+                                       tile_order=tile_orders and u.tc and u.transpose) for u in sched.plans]
             if view0_rows is None or view0_rows >= n[0]:
                 seg = list(n)
             else:                                # rows of view 0 per level: strided levels are sorted by key, batch most significant
@@ -484,6 +490,7 @@ class Runner:
                 u.fwd_tbl, u.fwd_stride = plan.fwd_tbl.data_ptr(), plan.fwd_tbl.shape[1]
                 km = plan.c_kmap("fwd_kmap")
                 u.fwd_kmap = ctypes.cast(km, ctypes.c_void_p) if km is not None else None
+                u.fwd_perm = ptr(plan.fwd_perm)
                 u.W = kern.data_ptr()
                 if s.tc:
                     tiles = s.conv._prepared.tiles(kern, me.FWD_FP16)

@@ -126,8 +126,10 @@ class ConvPlan:
     """Neighbour tables for one (input level, output level, kernel) triple -- ME's cached kernel map.
     fwd:   Y[j]  = sum_k X[fwd_tbl[fwd_kmap[k]][j]] W[k]
     dgrad: dX[i] = sum_k dY[dg_tbl[dg_kmap[k]][i]] W[k]^T
-    wgrad: dW[k] = sum_r A[wg_tbl[k][r]]^T B[r], (A,B) = (X,dY) if wg_gather_x else (dY,X) with transposed output."""
-    __slots__ = ("K", "n_in", "n_out", "fwd_tbl", "fwd_kmap", "dg_tbl", "dg_kmap", "wg_tbl", "wg_gather_x", "_counts", "_c_kmaps")
+    wgrad: dW[k] = sum_r A[wg_tbl[k][r]]^T B[r], (A,B) = (X,dY) if wg_gather_x else (dY,X) with transposed output.
+    fwd_perm: the tile order (pcb_conv_tile_order) of fwd_tbl for the tensor-core kernel, or None (identity)."""
+    __slots__ = ("K", "n_in", "n_out", "fwd_tbl", "fwd_kmap", "dg_tbl", "dg_kmap", "wg_tbl", "wg_gather_x", "fwd_perm", "_counts",
+                 "_c_kmaps")
 
     def pair_counts(self):
         """|M_k| per kernel offset (host list) -- the ME per-offset map sizes."""
@@ -143,6 +145,12 @@ class ConvPlan:
             vals = getattr(self, which)
             self._c_kmaps[which] = _c_int_array(vals) if vals is not None else None
         return self._c_kmaps[which]
+
+
+# Rows per window of the tile order: a tile's rows, sorted by neighbour mask, all come from one window of this many consecutive output
+# rows, so the input rows its gathers read stay close together (L2-resident) while the window still holds enough rows of each mask
+# class to fill whole tiles.  Chosen by the sweep of profiles/bench_conv_order.py (DESIGN.md section 7).
+TILE_ORDER_WINDOW = 16384
 
 
 def _c_int_array(vals):
@@ -258,8 +266,17 @@ class CoordsManager:
                                  ptr(tbl), stream()))
         return tbl
 
-    def conv_plan(self, in_key, out_key, kgen, transpose):
-        """Cached per (levels, kernel) like ME's kernel-map cache; strided conv and its transpose share tables."""
+    def _tile_order(self, tbl):
+        n = tbl.shape[1]
+        perm = torch.empty(n, dtype=torch.int32, device=self.device)
+        wsb = lib.pcb_conv_tile_order_ws_bytes(n)
+        ws = workspace(wsb, self.device)
+        check(lib.pcb_conv_tile_order(ptr(tbl), n, tbl.shape[0], n, TILE_ORDER_WINDOW, ptr(perm), ptr(ws), wsb, stream()))
+        return perm
+
+    def conv_plan(self, in_key, out_key, kgen, transpose, tile_order=False):
+        """Cached per (levels, kernel) like ME's kernel-map cache; strided conv and its transpose share tables.  tile_order: the plan
+        also carries the tile order of its forward table, built once per table (a 1-offset kernel has nothing to reorder)."""
         self._require_ready()
         fine, coarse = (out_key, in_key) if transpose else (in_key, out_key)
         ck = (fine.ts, coarse.ts, kgen.cache_key)
@@ -287,17 +304,20 @@ class CoordsManager:
         if "same" in ent:
             if ent["opp"] is None:
                 raise NotImplementedError("asymmetric stride-1 kernels are not on the hot path")
-            p.fwd_tbl, p.fwd_kmap = ent["same"], None
-            p.dg_tbl, p.dg_kmap = ent["same"], ent["opp"]
+            fwd, dg = "same", "same"
+            p.fwd_kmap, p.dg_kmap = None, ent["opp"]
             p.wg_tbl, p.wg_gather_x = ent["same"], True
-        elif not transpose:
-            p.fwd_tbl, p.fwd_kmap = ent["down"], None
-            p.dg_tbl, p.dg_kmap = ent["up"], None
-            p.wg_tbl, p.wg_gather_x = ent["down"], True
         else:
-            p.fwd_tbl, p.fwd_kmap = ent["up"], None
-            p.dg_tbl, p.dg_kmap = ent["down"], None
-            p.wg_tbl, p.wg_gather_x = ent["down"], False
+            fwd, dg = ("up", "down") if transpose else ("down", "up")
+            p.fwd_kmap = p.dg_kmap = None
+            p.wg_tbl, p.wg_gather_x = ent["down"], not transpose
+        p.fwd_tbl, p.dg_tbl = ent[fwd], ent[dg]
+        p.fwd_perm = None
+        if tile_order and p.K > 1:
+            if ("perm", fwd) not in ent:
+                with torch.cuda.device(self.device):
+                    ent[("perm", fwd)] = self._tile_order(ent[fwd])
+            p.fwd_perm = ent[("perm", fwd)]
         return p
 
 
@@ -405,15 +425,15 @@ def conv(kind, plan, Cin, Cout, x, ldx, y, ldy, tiles=None, w=None, bias=None, a
     K = plan.K
     record_profile(kind, plan, K, Cin, Cout, tiles is not None)
     if kind == "fwd":
-        tbl, kmap, n_out = plan.fwd_tbl, plan.c_kmap("fwd_kmap"), plan.n_out
+        tbl, kmap, perm, n_out = plan.fwd_tbl, plan.c_kmap("fwd_kmap"), plan.fwd_perm, plan.n_out
     else:
-        tbl, kmap, n_out, Cin, Cout = plan.dg_tbl, plan.c_kmap("dg_kmap"), plan.n_in, Cout, Cin
+        tbl, kmap, perm, n_out, Cin, Cout = plan.dg_tbl, plan.c_kmap("dg_kmap"), None, plan.n_in, Cout, Cin
     if tiles is not None:
         flags = (_lib.CONV_ACCUMULATE if accumulate else 0) | ((_lib.PLANES_A_FP16 | _lib.PLANES_B_FP16) if fp16 else 0)
         wsb = lib.pcb_conv_forward_split_ws_bytes(K, n_out, Cin, Cout)
         ws = workspace(wsb, _device())
-        check(lib.pcb_conv_forward_split(x[0], x[1], ldx, ptr(tbl), tbl.shape[1], kmap, K, n_out, Cin, Cout, tiles, bias, y, ldy,
-                                         ptr(ws), wsb, flags, stream()))
+        check(lib.pcb_conv_forward_split_ordered(x[0], x[1], ldx, ptr(tbl), tbl.shape[1], kmap, K, ptr(perm), n_out, Cin, Cout, tiles,
+                                                 bias, y, ldy, ptr(ws), wsb, flags, stream()))
     else:
         if accumulate:
             raise _lib.PcbError("the exact fp32 convolution writes its output, it does not accumulate")

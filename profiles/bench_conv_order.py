@@ -1,0 +1,141 @@
+"""Per-shape cost of the sparse-convolution kernel under tile orders (pcb_conv_tile_order): every tensor-core forward and data-gradient
+launch of one C1 training step (Res16UNet34C, 4 synthetic ScanNet-shape pairs at 2.5 cm, both views stacked), timed with CUDA events
+over windows of at least `--seconds` after warm-up, in the identity order and in the window-sorted order for each window of the sweep.
+Per shape it reports the kernel time, the kernel offsets a 128-row tile stages (of K) and the share of MMA rows that carry a real
+neighbour pair; `per_step_ms` weights each shape by how many units of the step issue it.  Offset-split launches (small levels) always run
+in the identity order and are left out.  Prints one JSON line.
+
+    python profiles/bench_conv_order.py [--seconds 1.0]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+from pointcontrast_b200 import _lib, fused, me, synth  # noqa: E402
+from pointcontrast_b200._lib import check, lib, ptr, stream  # noqa: E402
+from pointcontrast_b200.config import default_config  # noqa: E402
+from pointcontrast_b200.data import to_torch  # noqa: E402
+from pointcontrast_b200.model import load_model  # noqa: E402
+
+BM = 128
+WINDOWS = (4096, 8192, 16384, 0)          # 0: the whole level is one window
+
+
+def gpu_info():
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    try:
+        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout
+        return dict(zip(q.split(","), (v.strip() for v in out.splitlines()[torch.cuda.current_device()].split(","))))
+    except (OSError, IndexError, subprocess.SubprocessError):
+        return {"name": torch.cuda.get_device_name()}
+
+
+def tile_order(tbl, n, window):
+    wsb = lib.pcb_conv_tile_order_ws_bytes(n)
+    ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device="cuda")
+    perm = torch.empty(n, dtype=torch.int32, device="cuda")
+    check(lib.pcb_conv_tile_order(ptr(tbl), tbl.shape[1], tbl.shape[0], n, window, ptr(perm), ptr(ws), wsb, stream()))
+    return perm
+
+
+def tile_stats(mask, order):
+    """(mean offsets per tile, share of MMA rows with a real pair) of the 128-row tiles in `order`."""
+    m = np.concatenate([mask[order], np.zeros(-len(order) % BM, np.int64)]).reshape(-1, BM)
+    nk = np.array([bin(int(v)).count("1") for v in np.bitwise_or.reduce(m, axis=1)])
+    pairs = sum(bin(int(v)).count("1") for v in mask)
+    return float(nk.mean()), float(pairs / (nk.sum() * BM))
+
+
+def time_launch(fn, seconds):
+    """ms per call of fn, from CUDA events around enough back-to-back calls to fill `seconds`."""
+    for _ in range(3):
+        fn()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(5):
+        fn()
+    e1.record()
+    e1.synchronize()
+    reps = max(5, int(seconds * 1e3 / (e0.elapsed_time(e1) / 5)) + 1)
+    e0.record()
+    for _ in range(reps):
+        fn()
+    e1.record()
+    e1.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--seconds", type=float, default=1.0, help="least timed window per (shape, order)")
+    args = ap.parse_args()
+    dev = torch.device("cuda", torch.cuda.current_device())
+    torch.manual_seed(0)
+    net = load_model("Res16UNet34C")(3, 32, default_config(), D=3).to(dev).train()
+    sched = fused.schedule(net)
+    b = to_torch(synth.synth_batch(0, 4, 0.9, 0.025, 300_000), False)
+    sinput, n0 = fused.stack_views(b["sinput0_F"], b["sinput0_C"], b["sinput1_F"], b["sinput1_C"], dev)
+    geom = fused.Geometry(net, sinput, n0)
+
+    shapes = {}                                  # (plan, role, K, contraction, columns) -> units of one step that issue it
+    for u in sched.units:
+        if u.tc and u.K > 1:
+            for role in ("fwd", "dgrad"):
+                key = (u.plan, role, u.K) + ((u.Cin, u.Cout) if role == "fwd" else (u.Cout, u.Cin))
+                shapes[key] = shapes.get(key, 0) + 1
+    rows = []
+    totals = {}
+    for (pi, role, K, Ck, N), count in shapes.items():
+        plan = geom.plans[pi]
+        tbl, kmap = (plan.fwd_tbl, plan.c_kmap("fwd_kmap")) if role == "fwd" else (plan.dg_tbl, plan.c_kmap("dg_kmap"))
+        n_out, n_src = (plan.n_out, plan.n_in) if role == "fwd" else (plan.n_in, plan.n_out)
+        if lib.pcb_conv_forward_split_ws_bytes(K, n_out, Ck, N):
+            continue                             # offset-split: identity order
+        fp16 = role == "fwd" and me.FWD_FP16     # as the executor runs them: fp16 planes forward, bf16 for the data gradient
+        dt = torch.float16 if fp16 else torch.bfloat16
+        x = torch.randn(n_src, Ck, device=dev)
+        xh = x.to(dt)
+        xl = (x - xh.float()).to(dt)
+        W = torch.randn(K, Ck, N, device=dev) * (1.0 / (K * Ck) ** 0.5)
+        tiles = torch.empty(lib.pcb_weight_tile_bytes(K, Ck, N, 0), dtype=torch.uint8, device=dev)
+        spare = torch.empty(lib.pcb_weight_tile_bytes(K, Ck, N, 1), dtype=torch.uint8, device=dev)
+        check(lib.pcb_weight_tile(ptr(W), K, Ck, N, ptr(tiles), ptr(spare), _lib.PLANES_B_FP16 if fp16 else 0, stream()))
+        flags = (_lib.PLANES_A_FP16 | _lib.PLANES_B_FP16) if fp16 else 0
+        Y = torch.empty(n_out, N, device=dev)
+        t = tbl[:, :n_out].cpu().numpy()
+        mask = ((t >= 0).astype(np.int64) << np.arange(K)[:, None]).sum(0)
+        orders = {"identity": None}
+        for w in WINDOWS:
+            orders[str(w) if w else "level"] = tile_order(tbl, n_out, w if w else -(-n_out // BM) * BM)
+        rec = {"role": role, "K": K, "Cin": Ck, "Cout": N, "rows": n_out, "units_per_step": count, "ms": {}, "offsets_per_tile": {},
+               "useful_rows": {}}
+        ref = None
+        for name, perm in orders.items():
+            def call(perm=perm):
+                check(lib.pcb_conv_forward_split_ordered(ptr(xh), ptr(xl), Ck, ptr(tbl), tbl.shape[1], kmap, K, ptr(perm), n_out, Ck, N,
+                                                         ptr(tiles), None, ptr(Y), N, None, 0, flags, stream()))
+            call()
+            if ref is None:
+                ref = Y.clone()
+            rec["same_bits_as_identity" if name == "identity" else f"same_bits_{name}"] = bool(torch.equal(Y.view(torch.int32),
+                                                                                                             ref.view(torch.int32)))
+            rec["ms"][name] = round(time_launch(call, args.seconds), 4)
+            order = np.arange(n_out) if perm is None else perm.cpu().numpy()
+            nk, useful = tile_stats(mask, order)
+            rec["offsets_per_tile"][name] = round(nk, 2)
+            rec["useful_rows"][name] = round(useful, 3)
+            totals[name] = totals.get(name, 0.0) + count * rec["ms"][name]
+        rec.pop("same_bits_as_identity")
+        rows.append(rec)
+    print(json.dumps({"gpu": gpu_info(), "rows_per_level": geom.n, "seconds_per_measurement": args.seconds,
+                      "per_step_ms": {k: round(v, 3) for k, v in totals.items()}, "shapes": rows}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
