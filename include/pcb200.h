@@ -141,6 +141,21 @@ size_t pcb_frame_overlap_ws_bytes(int64_t n, int64_t F);
 int pcb_frame_overlap(const double* xyz, int64_t n, const int64_t* offsets, int64_t F, double radius, int64_t* counts, int32_t* status,
                       void* ws, size_t ws_bytes, void* stream);
 
+/* pcb_depth_to_points: `point_cloud_extractor.py:47-75` for a batch of F depth frames (device uint16 [F, H, W], millimetres) with
+ * the depth intrinsics fx, fy, cx, cy, bx, by and the camera-to-world poses (device fp64 [F, 4, 4], row-major).  Every pixel (u, v)
+ * with nonzero depth becomes one fp64 world point, one rounding per operation and no FMA:
+ *   d = depth / 1000, X = ((u - cx) d) / fx + bx, Y = ((v - cy) d) / fy + by, Z = d,
+ *   out[r] = ((X P[r][0] + Y P[r][1]) + Z P[r][2]) + P[r][3]      (r = 0, 1, 2)
+ * Rows frame-major, within a frame in row-major pixel order (the order of np.where on the flattened image); out holds up to
+ * F H W rows.  out_offsets (device int64 [F + 1]) delimit the frames; SYNCHRONISES once and copies them to out_offsets_host (host,
+ * F + 1 entries) and to nan_host (host int32 [F]) a flag per frame that is 1 when any of its coordinates is NaN.  F outside
+ * [1, 4096], H or W outside [1, 32768], F ceil(H W / 1024) >= 2^31 - 1, NULL pointers and a short workspace return PCB_ERR_ARG before
+ * anything is launched. */
+size_t pcb_depth_to_points_ws_bytes(int64_t F, int64_t H, int64_t W);
+int pcb_depth_to_points(const uint16_t* depth, int64_t F, int64_t H, int64_t W, double fx, double fy, double cx, double cy, double bx,
+                        double by, const double* poses, double* out, int64_t* out_offsets, int64_t* out_offsets_host, int32_t* nan_host,
+                        void* ws, size_t ws_bytes, void* stream);
+
 /* ----------------------------------------------------------------------------------------------- semseg on the original point cloud */
 /* The label transfer of `test_pointcloud` (`downstream/semseg/lib/datasets/scannet.py:131-172`, `stanford.py:41-84`): a scipy KD-tree
  * query of every original point against the predicted voxel centres, then `fast_hist` (`lib/utils.py:131-133`).

@@ -113,6 +113,8 @@ _SIGS = {
     "pcb_voxel_down_sample": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _p, _sz, _p]),
     "pcb_frame_overlap_ws_bytes": (_sz, [_l, _l]),
     "pcb_frame_overlap": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _sz, _p]),
+    "pcb_depth_to_points_ws_bytes": (_sz, [_l, _l, _l]),
+    "pcb_depth_to_points": (_i, [_p, _l, _l, _l, _d, _d, _d, _d, _d, _d, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "pcb_nearest_ws_bytes": (_sz, [_l, _l]),
     "pcb_nearest": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _sz, _p]),
     "pcb_label_transfer": (_i, [_p, _p, _l, _p, _l, _p, _i, _i, _p, _p, _p, _p]),

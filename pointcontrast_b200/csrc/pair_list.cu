@@ -6,8 +6,10 @@
 //     `:39-47`, `:67-74`)                                                                             -> pcb_frame_overlap
 // Both are integer work on the sort-and-unique pipeline and the run table of sort.cuh, in fp64 like the npz frames and open3d.
 // Results are exact and independent of the launch shape (tests/test_gpu_pair_list.py: bit-equal to oracle/pair_list_cpu.py).
+// The stage before them, `point_cloud_extractor.py:47-75` (depth frames back-projected into world points), is pcb_depth_to_points.
 #include <cmath>
 #include <vector>
+#include <cub/cub.cuh>
 #include "sort.cuh"
 
 using namespace pcb;
@@ -209,6 +211,97 @@ OverlapWs overlap_layout(Carve& c, int64_t n) {
 
 bool frames_ok(int64_t n, int64_t F) { return n >= 0 && n < (1ll << 31) && F >= 1 && F <= MAX_FRAMES; }
 
+// pcb_depth_to_points: a CTA takes one tile of DP_TILE consecutive pixels of one frame (grid: tiles x frames); a thread takes
+// DP_ITEMS consecutive pixels of the tile, so a block-wide exclusive scan over the threads in order ranks the valid pixels in
+// row-major order (a stable compaction).
+constexpr int DP_THREADS = 256;
+constexpr int DP_ITEMS = 4;
+constexpr int DP_TILE = DP_THREADS * DP_ITEMS;
+constexpr int64_t DP_MAX_SIDE = 1 << 15;
+using DpScan = cub::BlockScan<int, DP_THREADS>;
+
+// tile_count[f * T + t] = the number of nonzero pixels of tile t of frame f
+__global__ void __launch_bounds__(DP_THREADS) depth_count_kernel(const uint16_t* __restrict__ depth, int64_t P, int T,
+                                                                   int64_t* __restrict__ tile_count) {
+  using Reduce = cub::BlockReduce<int, DP_THREADS>;
+  __shared__ typename Reduce::TempStorage tmp;
+  const int f = blockIdx.y, t = blockIdx.x;
+  const uint16_t* d = depth + f * P;
+  const int64_t p0 = (int64_t)t * DP_TILE + threadIdx.x * DP_ITEMS;
+  int c = 0;
+  for (int k = 0; k < DP_ITEMS; ++k) c += (p0 + k < P && d[p0 + k] != 0);
+  c = Reduce(tmp).Sum(c);
+  if (threadIdx.x == 0) tile_count[(int64_t)f * T + t] = c;
+}
+
+// The reference's arithmetic (`point_cloud_extractor.py:51-75`), one rounding per operation:
+//   d = depth / 1000, X = ((u - cx) d) / fx + bx, Y = ((v - cy) d) / fy + by, Z = d,
+//   w_r = ((X P[r,0] + Y P[r,1]) + Z P[r,2]) + P[r,3]        (np.dot(points, pose.T) with the homogeneous 1 of `points`)
+// Pixel p goes to row tile_off[f * T + t] + (its rank among the tile's valid pixels).  A NaN coordinate sets the frame's flag.
+__global__ void __launch_bounds__(DP_THREADS) depth_write_kernel(const uint16_t* __restrict__ depth, int64_t W, int64_t P, int T,
+                                                                   double fx, double fy, double cx, double cy, double bx, double by,
+                                                                   const double* __restrict__ poses, const int64_t* __restrict__ tile_off,
+                                                                   double* __restrict__ out, unsigned long long* __restrict__ nan_flag) {
+  __shared__ typename DpScan::TempStorage tmp;
+  __shared__ double pose[12];
+  const int f = blockIdx.y, t = blockIdx.x;
+  if (threadIdx.x < 12) pose[threadIdx.x] = poses[(int64_t)f * 16 + threadIdx.x];
+  const uint16_t* d = depth + f * P;
+  const int64_t p0 = (int64_t)t * DP_TILE + threadIdx.x * DP_ITEMS;
+  uint16_t z[DP_ITEMS];
+  int valid[DP_ITEMS], rank[DP_ITEMS];
+  for (int k = 0; k < DP_ITEMS; ++k) {
+    z[k] = p0 + k < P ? d[p0 + k] : (uint16_t)0;
+    valid[k] = z[k] != 0;
+  }
+  DpScan(tmp).ExclusiveSum(valid, rank);
+  __syncthreads();                                            // the pose in shared memory
+  const int64_t base = tile_off[(int64_t)f * T + t];
+  bool nan = false;
+  for (int k = 0; k < DP_ITEMS; ++k) {
+    if (!valid[k]) continue;
+    const int64_t p = p0 + k;
+    const double u = (double)(p % W), v = (double)(p / W);
+    const double Z = __ddiv_rn((double)z[k], 1000.0);
+    const double X = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(u, cx), Z), fx), bx);
+    const double Y = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(v, cy), Z), fy), by);
+    double* o = out + 3 * (base + rank[k]);
+    for (int r = 0; r < 3; ++r) {
+      const double* P4 = pose + 4 * r;
+      const double w = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(X, P4[0]), __dmul_rn(Y, P4[1])), __dmul_rn(Z, P4[2])), P4[3]);
+      nan |= isnan(w);
+      o[r] = w;
+    }
+  }
+  if (__syncthreads_or(nan) && threadIdx.x == 0) atomicOr(&nan_flag[f], 1ull);
+}
+
+// offsets[f] = tile_off[f * T] for f <= F, to the device output and the host stage
+__global__ void depth_offsets_kernel(const int64_t* __restrict__ tile_off, int F, int T, int64_t* __restrict__ offsets,
+                                     int64_t* __restrict__ stage) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > F) return;
+  offsets[f] = stage[f] = tile_off[(int64_t)f * T];
+}
+
+// tile counts and their exclusive scan (F T + 1 entries: the last count is 0, so its offset is the total), the scan's temporary
+// storage, stage[2 F + 1]: the offsets, then the per-frame NaN flags, one copy to the host
+struct DepthWs { int64_t* count; int64_t* off; void* cub; size_t cub_bytes; int64_t* stage; };
+DepthWs depth_layout(Carve& c, int64_t F, int64_t T) {
+  const int64_t m = F * T + 1;
+  size_t cub_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (int64_t*)nullptr, (int64_t*)nullptr, (int)m);
+  DepthWs w{c.take<int64_t>(m), c.take<int64_t>(m), nullptr, cub_bytes, nullptr};
+  w.cub = c.take<char>(cub_bytes);
+  w.stage = c.take<int64_t>(2 * F + 1);
+  return w;
+}
+
+int64_t depth_tiles(int64_t H, int64_t W) { return (H * W + DP_TILE - 1) / DP_TILE; }
+bool depth_shape_ok(int64_t F, int64_t H, int64_t W) {
+  return F >= 1 && F <= MAX_FRAMES && H >= 1 && H <= DP_MAX_SIDE && W >= 1 && W <= DP_MAX_SIDE && F * depth_tiles(H, W) < (1ll << 31) - 1;
+}
+
 }  // namespace
 
 extern "C" size_t pcb_voxel_down_sample_ws_bytes(int64_t n, int64_t F) {
@@ -278,4 +371,38 @@ extern "C" int pcb_frame_overlap(const double* xyz, int64_t n, const int64_t* of
                                                                       (uint64_t)w.r.tcap - 1, w.r.start, w.r.end, w.sxyz, w.sframe,
                                                                       (unsigned long long*)counts);
   return check_launch("overlap_kernel");
+}
+
+extern "C" size_t pcb_depth_to_points_ws_bytes(int64_t F, int64_t H, int64_t W) {
+  if (!depth_shape_ok(F, H, W)) return 0;
+  return layout_bytes(depth_layout, F, depth_tiles(H, W));
+}
+
+extern "C" int pcb_depth_to_points(const uint16_t* depth, int64_t F, int64_t H, int64_t W, double fx, double fy, double cx, double cy,
+                                   double bx, double by, const double* poses, double* out, int64_t* out_offsets, int64_t* out_offsets_host,
+                                   int32_t* nan_host, void* ws, size_t ws_bytes, void* stream) {
+  PCB_ARG(depth_shape_ok(F, H, W));
+  const int64_t T = depth_tiles(H, W), P = H * W;
+  Carve c{(char*)ws};
+  const DepthWs w = depth_layout(c, F, T);
+  PCB_ARG(depth && poses && out && out_offsets && out_offsets_host && nan_host && ws && ws_bytes >= c.used);
+  cudaStream_t st = (cudaStream_t)stream;
+  PCB_CUDA(cudaMemsetAsync(w.count + F * T, 0, sizeof(int64_t), st));
+  PCB_CUDA(cudaMemsetAsync(w.stage + F + 1, 0, F * sizeof(int64_t), st));
+  const dim3 grid((unsigned)T, (unsigned)F);
+  depth_count_kernel<<<grid, DP_THREADS, 0, st>>>(depth, P, (int)T, w.count);
+  if (int e = check_launch("depth_count_kernel")) return e;
+  size_t cb = w.cub_bytes;
+  PCB_CUDA(cub::DeviceScan::ExclusiveSum(w.cub, cb, w.count, w.off, (int)(F * T + 1), st));
+  depth_write_kernel<<<grid, DP_THREADS, 0, st>>>(depth, W, P, (int)T, fx, fy, cx, cy, bx, by, poses, w.off, out,
+                                                  (unsigned long long*)(w.stage + F + 1));
+  if (int e = check_launch("depth_write_kernel")) return e;
+  depth_offsets_kernel<<<blocks_for(F + 1, 256), 256, 0, st>>>(w.off, (int)F, (int)T, out_offsets, w.stage);
+  if (int e = check_launch("depth_offsets_kernel")) return e;
+  std::vector<int64_t> host((size_t)(2 * F + 1));
+  PCB_CUDA(cudaMemcpyAsync(host.data(), w.stage, (2 * F + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  PCB_CUDA(cudaStreamSynchronize(st));
+  std::copy(host.begin(), host.begin() + F + 1, out_offsets_host);
+  for (int64_t f = 0; f < F; ++f) nan_host[f] = (int32_t)host[F + 1 + f];
+  return PCB_OK;
 }

@@ -7,6 +7,9 @@ correspondences indexing rows of the *batched* feature matrices (`:85-91`).
 
 Host-side numpy/scipy only; no CUDA and no oracle involved.
 """
+import struct
+import zlib
+
 import numpy as np
 from scipy.spatial import cKDTree
 
@@ -183,6 +186,38 @@ def synth_votenet_batch(seed, batch_size, num_points, scale=1.5):
     return out
 
 
+def _scan_rects(scale):
+    """The closed room of the scan walks (the `synth_room` surfaces and the two other walls), as plane arrays O, U, V, N at `scale`."""
+    rects = _rects() + [tuple(np.asarray(a, np.float64) for a in r) for r in (((_W, 0, 0), (0, _L, 0), (0, 0, _H)),      # wall x=W
+                                                                            ((0, _L, 0), (_W, 0, 0), (0, 0, _H)))]     # wall y=L
+    O, U, V = (np.stack([r[k] for r in rects]) * scale for k in range(3))
+    return O, U, V, np.cross(U, V)
+
+
+def _walk_pose(yaw, phase, scale):
+    """The camera of the scan walks: on a circle around the room centre at 60 % of the wall height, looking 20 degrees down in
+    direction `yaw`.  Returns (position, look, side, up)."""
+    centre = np.array([_W / 2, _L / 2, 0.6 * _H]) * scale
+    pos = centre + np.array([0.2 * _W * np.cos(phase), 0.2 * _L * np.sin(phase), 0.0]) * scale
+    look = np.array([np.cos(yaw), np.sin(yaw), -np.tan(np.deg2rad(20.0))])
+    look /= np.linalg.norm(look)
+    side = np.cross(look, [0.0, 0.0, 1.0])
+    side /= np.linalg.norm(side)
+    return pos, look, side, np.cross(side, look)
+
+
+def _first_hit(rays, pos, planes):
+    """The ray parameter of the nearest surface each ray (rows of `rays`, from `pos`) hits, inf where it hits none."""
+    O, U, V, N = planes
+    uu, vv = np.einsum("ij,ij->i", U, U), np.einsum("ij,ij->i", V, V)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        t = ((O - pos) * N).sum(1) / (rays @ N.T)                       # [m, rects]: the ray's parameter at each plane
+        a = (((pos - O) * U).sum(1) + t * (rays @ U.T)) / uu            # the hit point in the rectangle's (u, v) coordinates
+        b = (((pos - O) * V).sum(1) + t * (rays @ V.T)) / vv
+        t = np.where((t > 0) & (a >= 0) & (a <= 1) & (b >= 0) & (b <= 1), t, np.inf)
+    return t.min(1)
+
+
 def synth_scan_frames(seed, n_frames, points_per_frame=250_000, scale=2.0, half_angle_deg=30.0):
     """A depth-camera walk through a `synth_room`-style room (at `scale`): n_frames fp64 [points_per_frame, 3] world-frame clouds, the
     `pcd` of ScanNet's `<scene>/pcd/<frame>.npz` (about 250k points, like a 640x480 depth frame).  Frame k casts rays uniformly over a
@@ -190,34 +225,19 @@ def synth_scan_frames(seed, n_frames, points_per_frame=250_000, scale=2.0, half_
     every ray hits one), + N(0, 5 mm) noise.  The camera circles the room centre at 60 % of the wall height, looking 20 degrees down, and turns
     10-50 degrees between frames, so consecutive frames overlap by amounts on both sides of the pair list's 0.3 threshold."""
     rng = np.random.default_rng(seed)
-    rects = _rects() + [tuple(np.asarray(a, np.float64) for a in r) for r in (((_W, 0, 0), (0, _L, 0), (0, 0, _H)),      # wall x=W
-                                                                                ((0, _L, 0), (_W, 0, 0), (0, 0, _H)))]     # wall y=L
-    O, U, V = (np.stack([r[k] for r in rects]) * scale for k in range(3))
-    N = np.cross(U, V)
-    uu, vv = np.einsum("ij,ij->i", U, U), np.einsum("ij,ij->i", V, V)
-    centre = np.array([_W / 2, _L / 2, 0.6 * _H]) * scale
+    planes = _scan_rects(scale)
     cos_half = np.cos(np.deg2rad(half_angle_deg))
     yaw, phase = rng.random() * 2 * np.pi, rng.random() * 2 * np.pi
     frames = []
     for _ in range(n_frames):
-        pos = centre + np.array([0.2 * _W * np.cos(phase), 0.2 * _L * np.sin(phase), 0.0]) * scale
-        look = np.array([np.cos(yaw), np.sin(yaw), -np.tan(np.deg2rad(20.0))])
-        look /= np.linalg.norm(look)
-        side = np.cross(look, [0.0, 0.0, 1.0])
-        side /= np.linalg.norm(side)
-        up = np.cross(side, look)
+        pos, look, side, up = _walk_pose(yaw, phase, scale)
         got, parts, frac = 0, [], 0.5
         while got < points_per_frame:
             m = int(1.2 * (points_per_frame - got) / frac) + 1024
             c = 1.0 - rng.random(m) * (1.0 - cos_half)                      # uniform over the cone's solid angle
             s, phi = np.sqrt(1.0 - c * c), rng.random(m) * 2 * np.pi
             d = c[:, None] * look + (s * np.cos(phi))[:, None] * side + (s * np.sin(phi))[:, None] * up
-            with np.errstate(divide="ignore", invalid="ignore"):
-                t = ((O - pos) * N).sum(1) / (d @ N.T)                      # [m, rects]: the ray's parameter at each plane
-                a = (((pos - O) * U).sum(1) + t * (d @ U.T)) / uu           # the hit point in the rectangle's (u, v) coordinates
-                b = (((pos - O) * V).sum(1) + t * (d @ V.T)) / vv
-                t = np.where((t > 0) & (a >= 0) & (a <= 1) & (b >= 0) & (b <= 1), t, np.inf)
-            tmin = t.min(1)
+            tmin = _first_hit(d, pos, planes)
             keep = np.isfinite(tmin)
             frac = max(keep.mean(), 0.5)
             parts.append(pos + tmin[keep, None] * d[keep])
@@ -227,6 +247,81 @@ def synth_scan_frames(seed, n_frames, points_per_frame=250_000, scale=2.0, half_
         yaw += np.deg2rad(rng.uniform(10.0, 50.0))
         phase += np.deg2rad(rng.uniform(5.0, 20.0))
     return frames
+
+
+
+# ScanNet's depth camera (640 x 480; `_info.txt` of a scan): non-integral principal point
+SCANNET_DEPTH_INTRINSIC = np.array([[577.590698, 0.0, 318.905426, 0.0], [0.0, 578.729797, 242.683609, 0.0], [0.0, 0.0, 1.0, 0.0],
+                                    [0.0, 0.0, 0.0, 1.0]])
+SCANNET_COLOR_INTRINSIC = np.array([[1170.187988, 0.0, 647.75, 0.0], [0.0, 1170.187988, 483.75, 0.0], [0.0, 0.0, 1.0, 0.0],
+                                    [0.0, 0.0, 0.0, 1.0]])
+
+
+def write_sens(path, depth, poses, intrinsic_depth, seed=0, version=4, depth_compression=1, color_size=(1296, 968),
+               color_bytes=(90_000, 160_000)):
+    """A `.sens` file in the layout `SensorData.load` reads (`SensorData.py:57-79`): depth uint16 [F, H, W] zlib-compressed, poses
+    [F, 4, 4] stored as float32, the depth intrinsics and ScanNet's colour intrinsics, identity extrinsics.  Each frame's colour
+    payload is `color_bytes` random bytes (uniform in the range; a ScanNet JPEG is about that size), so that a loader that reads colour
+    pays for it.  `version` and `depth_compression` are written as given."""
+    depth = np.asarray(depth, np.uint16)
+    F, H, W = depth.shape
+    rng = np.random.default_rng(seed)
+    pool = rng.integers(0, 256, color_bytes[1], dtype=np.uint8).tobytes()
+    eye = np.eye(4, dtype=np.float32)
+    with open(path, "wb") as f:
+        name = b"StructureSensor"
+        f.write(struct.pack("<IQ", version, len(name)) + name)
+        for m in (SCANNET_COLOR_INTRINSIC, eye, intrinsic_depth, eye):
+            f.write(np.asarray(m, "<f4").tobytes())
+        f.write(struct.pack("<iiIIIIfQ", 2, depth_compression, color_size[0], color_size[1], W, H, 1000.0, F))
+        for i in range(F):
+            n = int(rng.integers(color_bytes[0], color_bytes[1] + 1))
+            start = int(rng.integers(0, color_bytes[1] - n + 1))
+            blob = zlib.compress(depth[i].astype("<u2").tobytes(), 1)
+            f.write(np.asarray(poses[i], "<f4").tobytes() + struct.pack("<QQQQ", 33_333 * i, 33_333 * i + 1, n, len(blob)))
+            f.write(pool[start:start + n])
+            f.write(blob)
+
+
+def synth_sens_scan(seed, n_frames, width=640, height=480, frames_per_view=1, render_every=1, holes=0.02, far=0.001, bad_poses=(),
+                    scale=2.0):
+    """A ScanNet-like depth scan for `write_sens`: (depth uint16 [n_frames, height, width] in millimetres, camera-to-world poses fp64
+    [n_frames, 4, 4], the 4 x 4 depth intrinsics).  The camera walks as in `synth_scan_frames` (room, circle, look direction), turning
+    1 / `frames_per_view` of that walk's step per frame; each frame renders the room through a pinhole with ScanNet's intrinsics
+    scaled to width x height (non-integral cx, cy; camera x right, y down, z forward), depth along the optical axis + N(0, 5 mm),
+    rounded to millimetres.  A `holes` share of the pixels is 0 (no reading) and a `far` share 65535 (the format's largest depth).
+    Frames f with f % render_every != 0 repeat the depth of the last rendered frame (a cheaper long scan).  The frames of `bad_poses`
+    get an all -inf pose, as ScanNet stores a frame without tracking."""
+    rng = np.random.default_rng(seed)
+    planes = _scan_rects(scale)
+    K = SCANNET_DEPTH_INTRINSIC.copy()
+    K[0] *= width / 640.0
+    K[1] *= height / 480.0
+    fx, fy, cx, cy = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
+    v, u = np.divmod(np.arange(height * width, dtype=np.float64), width)
+    cam = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u)], 1)          # the ray of each pixel in the camera frame, z = 1
+    yaw, phase = rng.random() * 2 * np.pi, rng.random() * 2 * np.pi
+    depth = np.empty((n_frames, height, width), np.uint16)
+    poses = np.empty((n_frames, 4, 4))
+    for i in range(n_frames):
+        pos, look, side, up = _walk_pose(yaw, phase, scale)
+        R = np.stack([side, -up, look], 1)
+        poses[i] = np.eye(4)
+        poses[i, :3, :3], poses[i, :3, 3] = R, pos
+        if i % render_every == 0:
+            z = _first_hit(cam @ R.T, pos, planes) + rng.normal(0.0, 0.005, height * width)
+            mm = np.where(np.isfinite(z), np.clip(np.rint(z * 1000.0), 0, 65535), 0)
+            r = rng.random(height * width)
+            mm[r < holes] = 0
+            mm[r > 1.0 - far] = 65535
+            depth[i] = mm.reshape(height, width)
+        else:
+            depth[i] = depth[i - 1]
+        yaw += np.deg2rad(rng.uniform(10.0, 50.0)) / frames_per_view
+        phase += np.deg2rad(rng.uniform(5.0, 20.0)) / frames_per_view
+    for i in bad_poses:
+        poses[i] = -np.inf
+    return depth, poses, K
 
 
 def synth_scene(seed, scale=2.5, voxel=0.05, n_raw=1_500_000):
