@@ -459,6 +459,67 @@ size_t pcb_det_ap_ws_bytes(int64_t D, int64_t G, int C, int T);
 int pcb_det_ap(const double* prop_corners, int64_t P, const int32_t* det_row, const int32_t* det_cls, const float* det_score,
                const int32_t* det_scan, int64_t D, const double* gt_corners, const int32_t* gt_scan, const int32_t* gt_cls, int64_t G, int C,
                const double* thresholds, int T, double* out, void* ws, size_t ws_bytes, void* stream);
+
+/* VoteNet's training loss (`downstream/votenet_det_new/models/loss_helper.py::get_loss` with `lib/utils/nn_distance.py`, DESIGN.md
+ * 8f-12).  Nothing synchronises; no floating-point atomics: every batch sum is fp64 in a fixed order, rounded once, so two calls give
+ * the same bits.  Per-element arithmetic is fp32 with one rounding per operation, as the original's torch ops round:
+ *   vote:        gt_j = vote_label[seed_inds] (j < 3) + seed_xyz; per GT vote the min over the V predicted votes of (|dx| + |dy|) + |dz|,
+ *                then the min over j (ties: smallest index, predicted vote first); sum(dist mask) / (sum(mask) + 1e-6).
+ *   assignment:  object_assignment = argmin_j ((dx dx + dy dy) + dz dz) from aggregated_vote_xyz to center_label[:, j, 0:3] over all K2
+ *                slots, padded zero slots included; e = sqrtf(d + 1e-6); objectness_label = e < 0.3, objectness_mask = label | e > 0.6.
+ *   objectness:  cross-entropy (row maximum subtracted) weighted [0.2, 0.8], masked mean.
+ *   center:      nn_distance(center, center_label) both ways: dist1 weighted by objectness_label, dist2 by box_label_mask.
+ *   heading / size / semantic: labels gathered through object_assignment; cross-entropy; Huber (delta 1) of the chosen residual minus
+ *                heading_residual_label * heading_scale, and of the chosen size residual minus size_residual_label / mean_size (mean of
+ *                the 3); each averaged over objectness_label.
+ * out fp32 [13] = (vote_loss, objectness_loss, center_loss, heading_cls_loss, heading_reg_loss, size_cls_loss, size_reg_loss,
+ * sem_cls_loss, box_loss, loss (x10), pos_ratio, neg_ratio, obj_acc).  A seed index outside [0, N) or a gathered heading, size or
+ * semantic class outside its range (where torch raises a device assert) reads nothing out of bounds and makes the affected terms NaN.
+ *
+ * Inputs, described once by pcb_det_loss_args: seed_xyz fp32 [B,S,3], seed_inds int32 or int64 (seed_inds_i64) [B,S], vote_xyz fp32
+ * [B,S*V,3], vote_label fp32 [B,N,9], vote_label_mask int64 [B,N], aggregated_vote_xyz fp32 [B,K,3] (all contiguous); the proposal head's
+ * outputs through their element strides (`decode_scores` slices them from one [B, X, K] tensor): center [B,K,3], objectness_scores
+ * [B,K,2], heading_scores / heading_residuals_normalized [B,K,NH], size_scores [B,K,NS], size_residuals_normalized [B,K,NS,3],
+ * sem_cls_scores [B,K,C]; labels center_label fp32 [B,K2,center_label_ld >= 3], heading_class_label / size_class_label /
+ * sem_cls_label int64 [B,K2], heading_residual_label fp32 [B,K2], size_residual_label fp32 [B,K2,3], box_label_mask fp32 [B,K2];
+ * mean_size HOST fp32 [NS, 3] (NS <= 64, copied into the launch); heading_scale = 1 / fp32(pi / NH), which is how torch divides an fp32
+ * tensor by a Python float on the GPU.
+ *
+ * pcb_det_loss_forward: out, objectness_label int64 [B,K], objectness_mask fp32 [B,K], object_assignment int64 [B,K], and `state`
+ * (pcb_det_loss_state_bytes: the argmins and denominators the backward reads; keep it until then).  Two launches.
+ * pcb_det_loss_backward: grad fp32 [13] = d/d out (box_loss and loss fold into the eight terms by their coefficients; the statistics
+ * carry none), with the forward's objectness_label, objectness_mask, object_assignment and state.  Writes dense fp32 gradients, each in
+ * full and each skipped when NULL: d_vote_xyz [B,S*V,3], d_seed_xyz [B,S,3], d_center [B,K,3], d_objectness_scores [B,K,2],
+ * d_heading_scores / d_heading_residuals_normalized [B,K,NH], d_size_scores [B,K,NS], d_size_residuals_normalized [B,K,NS,3],
+ * d_sem_cls_scores [B,K,C].  A min passes its gradient to the index it returned only, |x|' = 0 at 0, and the dist2 gradients of several
+ * ground-truth boxes on one proposal sum in ascending box order.  One launch.
+ * Both: a size below 1, B > 65535, NS > 64, center_label_ld < 3, B * max(S V, K, N) >= 2^31, NULL pointers and short ws / state
+ * return PCB_ERR_ARG before anything is launched.  ws: pcb_det_loss_ws_bytes (forward only). */
+typedef struct pcb_strided {
+  const float* p;
+  int64_t sb, sk, sc, sx;                    /* element strides of (scene, proposal, channel, xyz); sx only for size residuals */
+} pcb_strided;
+typedef struct pcb_det_loss_args {
+  int64_t B, S, V, N, K, K2;
+  int32_t NH, NS, C, seed_inds_i64;
+  float heading_scale;
+  const float* mean_size;
+  const float* seed_xyz; const void* seed_inds; const float* vote_xyz; const float* vote_label; const int64_t* vote_label_mask;
+  const float* aggregated_vote_xyz;
+  pcb_strided center, objectness_scores, heading_scores, heading_residuals_normalized, size_scores, size_residuals_normalized,
+      sem_cls_scores;
+  const float* center_label; int64_t center_label_ld;
+  const int64_t* heading_class_label; const float* heading_residual_label; const int64_t* size_class_label;
+  const float* size_residual_label; const int64_t* sem_cls_label; const float* box_label_mask;
+} pcb_det_loss_args;
+size_t pcb_det_loss_ws_bytes(int64_t B, int64_t S, int64_t K, int64_t K2);
+size_t pcb_det_loss_state_bytes(int64_t B, int64_t S, int64_t K, int64_t K2);
+int pcb_det_loss_forward(const pcb_det_loss_args* args, float* out, int64_t* objectness_label, float* objectness_mask,
+                         int64_t* object_assignment, void* state, size_t state_bytes, void* ws, size_t ws_bytes, void* stream);
+int pcb_det_loss_backward(const pcb_det_loss_args* args, const float* grad, const int64_t* objectness_label, const float* objectness_mask,
+                          const int64_t* object_assignment, const void* state, size_t state_bytes, float* d_vote_xyz, float* d_seed_xyz,
+                          float* d_center, float* d_objectness_scores, float* d_heading_scores, float* d_heading_residuals_normalized,
+                          float* d_size_scores, float* d_size_residuals_normalized, float* d_sem_cls_scores, void* stream);
 /* Row-wise L2 normalisation of the output features, y = x / ||x||_2 with no epsilon (`model/res16unet.py:262-266`), and its
  * backward dx = (dy - y (y.dy)) / ||x||.  inv_norm: [n] scratch written by forward, read by backward. */
 int pcb_l2norm_forward(const float* X, int64_t n, int C, float* Y, float* inv_norm, void* stream);

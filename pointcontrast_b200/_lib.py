@@ -24,6 +24,31 @@ def _load():
 lib = _load()
 
 _p, _i, _l, _f, _d, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double, C.c_size_t
+
+class PcbStrided(C.Structure):
+    """`struct pcb_strided` of include/pcb200.h: a float tensor read through its element strides (scene, proposal, channel, xyz)."""
+    _fields_ = [("p", _p), ("sb", _l), ("sk", _l), ("sc", _l), ("sx", _l)]
+
+
+class PcbDetLossArgs(C.Structure):
+    """`struct pcb_det_loss_args` of include/pcb200.h (field for field)."""
+    _fields_ = [
+        ("B", _l), ("S", _l), ("V", _l), ("N", _l), ("K", _l), ("K2", _l),
+        ("NH", C.c_int32), ("NS", C.c_int32), ("C", C.c_int32), ("seed_inds_i64", C.c_int32),
+        ("heading_scale", _f),
+        ("mean_size", _p),
+        ("seed_xyz", _p), ("seed_inds", _p), ("vote_xyz", _p), ("vote_label", _p), ("vote_label_mask", _p),
+        ("aggregated_vote_xyz", _p),
+        ("center", PcbStrided), ("objectness_scores", PcbStrided), ("heading_scores", PcbStrided),
+        ("heading_residuals_normalized", PcbStrided), ("size_scores", PcbStrided), ("size_residuals_normalized", PcbStrided),
+        ("sem_cls_scores", PcbStrided),
+        ("center_label", _p), ("center_label_ld", _l),
+        ("heading_class_label", _p), ("heading_residual_label", _p), ("size_class_label", _p),
+        ("size_residual_label", _p), ("sem_cls_label", _p), ("box_label_mask", _p),
+    ]
+
+
+_DLA = C.POINTER(PcbDetLossArgs)
 _SIGS = {
     "pcb_last_error": (C.c_char_p, []),
     "pcb_version": (C.c_char_p, []),
@@ -90,6 +115,10 @@ _SIGS = {
     "pcb_det_box_iou": (_i, [_p, _p, _l, _p, _p]),
     "pcb_det_ap_ws_bytes": (_sz, [_l, _l, _i, _i]),
     "pcb_det_ap": (_i, [_p, _l, _p, _p, _p, _p, _l, _p, _p, _p, _l, _i, _p, _i, _p, _p, _sz, _p]),
+    "pcb_det_loss_ws_bytes": (_sz, [_l, _l, _l, _l]),
+    "pcb_det_loss_state_bytes": (_sz, [_l, _l, _l, _l]),
+    "pcb_det_loss_forward": (_i, [_DLA, _p, _p, _p, _p, _p, _sz, _p, _sz, _p]),
+    "pcb_det_loss_backward": (_i, [_DLA, _p, _p, _p, _p, _p, _sz, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "pcb_profile_enable": (_i, [_i]),
     "pcb_profile_read": (_i, [_p, _p, _i, C.POINTER(C.c_int)]),
     "pcb_unit_ws_bytes": (_sz, [_i, _l, _l, _i, _i]),

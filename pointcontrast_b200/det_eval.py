@@ -361,7 +361,12 @@ class DetectionMetrics:
 def install(name="models.ap_helper"):
     """Register this module as `name` (and as the attribute of its parent package), so that `from models.ap_helper import
     APCalculator, parse_predictions, parse_groundtruths` -- VoteNet's lib/test.py and lib/train.py -- resolves here.  Returns the module."""
-    mod = sys.modules[__name__]
+    return register(sys.modules[__name__], name)
+
+
+def register(mod, name):
+    """Make `import name` resolve to mod: sys.modules[name], and the attribute of its parent package (created empty when it cannot be
+    imported).  Returns mod."""
     parent, _, child = name.rpartition(".")
     if parent:
         try:

@@ -186,6 +186,65 @@ def synth_votenet_batch(seed, batch_size, num_points, scale=1.5):
     return out
 
 
+def synth_votenet_loss_batch(seed, batch_size, num_points, num_seed, num_proposal, vote_factor, num_heading_bin, mean_size, num_class,
+                             max_obj=64, scale=1.5):
+    """A seeded labelled VoteNet batch with predictions: every `end_points` array `loss_helper.get_loss` reads, as numpy.
+
+    Labels follow `scannet_detection_dataset.py`: scene b is the room of `synth_votenet_batch(seed, ...)` with 3 to 12 random axis-aligned
+    boxes standing on its floor in the first slots of `max_obj`, the rest zero with box_label_mask 0; a point inside
+    a box votes for its centre (vote_label = centre - point, the 3 slots for the first 3 boxes that hold it, the first repeated) with
+    vote_label_mask 1.  Predictions stand in for the network: seeds a random subset (int32 seed_inds), votes near the true centres,
+    proposals (aggregated_vote_xyz) at votes, centres and scores with noise, half of the proposals near a box."""
+    rng = np.random.default_rng(seed)
+    B, N, S, K, V, NH, NS, C = batch_size, num_points, num_seed, num_proposal, vote_factor, num_heading_bin, len(mean_size), num_class
+    pc = synth_votenet_batch(seed, B, N, scale)
+    ep = {k: np.zeros(s, d) for k, s, d in (
+        ("vote_label", (B, N, 9), np.float32), ("vote_label_mask", (B, N), np.int64), ("center_label", (B, max_obj, 3), np.float32),
+        ("heading_class_label", (B, max_obj), np.int64), ("heading_residual_label", (B, max_obj), np.float32),
+        ("size_class_label", (B, max_obj), np.int64), ("size_residual_label", (B, max_obj, 3), np.float32),
+        ("sem_cls_label", (B, max_obj), np.int64), ("box_label_mask", (B, max_obj), np.float32))}
+    ep["point_clouds"] = pc
+    for b in range(B):
+        lo, hi = pc[b].min(0), pc[b].max(0)
+        boxes = []
+        for _ in range(rng.integers(3, 13)):
+            size = rng.uniform(0.3, 1.5, 3)
+            c = rng.uniform(lo + size / 2, hi - size / 2)
+            c[2] = lo[2] + size[2] / 2                                  # standing on the floor
+            boxes.append((c, size))
+        votes = [[] for _ in range(N)]
+        for j, (c, s) in enumerate(boxes):
+            sc = rng.integers(NS)
+            ep["center_label"][b, j] = c
+            ep["size_class_label"][b, j] = sc
+            ep["size_residual_label"][b, j] = s - np.asarray(mean_size, np.float32)[sc]
+            ep["heading_class_label"][b, j] = rng.integers(NH)
+            ep["heading_residual_label"][b, j] = rng.uniform(-np.pi / NH, np.pi / NH)
+            ep["sem_cls_label"][b, j] = rng.integers(C)
+            ep["box_label_mask"][b, j] = 1
+            for i in np.flatnonzero((np.abs(pc[b] - c) <= s / 2).all(1)):
+                votes[i].append(c - pc[b, i])
+        for i, v in enumerate(votes):
+            if v:
+                v = (v + [v[0]] * 3)[:3]
+                ep["vote_label"][b, i] = np.concatenate(v)
+                ep["vote_label_mask"][b, i] = 1
+    inds = np.stack([rng.choice(N, S, replace=False) for _ in range(B)]).astype(np.int32)
+    seed_xyz = np.take_along_axis(pc, inds[..., None].astype(np.int64), 1)
+    gt_vote = np.take_along_axis(ep["vote_label"], inds[..., None].astype(np.int64), 1)[:, :, :3]
+    vote_xyz = seed_xyz[:, :, None, :] + gt_vote[:, :, None, :] + rng.normal(0, 0.15, (B, S, V, 3))
+    agg = vote_xyz.reshape(B, S * V, 3)[np.arange(B)[:, None], np.stack([rng.choice(S * V, K, replace=K > S * V) for _ in range(B)])]
+    near = rng.random((B, K)) < 0.5
+    slot = np.stack([rng.integers(0, int(ep["box_label_mask"][b].sum()), K) for b in range(B)])
+    agg = np.where(near[..., None], ep["center_label"][np.arange(B)[:, None], slot] + rng.normal(0, 0.15, (B, K, 3)), agg)
+    ep.update(seed_inds=inds, seed_xyz=seed_xyz.astype(np.float32), vote_xyz=vote_xyz.reshape(B, S * V, 3).astype(np.float32),
+              aggregated_vote_xyz=agg.astype(np.float32), center=(agg + rng.normal(0, 0.1, (B, K, 3))).astype(np.float32))
+    for k, n in (("objectness_scores", (2,)), ("heading_scores", (NH,)), ("heading_residuals_normalized", (NH,)), ("size_scores", (NS,)),
+                 ("size_residuals_normalized", (NS, 3)), ("sem_cls_scores", (C,))):
+        ep[k] = rng.normal(0, 1.0 if k.endswith("scores") else 0.5, (B, K) + n).astype(np.float32)
+    return ep
+
+
 def _scan_rects(scale):
     """The closed room of the scan walks (the `synth_room` surfaces and the two other walls), as plane arrays O, U, V, N at `scale`."""
     rects = _rects() + [tuple(np.asarray(a, np.float64) for a in r) for r in (((_W, 0, 0), (0, _L, 0), (0, 0, _H)),      # wall x=W
