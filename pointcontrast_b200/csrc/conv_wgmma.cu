@@ -1,7 +1,7 @@
 // Hopper sparse convolution: the output-stationary gather-GEMM of conv.cu with the per-offset Cin x Cout contraction issued as
 // wgmma.mma_async, fp32 accumulators in registers.  CTA = 128 output rows x BN channels = one producer warpgroup and two consumer
 // warpgroups of M64.  The producer gathers the input, 16-bit hi/lo planes, per offset by cp.async (zero-filled where there is no
-// neighbour) into the K-major no-swizzle core-matrix layout, and fetches the weights, pre-tiled as shared-memory images, by one TMA
+// neighbour) into the 64-byte swizzled K-major layout, and fetches the weights, pre-tiled as shared-memory images, by one TMA
 // bulk copy per stage; both complete on the stage's mbarrier.  Per 32-channel step each consumer warpgroup issues 2 k16-steps x 3
 // products (lo.hi + hi.lo + hi.hi).  Offsets without a neighbour in the tile are skipped; small levels split the steps over
 // gridDim.z (partial planes + fixed-order reduce).  With a tile order `perm` (pcb_conv_tile_order), tile position i is output row
@@ -21,11 +21,13 @@ namespace hw {
 // 8 consumer warps, once wgmma.wait_group shows that the MMAs reading the slot have retired).
 constexpr int BM = 128, BK = 32, NPROD = 128, NCONS_WARPS = 8, NTHR = NPROD + 32 * NCONS_WARPS;
 constexpr int SMEM_OPTIN = 227 * 1024, SMEM_PER_SM = 228 * 1024;      // sm_90: largest dynamic shared memory of one CTA, of one SM
-constexpr int A_SBO = 128;
-// k8-chunk stride of the A tile: +32 bytes, so that the four 16-byte chunks (t & 3) x two rows (t >> 2) written by a quarter-warp of a
-// 128-bit st.shared cover eight different 16-byte slots of a 128-byte bank line.
-constexpr int A_LBO = (BM / 8) * 128 + 32;
-constexpr int A_PLANE = (BK / 8) * A_LBO;
+// A tile plane: the 64-byte swizzled K-major layout of wgmma (SWIZZLE_64B): tile row r's 32 channels are the 64 bytes at 64 r, its
+// 16-byte chunk c stored at chunk c ^ ((r >> 1) & 3).  The 8-row atoms (512 bytes) follow each other, and a k16 step starts 32 bytes
+// into the row.  A quarter-warp's copy (two rows x four chunks) covers one 128-byte bank line.
+constexpr int A_ROW = BK * 2, A_ATOM = 8 * A_ROW;
+constexpr int A_PLANE = BM * A_ROW;
+__device__ __forceinline__ uint32_t a_chunk(int r, int c) { return r * A_ROW + ((c ^ ((r >> 1) & 3)) << 4); }
+__device__ __forceinline__ uint64_t a_desc(uint32_t saddr) { return make_desc(saddr, 16, A_ATOM) | (2ull << 62); }   // layout type 2: 64B swizzle
 
 struct Args {
   const __nv_bfloat16* Xhi; const __nv_bfloat16* Xlo; int lds;      // the input as 16-bit hi/lo planes
@@ -51,7 +53,7 @@ struct Smem {
   static constexpr int B_SBO = 128;
   static constexpr int B_LBO = (BN / 8) * 128 + 16;
   static constexpr int B_PLANE = (BK / 8) * B_LBO;
-  static constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
+  static constexpr int STAGE = (2 * A_PLANE + 2 * B_PLANE + 511) / 512 * 512;   // A planes stay aligned to the 512-byte swizzle atom
   static constexpr int CTAS = BN <= 96 ? 2 : 1;                                  // resident CTAs per SM
   static constexpr int BUDGET = CTAS == 1 ? SMEM_OPTIN : SMEM_PER_SM / 2 - 1024;  // 1 KB per CTA is reserved by the system
   static constexpr int FIXED = PCB_MAX_KERNEL_VOLUME * BM * 4 + 72 * 4 + 16;
@@ -67,7 +69,7 @@ template <int BN, bool F16>
 __global__ void __launch_bounds__(NTHR, Smem<BN>::CTAS) conv_wgmma_kernel(const Args p) {
   using S = Smem<BN>;
   constexpr int NS = S::NS;
-  extern __shared__ __align__(128) unsigned char smem[];
+  extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2;
   const int64_t row0 = (int64_t)blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
@@ -153,7 +155,7 @@ __global__ void __launch_bounds__(NTHR, Smem<BN>::CTAS) conv_wgmma_kernel(const 
         const int r = r0 + 32 * q;
         const int idx = s_idx[k * BM + r];
         const int64_t off = (int64_t)(idx >= 0 ? idx : 0) * p.lds + kc * BK + k8 * 8;
-        const uint32_t dst = sb + k8 * A_LBO + (r >> 3) * A_SBO + (r & 7) * 16;
+        const uint32_t dst = sb + a_chunk(r, k8);
         cp_async16_zfill(dst, p.Xhi + off, idx >= 0 ? 16u : 0u);
         cp_async16_zfill(dst + A_PLANE, p.Xlo + off, idx >= 0 ? 16u : 0u);
       }
@@ -174,13 +176,13 @@ __global__ void __launch_bounds__(NTHR, Smem<BN>::CTAS) conv_wgmma_kernel(const 
       const int s = i % NS;
       mbar_wait(full_bar + 8 * s, (uint32_t)((i / NS) & 1));
       fence_proxy_async();                             // generic-proxy smem writes (cp.async) -> visible to the tensor cores
-      const uint32_t a_hi = smem_base + s * S::STAGE + h64 * 8 * A_SBO, a_lo = a_hi + A_PLANE;
+      const uint32_t a_hi = smem_base + s * S::STAGE + h64 * 64 * A_ROW, a_lo = a_hi + A_PLANE;
       const uint32_t b_hi = smem_base + s * S::STAGE + 2 * A_PLANE, b_lo = b_hi + S::B_PLANE;
       fence_regs(acc);
       wgmma_fence();
 #pragma unroll
       for (int j = 0; j < BK / 16; ++j) {
-        const uint64_t dah = make_desc(a_hi + j * 2 * A_LBO, A_LBO, A_SBO), dal = make_desc(a_lo + j * 2 * A_LBO, A_LBO, A_SBO);
+        const uint64_t dah = a_desc(a_hi + j * 32), dal = a_desc(a_lo + j * 32);
         const uint64_t dbh = make_desc(b_hi + j * 2 * S::B_LBO, S::B_LBO, S::B_SBO);
         const uint64_t dbl = make_desc(b_lo + j * 2 * S::B_LBO, S::B_LBO, S::B_SBO);
         wgmma<BN, F16, 0, 0>(acc, dal, dbh, 1u);

@@ -3,9 +3,12 @@ launch of one C1 training step (Res16UNet34C, 4 synthetic ScanNet-shape pairs at
 over windows of at least `--seconds` after warm-up, in the identity order and in the window-sorted order for each window of the sweep.
 Per shape it reports the kernel time, the kernel offsets a 128-row tile stages (of K) and the share of MMA rows that carry a real
 neighbour pair; `per_step_ms` weights each shape by how many units of the step issue it.  Offset-split launches (small levels) always run
-in the identity order and are left out.  Prints one JSON line.
+in the identity order and are left out.  Per shape `pool` describes how often the identity order's tiles read the same input row:
+distinct input rows per tile, gathers (entries with a neighbour) per distinct row, the largest row span of a tile, and the share of
+tiles that a shared-memory pool of POOL_ROWS distinct rows within POOL_SPAN rows could not hold (the pool measured in DESIGN.md
+section 7).  Prints one JSON line.
 
-    python profiles/bench_conv_order.py [--seconds 1.0]
+    python profiles/bench_conv_order.py [--seconds 1.0] [--windows 4096,8192,16384,0]
 """
 import argparse
 import json
@@ -24,7 +27,8 @@ from pointcontrast_b200.data import to_torch  # noqa: E402
 from pointcontrast_b200.model import load_model  # noqa: E402
 
 BM = 128
-WINDOWS = (4096, 8192, 16384, 0)          # 0: the whole level is one window
+WINDOWS = "4096,8192,16384,0"             # 0: the whole level is one window
+POOL_ROWS, POOL_SPAN = 512, 4096          # one 32-channel chunk of 512 rows, hi and lo planes: 64 KB of shared memory
 
 
 def gpu_info():
@@ -52,6 +56,20 @@ def tile_stats(mask, order):
     return float(nk.mean()), float(pairs / (nk.sum() * BM))
 
 
+def pool_stats(t):
+    """Row-pool view of the identity order's 128-row tiles of table t [K, n] (-1: no neighbour)."""
+    K, n = t.shape
+    m = np.concatenate([t, np.full((K, -n % BM), -1, t.dtype)], axis=1).reshape(K, -1, BM).transpose(1, 0, 2).reshape(-1, K * BM)
+    m = np.sort(m, axis=1)
+    valid = m >= 0
+    distinct = (valid & np.concatenate([np.ones((len(m), 1), bool), m[:, 1:] != m[:, :-1]], axis=1)).sum(1)
+    span = np.where(valid.any(1), m.max(1) - np.where(valid, m, np.iinfo(m.dtype).max).min(1), 0)
+    fallback = (span >= POOL_SPAN) | (distinct > POOL_ROWS)
+    return {"distinct_rows_mean": round(float(distinct.mean()), 1), "distinct_rows_max": int(distinct.max()),
+            "gathers_per_distinct_row": round(float(valid.sum() / max(int(distinct.sum()), 1)), 2), "span_max": int(span.max()),
+            "fallback_share": round(float(fallback.mean()), 4)}
+
+
 def time_launch(fn, seconds):
     """ms per call of fn, from CUDA events around enough back-to-back calls to fill `seconds`."""
     for _ in range(3):
@@ -74,6 +92,7 @@ def time_launch(fn, seconds):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--seconds", type=float, default=1.0, help="least timed window per (shape, order)")
+    ap.add_argument("--windows", default=WINDOWS, help="tile-order windows to time besides the identity order (comma list, may be empty)")
     args = ap.parse_args()
     dev = torch.device("cuda", torch.cuda.current_device())
     torch.manual_seed(0)
@@ -111,10 +130,10 @@ def main():
         t = tbl[:, :n_out].cpu().numpy()
         mask = ((t >= 0).astype(np.int64) << np.arange(K)[:, None]).sum(0)
         orders = {"identity": None}
-        for w in WINDOWS:
+        for w in (int(v) for v in args.windows.split(",") if v.strip()):
             orders[str(w) if w else "level"] = tile_order(tbl, n_out, w if w else -(-n_out // BM) * BM)
         rec = {"role": role, "K": K, "Cin": Ck, "Cout": N, "rows": n_out, "units_per_step": count, "ms": {}, "offsets_per_tile": {},
-               "useful_rows": {}}
+               "useful_rows": {}, "pool": pool_stats(t)}
         ref = None
         for name, perm in orders.items():
             def call(perm=perm):
