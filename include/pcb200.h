@@ -520,6 +520,67 @@ int pcb_det_loss_backward(const pcb_det_loss_args* args, const float* grad, cons
                           const int64_t* object_assignment, const void* state, size_t state_bytes, float* d_vote_xyz, float* d_seed_xyz,
                           float* d_center, float* d_objectness_scores, float* d_heading_scores, float* d_heading_residuals_normalized,
                           float* d_size_scores, float* d_size_residuals_normalized, float* d_sem_cls_scores, void* stream);
+
+/* ----------------------------------------------------------------------------------------------- VoteNet detection data (det_data.cu)
+ * A batch of B ScanNet or SUN RGB-D detection scenes (`lib/datasets/{scannet,sunrgbd}/*_detection_dataset.py` `__getitem__`) as ragged
+ * rows: scene b's source points are rows [offsets[b], offsets[b+1]) of the concatenated arrays (every scene non-empty), its boxes rows
+ * [box_offsets[b], box_offsets[b+1]) of `boxes` (at most PCB_DET_MAX_OBJ).  Offsets are given twice, on the host (checked: start at 0,
+ * monotone, end at M / the box count) and on the device (read by the kernels).  Arithmetic is the original's: fp32 where numpy's is fp32,
+ * fp64 where it is fp64, one rounding per operation and no contraction; its 3-term dot products sum in index order.
+ *
+ * pcb_det_floor_height: floor[b] = np.percentile(z of scene b, 0.99) with numpy's `linear` rule (virtual index (n-1) q in the data's type,
+ * a + (b-a) t, or b - (b-a)(1-t) where t >= 0.5), z read at element stride `stride` from fp32 (f64 = 0) or fp64 (f64 = 1) rows; the
+ * result is exact in fp64.  Two order statistics by radix selection, one CTA per scene, one launch.
+ * pcb_det_choices: out [B, k] int64 scene-local indices, `np.random.choice(n_b, k, replace=n_b < k)`: the first k of a random order of
+ * the scene (sorted random 64-bit keys, the scene's bits on top) when n_b >= k, else k iid uniform indices; from a Philox4x32-10 stream
+ * keyed by (seed, offset), so equal generator states give equal sets.  ws: pcb_det_choices_ws_bytes(M).
+ * pcb_det_points: the sampled rows' point_clouds fp32 [B, k, C], vote_label fp32 [B, k, 9], vote_label_mask int64 [B, k] and, ScanNet,
+ * pcl_color fp32 [B, k, 3].  ScanNet: flips, z-rotation (fp64, rounded to fp32) and the floor height column; then the instance votes:
+ * per (scene, instance id) the fp32 min / max of the sampled rows (order-independent atomics), applied when the semantic label of the
+ * instance's first sampled row is in nyu40ids.  SUN RGB-D: flip, rotation of points and vote end points, colour, scale, all fp64.
+ * A choice outside [0, n_b) reads nothing out of bounds: its row takes the scene's first point and NaN coordinates.
+ * ws: pcb_det_points_ws_bytes(B, k).
+ * pcb_det_boxes: the box labels of every scene in fp64, one launch: center_label fp32 [B,64,3], heading_class_label int64 [B,64],
+ * heading_residual_label fp32 [B,64], size_class_label int64 [B,64], size_residual_label fp32 [B,64,3], sem_cls_label int64 [B,64],
+ * box_label_mask fp32 [B,64] and, SUN RGB-D, max_gt_bboxes fp64 [B,64,8].
+ * Sizes below 1, B * k >= 2^31, M >= 2^31, bad offsets, a scene with more than 64 boxes, NULL pointers and short ws return PCB_ERR_ARG
+ * before anything is launched. */
+#define PCB_DET_MAX_OBJ 64
+#define PCB_DET_SCANNET 0
+#define PCB_DET_SUNRGBD 1
+#define PCB_DET_HEIGHT 1          /* pcb_det_batch.flags: a floor-height column */
+#define PCB_DET_COLOR 2           /* colour columns (SUN RGB-D only) */
+#define PCB_DET_AUGMENT 4         /* apply the per-scene draws in `params` */
+#define PCB_DET_NPARAM 11         /* params per scene: flip_x, flip_y, cos, sin of the rotation, scale, brightness[3], shift[3] */
+typedef struct pcb_det_batch {
+  int64_t B, M, num_points;                  /* scenes, source rows in all, sampled rows per scene (k) */
+  int32_t dataset, flags;                    /* PCB_DET_SCANNET / PCB_DET_SUNRGBD, PCB_DET_* flags */
+  const int64_t* offsets_host; const int64_t* offsets;              /* [B + 1] */
+  const int64_t* box_offsets_host; const int64_t* box_offsets;      /* [B + 1] */
+  const double* params;                      /* [B, PCB_DET_NPARAM] */
+  const double* floor;                       /* [B] pcb_det_floor_height (PCB_DET_HEIGHT) */
+  const int64_t* choices;                    /* [B, k] pcb_det_choices */
+  const float* vert; const uint32_t* sem; const uint32_t* ins;      /* ScanNet: [M, 6], [M], [M] */
+  const double* pc; const double* votes;     /* SUN RGB-D: [M, 6], [M, 10] */
+  const double* jitter; const double* dropout;                      /* SUN RGB-D colour draws [M] (PCB_DET_COLOR with augmentation) */
+  const double* boxes;                       /* [box count, 7] (ScanNet) or [box count, 8] (SUN RGB-D) */
+  const double* headings;                    /* SUN RGB-D [box count, 3]: augmented heading, cos and sin of minus it (numpy's values) */
+  const int64_t* nyu40ids; int32_t n_ids;    /* ScanNet: the detected nyu40 ids */
+  int32_t num_heading_bin;
+  const double* mean_size; int32_t n_size;   /* [n_size, 3] */
+  int32_t pad_;
+  float* point_clouds; float* pcl_color; float* vote_label; int64_t* vote_label_mask;
+  float* center_label; int64_t* heading_class_label; float* heading_residual_label; int64_t* size_class_label;
+  float* size_residual_label; int64_t* sem_cls_label; float* box_label_mask; double* max_gt_bboxes;
+} pcb_det_batch;
+int pcb_det_floor_height(const void* z, int64_t stride, int32_t f64, const int64_t* offsets_host, const int64_t* offsets, int64_t B,
+                         double* floor, void* stream);
+size_t pcb_det_choices_ws_bytes(int64_t M);
+int pcb_det_choices(const int64_t* offsets_host, const int64_t* offsets, int64_t B, int64_t k, uint64_t seed, uint64_t offset, int64_t* out,
+                    void* ws, size_t ws_bytes, void* stream);
+size_t pcb_det_points_ws_bytes(int64_t B, int64_t k);
+int pcb_det_points(const pcb_det_batch* a, void* ws, size_t ws_bytes, void* stream);
+int pcb_det_boxes(const pcb_det_batch* a, void* stream);
 /* Row-wise L2 normalisation of the output features, y = x / ||x||_2 with no epsilon (`model/res16unet.py:262-266`), and its
  * backward dx = (dy - y (y.dy)) / ||x||.  inv_norm: [n] scratch written by forward, read by backward. */
 int pcb_l2norm_forward(const float* X, int64_t n, int C, float* Y, float* inv_norm, void* stream);

@@ -48,7 +48,23 @@ class PcbDetLossArgs(C.Structure):
     ]
 
 
+class PcbDetBatch(C.Structure):
+    """`struct pcb_det_batch` of include/pcb200.h (field for field)."""
+    _fields_ = [
+        ("B", _l), ("M", _l), ("num_points", _l), ("dataset", C.c_int32), ("flags", C.c_int32),
+        ("offsets_host", _p), ("offsets", _p), ("box_offsets_host", _p), ("box_offsets", _p),
+        ("params", _p), ("floor", _p), ("choices", _p),
+        ("vert", _p), ("sem", _p), ("ins", _p), ("pc", _p), ("votes", _p), ("jitter", _p), ("dropout", _p),
+        ("boxes", _p), ("headings", _p), ("nyu40ids", _p), ("n_ids", C.c_int32), ("num_heading_bin", C.c_int32),
+        ("mean_size", _p), ("n_size", C.c_int32), ("pad_", C.c_int32),
+        ("point_clouds", _p), ("pcl_color", _p), ("vote_label", _p), ("vote_label_mask", _p),
+        ("center_label", _p), ("heading_class_label", _p), ("heading_residual_label", _p), ("size_class_label", _p),
+        ("size_residual_label", _p), ("sem_cls_label", _p), ("box_label_mask", _p), ("max_gt_bboxes", _p),
+    ]
+
+
 _DLA = C.POINTER(PcbDetLossArgs)
+_DDB = C.POINTER(PcbDetBatch)
 _SIGS = {
     "pcb_last_error": (C.c_char_p, []),
     "pcb_version": (C.c_char_p, []),
@@ -119,6 +135,12 @@ _SIGS = {
     "pcb_det_loss_state_bytes": (_sz, [_l, _l, _l, _l]),
     "pcb_det_loss_forward": (_i, [_DLA, _p, _p, _p, _p, _p, _sz, _p, _sz, _p]),
     "pcb_det_loss_backward": (_i, [_DLA, _p, _p, _p, _p, _p, _sz, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "pcb_det_floor_height": (_i, [_p, _l, C.c_int32, _p, _p, _l, _p, _p]),
+    "pcb_det_choices_ws_bytes": (_sz, [_l]),
+    "pcb_det_choices": (_i, [_p, _p, _l, _l, C.c_uint64, C.c_uint64, _p, _p, _sz, _p]),
+    "pcb_det_points_ws_bytes": (_sz, [_l, _l]),
+    "pcb_det_points": (_i, [_DDB, _p, _sz, _p]),
+    "pcb_det_boxes": (_i, [_DDB, _p]),
     "pcb_profile_enable": (_i, [_i]),
     "pcb_profile_read": (_i, [_p, _p, _i, C.POINTER(C.c_int)]),
     "pcb_unit_ws_bytes": (_sz, [_i, _l, _l, _i, _i]),
@@ -190,6 +212,9 @@ CONV_FORCE_SIMT, CONV_ACCUMULATE = 1, 4               # flags of the convolution
 PLANES_A_FP16, PLANES_B_FP16 = 8, 16                  # flags: 16-bit plane formats of the split-operand calls
 BN_RELU = 1                                           # flag of pcb_bn_apply_seg
 UNIT_SEPARATE_STATS, UNIT_FP16_FORWARD, UNIT_EVAL = 1, 2, 4     # pcb_unit.flags
+DET_MAX_OBJ, DET_NPARAM = 64, 11                      # detection data: box slots per scene, params per scene
+DET_SCANNET, DET_SUNRGBD = 0, 1                       # pcb_det_batch.dataset
+DET_HEIGHT, DET_COLOR, DET_AUGMENT = 1, 2, 4          # pcb_det_batch.flags
 EXPORTS = sorted(_SIGS)
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)          # AttributeError here == the library does not export a declared symbol

@@ -11,7 +11,7 @@ CPU worker per loader.
 Randomness: scalar decisions (gates, angles, scale, blend factor, translation) come from Python `random` / `np.random` in the
 reference's call order; arrays (the elastic noise grid, the jitter noise, the dropout index set) from a `torch.Generator` on the
 device.  Both go through a `Draws` object, so a `ReplayDraws` of a recorded sequence reproduces a scene exactly, and every
-transform's `apply` also takes its draws as arguments.
+transform's `apply` also takes its draws as arguments.  `det_data` (the VoteNet detection loader) draws through the same objects.
 """
 import ctypes
 import logging
@@ -107,10 +107,34 @@ class Draws:
         """`np.random.choice(n, k, replace=False)`: k distinct indices in random order (int64, device)."""
         return torch.randperm(n, generator=self.generator, device=self.device)[:k]
 
+    def rand_device(self, n):
+        """`np.random.random(n)` on the device: fp64 uniform [0, 1) [n]."""
+        return torch.rand(int(n), generator=self.generator, device=self.device, dtype=torch.float64)
+
+    def choices(self, ns, k):
+        """`np.random.choice(n, k, replace=n < k)` for every scene size n in `ns`, in one call: int64 [len(ns), k] scene-local indices on
+        the device.  A scene with n >= k gets a uniformly random ordered k-subset (no repeats), a smaller one k iid indices.  The sets
+        come from `pcb_det_choices`, a Philox stream keyed by the generator's seed and offset, which the call advances: equal generator
+        states give equal sets."""
+        off = np.zeros(len(ns) + 1, np.int64)
+        off[1:] = np.cumsum(np.asarray(ns, np.int64))
+        if len(ns) == 0 or int(k) < 1 or (np.diff(off) < 1).any():
+            raise ValueError(f"choices: every scene needs a point and k >= 1 (sizes {list(ns)}, k {k})")
+        seed, offset = self.generator.initial_seed(), self.generator.get_offset()
+        self.generator.set_offset(offset + 4)
+        out = torch.empty(len(ns), int(k), dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            d_off = torch.from_numpy(off).to(self.device)
+            wsb = lib.pcb_det_choices_ws_bytes(int(off[-1]))
+            ws = workspace(wsb, self.device)
+            check(lib.pcb_det_choices(off.ctypes.data, ptr(d_off), len(ns), int(k), seed & (2 ** 64 - 1), offset, ptr(out), ptr(ws), wsb,
+                                      stream()))
+        return out
+
 
 class ReplayDraws:
     """Replays a recorded sequence of draws [(kind, value), ...] (kinds: random, uniform, rand, shuffle (the permutation), randn,
-    choice), checking that the calls come in the recorded order."""
+    choice, rand_device, choices (one index array per scene)), checking that the calls come in the recorded order."""
 
     def __init__(self, record, device="cuda"):
         self.record, self.pos, self.device = list(record), 0, torch.device(device)
@@ -148,6 +172,18 @@ class ReplayDraws:
         v = torch.as_tensor(np.asarray(self._next("choice"), np.int64))
         assert len(v) == k
         return v.to(self.device)
+
+    def rand_device(self, n):
+        v = torch.as_tensor(np.asarray(self._next("rand_device"), np.float64))
+        assert tuple(v.shape) == (int(n),)
+        return v.to(self.device)
+
+    def choices(self, ns, k):
+        v = [np.asarray(c, np.int64) for c in self._next("choices")]
+        assert len(v) == len(ns) and all(c.shape == (int(k),) for c in v)
+        if any(len(c) and (c.min() < 0 or c.max() >= n) for c, n in zip(v, ns)):
+            raise ValueError("replay: a recorded choice set is outside its scene")
+        return torch.from_numpy(np.stack(v)).to(self.device)
 
 
 _DEFAULT = {}

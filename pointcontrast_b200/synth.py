@@ -392,3 +392,54 @@ def synth_scene(seed, scale=2.5, voxel=0.05, n_raw=1_500_000):
     f = (rng.integers(0, 256, size=(len(c), 3)).astype(np.float32) / 255.0 - 0.5)
     C = np.concatenate([np.zeros((len(c), 1), np.int32), c], 1)
     return {"coords": C, "feats": f}
+
+
+# ScanNet nyu40 ids of the detected classes (`model_util_scannet.py`), used when no config is given
+SCANNET_NYU40IDS = (3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 14, 16, 24, 28, 33, 34, 36, 39)
+
+
+def write_scannet_detection_scene(path, name, seed, n, n_boxes, n_inst=8, nyu40ids=SCANNET_NYU40IDS):
+    """`<path>/<name>_{vert,sem_label,ins_label,bbox}.npy` in the format of the original preprocessing (`batch_load_scannet_data.py`):
+    vert fp32 [n, 6] (xyz in a 6 x 5 x 3 m room, colour 0-255), sem / ins labels uint32 [n], bbox fp64 [n_boxes, 7] (centre, size,
+    nyu40 id).  Instance ids are arbitrary uint32 values: 0 (unannotated) and ids near 2^32 are always present.  The last instance mixes
+    object and non-object semantic labels row by row, so whether it gets votes depends on its first sampled row."""
+    rng = np.random.default_rng(seed)
+    xyz = rng.uniform((-3, -2.5, 0), (3, 2.5, 3), (n, 3)).astype(np.float32)
+    rgb = rng.integers(0, 256, (n, 3)).astype(np.float32)
+    ids = np.unique(np.concatenate([[0, 4294967295, 2147483648 + seed],
+                                    rng.choice(4294967000, max(n_inst - 3, 0), replace=False)]).astype(np.uint32))
+    ins = ids[rng.integers(0, len(ids), n)].astype(np.uint32)
+    sem_of = {int(i): (int(rng.choice(nyu40ids)) if rng.random() < 0.8 else int(rng.choice([1, 2, 22, 40]))) for i in ids}
+    sem = np.array([sem_of[int(i)] for i in ins], np.uint32)
+    mixed = ins == ids[-1]
+    sem[mixed] = np.where(rng.random(int(mixed.sum())) < 0.5, nyu40ids[0], 1).astype(np.uint32)
+    bbox = np.zeros((n_boxes, 7))
+    bbox[:, 0:3] = rng.uniform((-2.5, -2, 0.2), (2.5, 2, 2.5), (n_boxes, 3))
+    bbox[:, 3:6] = rng.uniform(0.2, 2.0, (n_boxes, 3))
+    bbox[:, 6] = rng.choice(nyu40ids, n_boxes)
+    np.save(f"{path}/{name}_vert.npy", np.concatenate([xyz, rgb], 1))
+    np.save(f"{path}/{name}_sem_label.npy", sem)
+    np.save(f"{path}/{name}_ins_label.npy", ins)
+    np.save(f"{path}/{name}_bbox.npy", bbox)
+
+
+def write_sunrgbd_detection_scene(path, name, seed, n, n_boxes, n_class=10):
+    """`<path>/<name>_pc.npz` (pc fp64 [n, 6], colour in 0-1), `<name>_bbox.npy` fp64 [n_boxes, 8] (centre, half sizes, heading, class)
+    and `<name>_votes.npz` (point_votes fp64 [n, 10]: mask, then three votes; a point inside fewer than three boxes repeats its first
+    vote, as the original's `sunrgbd_data.py` export does), compressed like the original's."""
+    rng = np.random.default_rng(seed)
+    pc = np.concatenate([rng.uniform((-3, 0.5, -1.2), (3, 6, 1.5), (n, 3)), rng.random((n, 3))], 1)
+    bbox = np.zeros((n_boxes, 8))
+    bbox[:, 0:3] = rng.uniform((-2.5, 1, -1), (2.5, 5.5, 1), (n_boxes, 3))
+    bbox[:, 3:6] = rng.uniform(0.1, 1.2, (n_boxes, 3))
+    bbox[:, 6] = rng.uniform(-np.pi, np.pi, n_boxes)
+    bbox[:, 7] = rng.integers(0, n_class, n_boxes)
+    votes = np.zeros((n, 10))
+    nv = rng.integers(0, 4, n) * (rng.random(n) < 0.6)
+    for j in range(3):
+        v = rng.uniform(-1, 1, (n, 3))
+        votes[:, 1 + 3 * j:4 + 3 * j] = np.where((nv > j)[:, None], v, votes[:, 1:4])
+    votes[:, 0] = nv > 0
+    np.savez_compressed(f"{path}/{name}_pc.npz", pc=pc)
+    np.savez_compressed(f"{path}/{name}_votes.npz", point_votes=votes)
+    np.save(f"{path}/{name}_bbox.npy", bbox)
