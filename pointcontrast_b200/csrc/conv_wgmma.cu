@@ -23,7 +23,8 @@ constexpr int BM = 128, BK = 32, NPROD = 128, NCONS_WARPS = 8, NTHR = NPROD + 32
 constexpr int SMEM_OPTIN = 227 * 1024, SMEM_PER_SM = 228 * 1024;      // sm_90: largest dynamic shared memory of one CTA, of one SM
 // A tile plane: the 64-byte swizzled K-major layout of wgmma (SWIZZLE_64B): tile row r's 32 channels are the 64 bytes at 64 r, its
 // 16-byte chunk c stored at chunk c ^ ((r >> 1) & 3).  The 8-row atoms (512 bytes) follow each other, and a k16 step starts 32 bytes
-// into the row.  A quarter-warp's copy (two rows x four chunks) covers one 128-byte bank line.
+// into the row.  A quarter-warp's copy (two rows x four chunks) covers one 128-byte bank line.  The weight-gradient kernel (wg::)
+// stores its MN-major atoms with the same byte pattern.
 constexpr int A_ROW = BK * 2, A_ATOM = 8 * A_ROW;
 constexpr int A_PLANE = BM * A_ROW;
 __device__ __forceinline__ uint32_t a_chunk(int r, int c) { return r * A_ROW + ((c ^ ((r >> 1) & 3)) << 4); }
@@ -285,8 +286,10 @@ int launch_conv_wgmma(const uint16_t* Xhi, const uint16_t* Xlo, int lds, const v
 // A CTA owns a group of GK kernel offsets, a CB-channel block of A (CB = pick_tile(Ca)), a TN-channel block of B and one row split.
 // The offsets are stacked along M: D[M = GK offsets x CB channels][N = TN] += A[M x 16 rows] . B[16 rows x N], so the row-aligned
 // operand B is staged once per row step and shared by every offset of the group, and GK * CB fills whole M64 slices without padding.
-// Both operands are MN-major (a matrix row is contiguous along channels): core matrix = 8 rows (K) x 16 B (8 channels), chunk stride
-// 128 B, 8-row-group stride LBO; the stacked A tile's chunks run (offset, channel).
+// Both operands are MN-major (a matrix row is contiguous along channels) in wgmma's 64-byte swizzled layout: an atom is 8 rows (K) x
+// 32 channels, row r's 64 bytes at 64 (r % 8) with its 16-byte chunk c at chunk c ^ ((r >> 1) & 3) (hw::a_chunk, the forward kernel's
+// A-tile pattern); atoms follow each other along the channels (LBO = hw::A_ATOM), then along the rows (SBO = one 8-row group of atoms).
+// The stacked A tile's atoms run (offset, channel).
 // Warpgroup 0 produces: per 32-row stage, the zero-filling cp.async copies of B's rows (not read where no offset of the group has a
 // neighbour) and of every offset's gathered A rows, completing on the slot's "full" mbarrier; the table entries they depend on are
 // loaded TF stages earlier into registers.  Warpgroups 1 and 2 consume, each SL of the tile's M64 slices, and release a slot on its
@@ -307,7 +310,12 @@ struct Args {
   float* partial; int transpose_out;
 };
 
-// Stage = B hi, B lo, A hi, A lo planes of RS rows; the ring takes every slot that fits.
+// MN-major 64-byte swizzled operand: LBO = the stride between atoms along M / N, SBO = the stride between 8-row groups along K;
+// layout type 2: 64B swizzle
+__device__ __forceinline__ uint64_t mn_desc(uint32_t saddr, uint32_t sbo) { return hw::make_desc(saddr, hw::A_ATOM, sbo) | (2ull << 62); }
+
+// Stage = B hi, B lo, A hi, A lo planes of RS rows, each a multiple of 2 KB, so every atom stays 512-byte aligned; the ring takes
+// every slot that fits.
 template <int CB, int TN>
 struct Smem {
   static constexpr int GK = CB % 64 == 0 ? 2 : 4;        // offsets per CTA: GK * CB is a multiple of 128 (two consumers x M64)
@@ -315,8 +323,8 @@ struct Smem {
   static constexpr int SL = MT / 128;                     // M64 slices per consumer warpgroup
   static constexpr int RS = 32;                           // rows per stage
   static constexpr int NQ = RS / 32;                      // rows per producer thread
-  static constexpr int A_LBO = MT / 8 * 128, B_LBO = TN / 8 * 128;
-  static constexpr int A_PLANE = RS / 8 * A_LBO, B_PLANE = RS / 8 * B_LBO;
+  static constexpr int A_SBO = MT / 32 * hw::A_ATOM, B_SBO = TN / 32 * hw::A_ATOM;   // one 8-row group of atoms
+  static constexpr int A_PLANE = RS / 8 * A_SBO, B_PLANE = RS / 8 * B_SBO;
   static constexpr int A_OFF = 2 * B_PLANE;
   static constexpr int STAGE = 2 * B_PLANE + 2 * A_PLANE;
   static constexpr int NS = (hw::SMEM_OPTIN - 16) / (STAGE + 16);    // + full and empty barrier per slot
@@ -330,7 +338,7 @@ __global__ void __launch_bounds__(NTHR, 1) wgrad_wgmma_kernel(const Args p) {
   using namespace hw;
   using S = Smem<CB, TN>;
   constexpr int GK = S::GK, NS = S::NS, RS = S::RS, NQ = S::NQ, ACH = CB / 8, BCH = TN / 8;
-  extern __shared__ __align__(128) unsigned char smem[];
+  extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = warp >> 2;
   const int mblocks = p.Ca / CB, nblocks = p.Cb / TN;
   int bx = blockIdx.x;
@@ -359,10 +367,11 @@ __global__ void __launch_bounds__(NTHR, 1) wgrad_wgmma_kernel(const Args p) {
   if (wgi == 0) {
     setmaxnreg_dec<PROD_REGS>();
     // thread: rows r + 32 q of every stage, 16-byte channel chunks c4 + 4 j of B and of each offset's A block.  A warp's copy covers
-    // 8 rows x 64 contiguous bytes in global memory and four whole 128-byte chunk columns in shared memory.
+    // 8 rows x 64 contiguous bytes in global memory and one 8-row group of atoms in shared memory; a quarter-warp's (two rows x four
+    // chunks) fills one 128-byte bank line.
     const int r = 8 * warp + (lane >> 2), c4 = lane & 3;
-    const uint32_t dst = (r & 7) * 16 + c4 * 128;
-    const uint32_t dst_b = dst + (r >> 3) * S::B_LBO, dst_a = S::A_OFF + dst + (r >> 3) * S::A_LBO;
+    const uint32_t dst = a_chunk(r & 7, c4);
+    const uint32_t dst_b = dst + (r >> 3) * S::B_SBO, dst_a = S::A_OFF + dst + (r >> 3) * S::A_SBO;
     int tq[TF + 1][NQ][GK];                              // table entries of stages i .. i + TF
     auto fetch = [&](int (&d)[NQ][GK], int st) {
 #pragma unroll
@@ -383,15 +392,15 @@ __global__ void __launch_bounds__(NTHR, 1) wgrad_wgmma_kernel(const Args p) {
 #pragma unroll
       for (int q = 0; q < NQ; ++q) {
         const int64_t row = r_begin + (int64_t)i * RS + r + 32 * q;
-        const uint32_t sb = smem_base + s * S::STAGE + q * 4 * S::B_LBO, sa = smem_base + s * S::STAGE + q * 4 * S::A_LBO;
+        const uint32_t sb = smem_base + s * S::STAGE + q * 4 * S::B_SBO, sa = smem_base + s * S::STAGE + q * 4 * S::A_SBO;
         bool any = false;
 #pragma unroll
         for (int g = 0; g < GK; ++g) any |= tq[0][q][g] >= 0;
         const int64_t boff = (any ? row : 0) * p.ldb + n0 + c4 * 8;
 #pragma unroll
         for (int j = 0; j < BCH / 4; ++j) {
-          cp_async16_zfill(sb + dst_b + j * 512, p.Bhi + boff + j * 32, any ? 16u : 0u);
-          cp_async16_zfill(sb + S::B_PLANE + dst_b + j * 512, p.Blo + boff + j * 32, any ? 16u : 0u);
+          cp_async16_zfill(sb + dst_b + j * A_ATOM, p.Bhi + boff + j * 32, any ? 16u : 0u);
+          cp_async16_zfill(sb + S::B_PLANE + dst_b + j * A_ATOM, p.Blo + boff + j * 32, any ? 16u : 0u);
         }
 #pragma unroll
         for (int g = 0; g < GK; ++g) {
@@ -399,7 +408,7 @@ __global__ void __launch_bounds__(NTHR, 1) wgrad_wgmma_kernel(const Args p) {
           const int64_t aoff = (int64_t)(c >= 0 ? c : 0) * p.lda + m0 + c4 * 8;
 #pragma unroll
           for (int j = 0; j < ACH / 4; ++j) {
-            const uint32_t d = sa + dst_a + (g * ACH + 4 * j) * 128;
+            const uint32_t d = sa + dst_a + (g * ACH / 4 + j) * A_ATOM;
             cp_async16_zfill(d, p.Ahi + aoff + j * 32, c >= 0 ? 16u : 0u);
             cp_async16_zfill(d + S::A_PLANE, p.Alo + aoff + j * 32, c >= 0 ? 16u : 0u);
           }
@@ -443,12 +452,13 @@ __global__ void __launch_bounds__(NTHR, 1) wgrad_wgmma_kernel(const Args p) {
       // fragment rows of offsets past K are never read back
 #pragma unroll
       for (int kk = 0; kk < RS / WK; ++kk) {
-        const uint32_t b_hi = sb + kk * 2 * S::B_LBO;
-        const uint64_t dbh = make_desc(b_hi, S::B_LBO, 128), dbl = make_desc(b_hi + S::B_PLANE, S::B_LBO, 128);
+        // a k16 step is two 8-row groups; an M64 slice of A is two atoms
+        const uint32_t b_hi = sb + kk * 2 * S::B_SBO;
+        const uint64_t dbh = mn_desc(b_hi, S::B_SBO), dbl = mn_desc(b_hi + S::B_PLANE, S::B_SBO);
 #pragma unroll
         for (int sl = 0; sl < S::SL; ++sl) {
-          const uint32_t a_hi = sb + S::A_OFF + kk * 2 * S::A_LBO + (h * S::SL + sl) * 8 * 128;
-          const uint64_t dah = make_desc(a_hi, S::A_LBO, 128), dal = make_desc(a_hi + S::A_PLANE, S::A_LBO, 128);
+          const uint32_t a_hi = sb + S::A_OFF + kk * 2 * S::A_SBO + (h * S::SL + sl) * 2 * A_ATOM;
+          const uint64_t dah = mn_desc(a_hi, S::A_SBO), dal = mn_desc(a_hi + S::A_PLANE, S::A_SBO);
           wgmma<TN, false, 1, 1>(acc[sl], dal, dbh, 1u);
           wgmma<TN, false, 1, 1>(acc[sl], dah, dbl, 1u);
           wgmma<TN, false, 1, 1>(acc[sl], dah, dbh, 1u);

@@ -6,15 +6,19 @@ neighbour pair; `per_step_ms` weights each shape by how many units of the step i
 in the identity order and are left out.  Per shape `pool` describes how often the identity order's tiles read the same input row:
 distinct input rows per tile, gathers (entries with a neighbour) per distinct row, the largest row span of a tile, and the share of
 tiles that a shared-memory pool of POOL_ROWS distinct rows within POOL_SPAN rows could not hold (the pool measured in DESIGN.md
-section 7).  Prints one JSON line.
+section 7).  The `wgrad` block times every `pcb_conv_wgrad_split` shape of the same step (weight-gradient kernel plus its reduce, in the
+executor's orientation and accumulating into dW, as the step issues it) the same way, with a CRC of the dW one non-accumulating call
+returns, so two builds can be compared for bits; its `per_step_ms` weights each shape by its launches per step.  `--parts` picks the
+blocks to run.  Prints one JSON line, with the card's name, power limit and SM clock.
 
-    python profiles/bench_conv_order.py [--seconds 1.0] [--windows 4096,8192,16384,0]
+    python profiles/bench_conv_order.py [--seconds 1.0] [--windows 4096,8192,16384,0] [--parts conv,wgrad]
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
+import zlib
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
@@ -89,11 +93,50 @@ def time_launch(fn, seconds):
     return e0.elapsed_time(e1) / reps
 
 
+def wgrad_shapes(sched, geom, dev, seconds):
+    """Per-shape time of every tensor-core weight-gradient call of one step (pcb_unit_backward and the final layer's me.wgrad)."""
+    shapes = {}                                  # (plan, K, Cin, Cout) -> launches per step
+    for u in list(sched.units) + [sched.final]:
+        if u.tc:
+            key = (u.plan, u.K, u.Cin, u.Cout)
+            shapes[key] = shapes.get(key, 0) + 1
+    rows, total = [], 0.0
+    for (pi, K, Cin, Cout), count in shapes.items():
+        plan = geom.plans[pi]
+        if plan.wg_gather_x:                     # A = the input, gathered; B = the output gradient
+            Ca, Cb, tr, n_a, rows_ = Cin, Cout, 0, plan.n_in, plan.n_out
+        else:                                    # A = the output gradient, gathered; B = the input; dW written transposed
+            Ca, Cb, tr, n_a, rows_ = Cout, Cin, 1, plan.n_out, plan.n_in
+        planes = []
+        for n, C in ((n_a, Ca), (rows_, Cb)):
+            v = torch.randn(n, C, device=dev)
+            hi = v.to(torch.bfloat16)
+            planes += [hi, (v - hi.float()).to(torch.bfloat16)]
+        ah, al, bh, bl = planes
+        tbl = plan.wg_tbl
+        dW = torch.zeros(K, Ca, Cb, device=dev)
+        wsb = lib.pcb_conv_wgrad_split_ws_bytes(K, rows_, Ca, Cb)
+        ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=dev)
+
+        def call(flags=_lib.CONV_ACCUMULATE):
+            check(lib.pcb_conv_wgrad_split(ptr(ah), ptr(al), Ca, ptr(bh), ptr(bl), Cb, ptr(tbl), tbl.shape[1], K, rows_, Ca, Cb, ptr(dW), tr,
+                                           ptr(ws), wsb, flags, stream()))
+        call(0)
+        crc = zlib.crc32(dW.cpu().numpy().tobytes())
+        ms = time_launch(call, seconds)
+        total += count * ms
+        rows.append({"K": K, "Ca": Ca, "Cb": Cb, "rows": rows_, "transposed_out": tr, "launches_per_step": count, "ms": round(ms, 4),
+                     "ms_per_step": round(count * ms, 4), "dW_crc32": crc})
+    return {"per_step_ms": round(total, 3), "launches_per_step": sum(shapes.values()), "shapes": rows}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--seconds", type=float, default=1.0, help="least timed window per (shape, order)")
     ap.add_argument("--windows", default=WINDOWS, help="tile-order windows to time besides the identity order (comma list, may be empty)")
+    ap.add_argument("--parts", default="conv,wgrad", help="blocks to run: conv (forward / data-gradient launches), wgrad")
     args = ap.parse_args()
+    parts = set(args.parts.split(","))
     dev = torch.device("cuda", torch.cuda.current_device())
     torch.manual_seed(0)
     net = load_model("Res16UNet34C")(3, 32, default_config(), D=3).to(dev).train()
@@ -102,8 +145,11 @@ def main():
     sinput, n0 = fused.stack_views(b["sinput0_F"], b["sinput0_C"], b["sinput1_F"], b["sinput1_C"], dev)
     geom = fused.Geometry(net, sinput, n0)
 
+    out = {"rows_per_level": geom.n, "seconds_per_measurement": args.seconds}
+    if "wgrad" in parts:
+        out["wgrad"] = wgrad_shapes(sched, geom, dev, args.seconds)
     shapes = {}                                  # (plan, role, K, contraction, columns) -> units of one step that issue it
-    for u in sched.units:
+    for u in sched.units if "conv" in parts else ():
         if u.tc and u.K > 1:
             for role in ("fwd", "dgrad"):
                 key = (u.plan, role, u.K) + ((u.Cin, u.Cout) if role == "fwd" else (u.Cout, u.Cin))
@@ -152,8 +198,9 @@ def main():
             totals[name] = totals.get(name, 0.0) + count * rec["ms"][name]
         rec.pop("same_bits_as_identity")
         rows.append(rec)
-    print(json.dumps({"gpu": gpu_info(), "rows_per_level": geom.n, "seconds_per_measurement": args.seconds,
-                      "per_step_ms": {k: round(v, 3) for k, v in totals.items()}, "shapes": rows}), flush=True)
+    if "conv" in parts:
+        out.update(per_step_ms={k: round(v, 3) for k, v in totals.items()}, shapes=rows)
+    print(json.dumps({"gpu": gpu_info(), **out}), flush=True)
 
 
 if __name__ == "__main__":
