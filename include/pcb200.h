@@ -182,6 +182,43 @@ int pcb_nearest(const double* ref, int64_t m, const double* query, int64_t n, do
 int pcb_label_transfer(const int32_t* idx, const int32_t* ref_label, int64_t m, const int32_t* query_label, int64_t n, const int32_t* lut,
                        int lut_n, int C, int32_t* point_label, int64_t* hist, int32_t* status, void* stream);
 
+/* ----------------------------------------------------------------------------------------------- S3DIS preprocessing (8f-14) */
+/* One room of `downstream/semseg/lib/datasets/preprocessing/stanford.py` `convert_to_ply`: its annotation files' bytes concatenated in
+ * `text` (device, 16-byte aligned, readable up to nbytes rounded up to 16), file f = bytes [file_off[f], file_off[f+1]) (device int64
+ * [nfiles + 1], non-decreasing from 0 to nbytes; a file may be empty).
+ *
+ * pcb_text_lines: the lines of Python's text-mode iteration of each file (universal newlines: "\n", "\r\n" and a lone "\r" end a line; a
+ * last line without one counts; no line crosses a file; an empty file has none).  chunk_off (device int64 [ceil(nbytes / 16) + 1]) receives
+ * the first line index of every 16-byte chunk, flags (device int32 [nfiles]) PCB_TEXT_NONASCII for every file holding a byte >= 0x80,
+ * *n_lines (host) the number of lines.  SYNCHRONISES.
+ *
+ * pcb_s3dis_parse (after pcb_text_lines, same text / file_off / chunk_off / flags): line_start (int64 [n_lines + 1]) = each line's first
+ * byte, then nbytes; per line j, `[float(t) for t in line.split()]` (`stanford.py:47-64`) decided on the device where it is exact --
+ * status[j] (uint8):
+ *   PCB_LINE_KEPT      6 tokens: xyz = float32(float()) (fp32 [n_lines, 3]), rgb = uint8(float32(float())) (uint8 [n_lines, 3]),
+ *                      cell = floor(float64(xyz) / 0.01) in true fp64 division (int32 [n_lines, 3]; clamped to +-2^30)
+ *   PCB_LINE_SKIPPED   a token float() rejects (the original's except branch)
+ *   PCB_LINE_HOST      not decided here: a token outside [0-9+-.eE] that float() may accept (inf, nan, '_'), more than 19
+ *                      significant digits, a value not exact by Clinger's fast path, an rgb value whose float32 lies outside [0, 256),
+ *                      a line longer than 512 bytes, or any line of a PCB_TEXT_NONASCII file
+ *   PCB_LINE_ERROR     only exact tokens, but not 6 of them (a blank line included): the original raises
+ * label[j] = file_label[file of j] (int32 [n_lines]).  Values of lines not KEPT are unspecified.  Does not synchronise.
+ *
+ * pcb_ply_rows: rows[i] (16 bytes, of a 16-byte aligned buffer [m, 16]) = x, y, z <f4 of xyz[sel[i]], red, green, blue of rgb[sel[i]],
+ * labels[i] & 0xff -- the PLY body `lib/pc_utils.py:41-70` writes for `sel` / `labels` of pcb_voxelize_labels.  Does not synchronise. */
+#define PCB_TEXT_NONASCII 1
+#define PCB_LINE_KEPT 0
+#define PCB_LINE_SKIPPED 1
+#define PCB_LINE_HOST 2
+#define PCB_LINE_ERROR 3
+size_t pcb_text_lines_ws_bytes(int64_t nbytes);
+int pcb_text_lines(const uint8_t* text, int64_t nbytes, const int64_t* file_off, int32_t nfiles, int64_t* chunk_off, int32_t* flags,
+                   int64_t* n_lines, void* ws, size_t ws_bytes, void* stream);
+int pcb_s3dis_parse(const uint8_t* text, int64_t nbytes, const int64_t* file_off, const int32_t* file_label, int32_t nfiles,
+                    const int64_t* chunk_off, int32_t* flags, int64_t n_lines, int64_t* line_start, float* xyz, uint8_t* rgb, int32_t* label,
+                    int32_t* cell, uint8_t* status, void* stream);
+int pcb_ply_rows(const float* xyz, const uint8_t* rgb, const int32_t* sel, const int32_t* labels, int64_t m, uint8_t* rows, void* stream);
+
 /* ----------------------------------------------------------------------------------------------- semseg training data (8f-6) */
 /* Label-aware voxelisation of integer coordinates (int32 [N,3], |c| < 2^20): the M occupied voxels in ascending (x,y,z) order
  * (out_coords int32 [M,3]), sel[M] = the smallest index of a point in the voxel, out_labels[M] = the label all of the voxel's points

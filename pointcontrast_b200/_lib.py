@@ -169,6 +169,10 @@ _SIGS = {
     "pcb_nearest_ws_bytes": (_sz, [_l, _l]),
     "pcb_nearest": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _sz, _p]),
     "pcb_label_transfer": (_i, [_p, _p, _l, _p, _l, _p, _i, _i, _p, _p, _p, _p]),
+    "pcb_text_lines_ws_bytes": (_sz, [_l]),
+    "pcb_text_lines": (_i, [_p, _l, _p, C.c_int32, _p, _p, C.POINTER(C.c_int64), _p, _sz, _p]),
+    "pcb_s3dis_parse": (_i, [_p, _l, _p, _p, C.c_int32, _p, _p, _l, _p, _p, _p, _p, _p, _p, _p]),
+    "pcb_ply_rows": (_i, [_p, _p, _p, _p, _l, _p, _p]),
 }
 
 
@@ -208,6 +212,8 @@ ERR_RANGE, ERR_DUPLICATE = 3, 4                       # return codes, and the st
 MAX_KERNEL_VOLUME = 27
 FRAMES_RANGE, FRAMES_OFFSETS = 1, 2                   # status bits of pcb_frame_overlap
 NEAREST_RANGE, LABEL_RANGE = 1, 2                     # status bits of pcb_nearest / pcb_label_transfer
+TEXT_NONASCII = 1                                     # file flag of pcb_text_lines
+LINE_KEPT, LINE_SKIPPED, LINE_HOST, LINE_ERROR = 0, 1, 2, 3     # line status of pcb_s3dis_parse
 CONV_FORCE_SIMT, CONV_ACCUMULATE = 1, 4               # flags of the convolution and weight-gradient entry points
 PLANES_A_FP16, PLANES_B_FP16 = 8, 16                  # flags: 16-bit plane formats of the split-operand calls
 BN_RELU = 1                                           # flag of pcb_bn_apply_seg

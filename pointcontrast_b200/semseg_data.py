@@ -691,6 +691,28 @@ class StanfordDataset(VoxelizationDataset):
                          draws=draws)
 
 
+
+class StanfordArea5Dataset(StanfordDataset):
+    """`lib/datasets/stanford.py:165-171`: Areas 1-4 and 6 train, Area 5 is validation and test (no TrainVal split), from the split files
+    `semseg_prep.generate_splits` writes."""
+    DATA_PATH_FILE = {"Train": ["area1.txt", "area2.txt", "area3.txt", "area4.txt", "area6.txt"], "Val": "area5.txt", "Test": "area5.txt"}
+
+
+class StanfordArea53cmDataset(StanfordArea5Dataset):
+    """`lib/datasets/stanford.py:174-176`."""
+    CLIP_BOUND = 3.2
+    VOXEL_SIZE = 0.03
+
+
+class StanfordArea57d5cmDataset(StanfordArea5Dataset):
+    """`lib/datasets/stanford.py:179-180`."""
+    VOXEL_SIZE = 0.075
+
+
+class StanfordArea510cmDataset(StanfordArea5Dataset):
+    """`lib/datasets/stanford.py:183-184`."""
+    VOXEL_SIZE = 0.1
+
 # ---------------------------------------------------------------------------------------------------------------- collate / loader
 
 class cfl_collate_fn_factory:

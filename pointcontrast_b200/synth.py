@@ -443,3 +443,79 @@ def write_sunrgbd_detection_scene(path, name, seed, n, n_boxes, n_class=10):
     np.savez_compressed(f"{path}/{name}_pc.npz", pc=pc)
     np.savez_compressed(f"{path}/{name}_votes.npz", point_votes=votes)
     np.save(f"{path}/{name}_bbox.npy", bbox)
+
+
+S3DIS_CLASSES = ('clutter', 'beam', 'board', 'bookcase', 'ceiling', 'chair', 'column', 'door', 'floor', 'sofa', 'stairs', 'table', 'wall',
+                 'window')
+
+
+def write_s3dis_tree(root, seed, areas=(1, 5), rooms_per_area=2, points_per_room=20_000, files_per_room=6, empty_room=True):
+    """A `Stanford3dDataset_v1.2_Aligned_Version`-shaped tree: `<root>/Area_i/<room>/<room>.txt` and `Annotations/<class>_<k>.txt`, lines
+    `%.3f %.3f %.3f %d %d %d`.  The annotation files cycle through the 14 classes; coordinates are millimetres in a room-sized box, many
+    on 1 cm boundaries, and every file repeats some of the previous file's points (duplicates across files, mixed-label voxels).  With
+    `empty_room`, Area 1 gets a room without annotation files.  Returns the room directories."""
+    import os
+    rng = np.random.default_rng(seed)
+    rooms, cls = [], 0
+    for a in areas:
+        for r in range(rooms_per_area):
+            room = os.path.join(root, f"Area_{a}", f"office_{r + 1}")
+            ann = os.path.join(room, "Annotations")
+            os.makedirs(ann, exist_ok=True)
+            pts = []
+            n = points_per_room // files_per_room
+            prev = None
+            for k in range(files_per_room):
+                mm = rng.integers(-4000, 6000, size=(n, 3))
+                mm[: n // 4] = mm[: n // 4] // 10 * 10                       # on 1 cm boundaries
+                rgb = rng.integers(0, 256, size=(n, 3))
+                if prev is not None:                                          # points of the previous file again
+                    m = n // 10
+                    mm[-m:], rgb[-m:] = prev[0][:m], prev[1][:m]
+                prev = (mm, rgb)
+                name = f"{S3DIS_CLASSES[cls % len(S3DIS_CLASSES)]}_{k + 1}.txt"
+                cls += 1
+                lines = ["%.3f %.3f %.3f %d %d %d" % (x / 1000, y / 1000, z / 1000, cr, cg, cb)
+                         for (x, y, z), (cr, cg, cb) in zip(mm.tolist(), rgb.tolist())]
+                with open(os.path.join(ann, name), "w") as f:
+                    f.write("\n".join(lines) + "\n")
+                pts += lines
+            with open(os.path.join(room, f"office_{r + 1}.txt"), "w") as f:
+                f.write("\n".join(pts) + "\n")
+            rooms.append(room)
+    if empty_room:
+        room = os.path.join(root, f"Area_{areas[0]}", "storage_1")
+        os.makedirs(os.path.join(room, "Annotations"), exist_ok=True)
+        with open(os.path.join(room, "storage_1.txt"), "w") as f:
+            f.write("0.000 0.000 0.000 0 0 0\n")
+        rooms.append(room)
+    return rooms
+
+
+def write_scannet_raw_scene(root, subset, name, seed, n=2000, labels=True, alpha=255):
+    """`<root>/<subset>/<name>/<name>_vh_clean_2.ply` (x, y, z float, red, green, blue, alpha uchar, as ScanNet releases it) and, with
+    `labels`, `<name>_vh_clean_2.labels.ply` (the same vertices, a ushort `label` column of NYU40 ids).  `alpha` may be an array."""
+    import os
+    rng = np.random.default_rng(seed)
+    d = os.path.join(root, subset, name)
+    os.makedirs(d, exist_ok=True)
+    xyz = rng.uniform(0, 5, size=(n, 3)).astype(np.float32)
+    rgb = rng.integers(0, 256, size=(n, 3)).astype(np.uint8)
+
+    def write(path, extra):
+        fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"), ("blue", "u1"), extra[0]]
+        v = np.empty(n, dtype=fields)
+        v["x"], v["y"], v["z"] = xyz.T
+        v["red"], v["green"], v["blue"] = rgb.T
+        v[extra[0][0]] = extra[1]
+        types = {"<f4": "float", "u1": "uchar", "<u2": "ushort"}
+        head = ["ply", "format binary_little_endian 1.0", f"element vertex {n}"] + [f"property {types[t]} {k}" for k, t in fields]
+        with open(path, "wb") as f:
+            f.write(("\n".join(head + ["end_header"]) + "\n").encode("ascii"))
+            f.write(v.tobytes())
+
+    write(os.path.join(d, f"{name}_vh_clean_2.ply"), (("alpha", "u1"), alpha))
+    if labels:
+        lab = rng.choice(np.array([0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 14, 16, 24, 28, 33, 34, 36, 39, 40, 50, 149]), n)
+        write(os.path.join(d, f"{name}_vh_clean_2.labels.ply"), (("label", "<u2"), lab))
+    return d
