@@ -219,6 +219,33 @@ int pcb_s3dis_parse(const uint8_t* text, int64_t nbytes, const int64_t* file_off
                     int32_t* cell, uint8_t* status, void* stream);
 int pcb_ply_rows(const float* xyz, const uint8_t* rgb, const int32_t* sel, const int32_t* labels, int64_t m, uint8_t* rows, void* stream);
 
+/* ----------------------------------------------------------------------------------------------- VoteNet detection preprocessing (8f-15) */
+/* pcb_scannet_annotate: the per-vertex work of one scene of `lib/datasets/scannet/load_scannet_data.py` `export`.  vin (device fp32 [V, 6]:
+ * x y z r g b), align (device fp64 [16], the row-major `axisAlignment` matrix M), seg (device int64 [V], `segIndices`, each < INT64_MAX).
+ * The host restates `read_aggregation` as two write lists in the original's loop order: label writes (lab_seg int64, lab_val uint32)
+ * [n_lab] and instance writes (ins_seg int64, ins_obj int32 = the object's dict index) [n_ins]; per object d < n_obj (dict order):
+ * obj_id[d] (uint32, the instance id), first_seg[d] (its first segment) and obj_row[d] (its box row, `obj_id - 1` wrapped as numpy
+ * indexes, or -1 outside [0, n_rows)).  Outputs (device): vout fp32 [V, 6] (xyz = fp32 of fp64 [x y z 1] . M^T, one rounding per
+ * operation in k order; rgb copied), sem / ins uint32 [V] (the last write to the vertex's segment wins, 0 where none), bbox fp64
+ * [n_rows, 7] (per object with vertices: fp32 (min + max) / 2, max - min of its aligned xyz, then the label at the lowest vertex of its
+ * first segment; a row no such object owns is zero; -0.0 is the minimum and +0.0 the maximum when both occur; a NaN coordinate makes
+ * both bounds of its axis NaN), status int32 [2]: [0] the lowest write ordinal (label writes first, then instance writes) whose
+ * segment no vertex has, [1] the lowest object with vertices and obj_row -1; 0x7f7f7f7f where none.  Does not synchronise. */
+size_t pcb_scannet_annotate_ws_bytes(int64_t V, int64_t n_obj, int64_t n_rows);
+int pcb_scannet_annotate(const float* vin, const double* align, int64_t V, const int64_t* seg, const int64_t* lab_seg,
+                         const uint32_t* lab_val, int64_t n_lab, const int64_t* ins_seg, const int32_t* ins_obj, int64_t n_ins,
+                         const uint32_t* obj_id, const int64_t* first_seg, const int32_t* obj_row, int64_t n_obj, int64_t n_rows,
+                         float* vout, uint32_t* sem, uint32_t* ins, double* bbox, int32_t* status, void* ws, size_t ws_bytes,
+                         void* stream);
+/* pcb_sunrgbd_votes: the ground-truth votes of `lib/datasets/sunrgbd/sunrgbd_data.py` `extract_sunrgbd_data` for B scenes in one launch.
+ * pts (device fp64 [N, ld], ld >= 3, xyz first), scene b = rows [pt_off[b], pt_off[b+1]); boxes (device fp64 [K, 8]: cx, cy, cz, l, w, h,
+ * cos(-heading), sin(-heading)), scene b's boxes = rows [box_off[b], box_off[b+1]) in file order; offsets as int64 [B + 1] on both the
+ * host and the device.  votes (device fp64 [N, 10]): column 0 = 1 if the point is in a box, then three votes centroid - p; the point's
+ * k-th box writes slot min(k, 2), its first box all three.  Inside: |u| <= (l, w, h) for u = rotz(-heading)^T (p - centroid).  Boxes
+ * with l, w or h not > 0, or a non-finite value, are skipped.  Does not synchronise. */
+int pcb_sunrgbd_votes(const double* pts, int32_t ld, const int64_t* pt_off_host, const int64_t* pt_off, const double* boxes,
+                      const int64_t* box_off_host, const int64_t* box_off, int64_t B, double* votes, void* stream);
+
 /* ----------------------------------------------------------------------------------------------- semseg training data (8f-6) */
 /* Label-aware voxelisation of integer coordinates (int32 [N,3], |c| < 2^20): the M occupied voxels in ascending (x,y,z) order
  * (out_coords int32 [M,3]), sel[M] = the smallest index of a point in the voxel, out_labels[M] = the label all of the voxel's points

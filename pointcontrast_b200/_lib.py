@@ -173,6 +173,9 @@ _SIGS = {
     "pcb_text_lines": (_i, [_p, _l, _p, C.c_int32, _p, _p, C.POINTER(C.c_int64), _p, _sz, _p]),
     "pcb_s3dis_parse": (_i, [_p, _l, _p, _p, C.c_int32, _p, _p, _l, _p, _p, _p, _p, _p, _p, _p]),
     "pcb_ply_rows": (_i, [_p, _p, _p, _p, _l, _p, _p]),
+    "pcb_scannet_annotate_ws_bytes": (_sz, [_l, _l, _l]),
+    "pcb_scannet_annotate": (_i, [_p, _p, _l, _p, _p, _p, _l, _p, _p, _l, _p, _p, _p, _l, _l, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "pcb_sunrgbd_votes": (_i, [_p, C.c_int32, _p, _p, _p, _p, _p, _l, _p, _p]),
 }
 
 

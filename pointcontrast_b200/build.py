@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["coords.cu", "voxel.cu", "conv.cu", "conv_wgmma.cu", "bn.cu", "loss.cu", "nce_wgmma.cu", "unit.cu", "pointnet2.cu", "augment.cu",
            "metrics.cu", "det_eval.cu", "det_loss.cu", "pair_list.cu", "fulleval.cu", "det_data.cu",
-           "semseg_prep.cu"]
+           "semseg_prep.cu", "det_prep.cu"]
 OUT = os.path.join(HERE, "libpcb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--threads", "4",

@@ -132,6 +132,32 @@ __device__ __forceinline__ void warp_row_max_sumexp(const float* __restrict__ x,
   for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
 }
 
+// Order-preserving integer keys of floating-point values: key(a) < key(b) when a < b, -0.0 below +0.0, a NaN below -inf or above
+// +inf by its sign bit.  Radix selection (det_data.cu) and atomic min / max of bounds (det_data.cu, det_prep.cu) work on these keys;
+// add / sub / mul are the explicitly rounded operations of the type.
+template <class T> struct Ord;
+template <> struct Ord<float> {
+  using K = uint32_t;
+  static constexpr int BITS = 32;
+  __device__ static K key(float v) { const uint32_t u = __float_as_uint(v); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
+  __device__ static float val(K k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+  __device__ static float add(float a, float b) { return __fadd_rn(a, b); }
+  __device__ static float sub(float a, float b) { return __fsub_rn(a, b); }
+  __device__ static float mul(float a, float b) { return __fmul_rn(a, b); }
+};
+template <> struct Ord<double> {
+  using K = unsigned long long;
+  static constexpr int BITS = 64;
+  __device__ static K key(double v) {
+    const K u = (K)__double_as_longlong(v);
+    return (u >> 63) ? ~u : (u | (1ull << 63));
+  }
+  __device__ static double val(K k) { return __longlong_as_double((long long)((k >> 63) ? (k & ~(1ull << 63)) : ~k)); }
+  __device__ static double add(double a, double b) { return __dadd_rn(a, b); }
+  __device__ static double sub(double a, double b) { return __dsub_rn(a, b); }
+  __device__ static double mul(double a, double b) { return __dmul_rn(a, b); }
+};
+
 inline int current_device() { int dev = 0; cudaGetDevice(&dev); return (dev >= 0 && dev < 64) ? dev : 0; }
 
 inline int num_sms() {

@@ -15,29 +15,6 @@ constexpr double PI = 3.141592653589793;      // np.pi
 
 // ---------------------------------------------------------------------------------------------------------------- floor height
 
-template <class T> struct Ord;
-template <> struct Ord<float> {
-  using K = uint32_t;
-  static constexpr int BITS = 32;
-  __device__ static K key(float v) { const uint32_t u = __float_as_uint(v); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
-  __device__ static float val(K k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
-  __device__ static float add(float a, float b) { return __fadd_rn(a, b); }
-  __device__ static float sub(float a, float b) { return __fsub_rn(a, b); }
-  __device__ static float mul(float a, float b) { return __fmul_rn(a, b); }
-};
-template <> struct Ord<double> {
-  using K = unsigned long long;
-  static constexpr int BITS = 64;
-  __device__ static K key(double v) {
-    const K u = (K)__double_as_longlong(v);
-    return (u >> 63) ? ~u : (u | (1ull << 63));
-  }
-  __device__ static double val(K k) { return __longlong_as_double((long long)((k >> 63) ? (k & ~(1ull << 63)) : ~k)); }
-  __device__ static double add(double a, double b) { return __dadd_rn(a, b); }
-  __device__ static double sub(double a, double b) { return __dsub_rn(a, b); }
-  __device__ static double mul(double a, double b) { return __dmul_rn(a, b); }
-};
-
 // the key of rank r (0-based, ascending) among the n keys of z[lo .. lo + n) by 8-bit radix selection; every thread gets it
 template <class T>
 __device__ typename Ord<T>::K radix_select(const T* __restrict__ z, int64_t stride, int64_t lo, int64_t n, int64_t r, int* hist) {

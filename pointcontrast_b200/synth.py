@@ -519,3 +519,133 @@ def write_scannet_raw_scene(root, subset, name, seed, n=2000, labels=True, alpha
         lab = rng.choice(np.array([0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 14, 16, 24, 28, 33, 34, 36, 39, 40, 50, 149]), n)
         write(os.path.join(d, f"{name}_vh_clean_2.labels.ply"), (("label", "<u2"), lab))
     return d
+
+
+# `scannetv2-labels.combined.tsv`'s columns; the rows are synthetic (raw_category -> nyu40id), with two raw names per id for some ids
+SCANNET_TSV_COLUMNS = ("id", "raw_category", "category", "count", "nyu40id", "eigen13id", "nyuClass", "nyu40class", "eigen13class",
+                       "ModelNet40", "ModelNet10", "ShapeNetCore55", "synsetoffset", "wnsynsetid", "wnsynsetkey", "mpcat40", "mpcat40index")
+SCANNET_DET_LABELS = (("wall", 1), ("floor", 2), ("kitchen cabinet", 3), ("cabinet", 3), ("bed", 4), ("chair", 5), ("office chair", 5),
+                      ("sofa", 6), ("table", 7), ("door", 8), ("window", 9), ("bookshelf", 10), ("picture", 11), ("counter", 12),
+                      ("desk", 14), ("curtain", 16), ("refrigerator", 24), ("shower curtain", 28), ("toilet", 33), ("sink", 34),
+                      ("bathtub", 36), ("trash can", 39), ("lamp", 35), ("pillow", 18))
+
+
+def write_scannet_label_map(path):
+    """A small label map in the released TSV layout (`raw_category` -> `nyu40id`)."""
+    with open(path, "w") as f:
+        f.write("\t".join(SCANNET_TSV_COLUMNS) + "\n")
+        for k, (name, nyu) in enumerate(SCANNET_DET_LABELS):
+            f.write("\t".join([str(k + 1), name, name, str(100 - k), str(nyu)] + [""] * (len(SCANNET_TSV_COLUMNS) - 5)) + "\n")
+    return path
+
+
+def write_scannet_det_raw_scene(scans_root, name, seed, n=3000, n_seg=80, n_obj=10, fault=None):
+    """`<scans_root>/<name>/` as ScanNet releases a scene: `<name>_vh_clean_2.ply` (x, y, z float, red, green, blue, alpha uchar),
+    `<name>.aggregation.json`, `<name>_vh_clean_2.0.010000.segs.json` and `<name>.txt` with an axisAlignment line.  Every scene has
+    overlapping objects, repeated labels (the original's list aliasing), a repeated objectId and an object left without vertices.  `fault`
+    makes the original raise: 'no_align', 'unknown_seg', 'unknown_label', 'no_segments', 'id_range' or 'vertex_count'."""
+    import json
+    import os
+    rng = np.random.default_rng(seed)
+    d = os.path.join(scans_root, name)
+    os.makedirs(d, exist_ok=True)
+    xyz = rng.uniform((-1, -2, 0), (6, 5, 3), (n, 3)).astype(np.float32)
+    rgb = rng.integers(0, 256, (n, 3)).astype(np.uint8)
+    v = np.empty(n, [("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"), ("blue", "u1"), ("alpha", "u1")])
+    v["x"], v["y"], v["z"] = xyz.T
+    v["red"], v["green"], v["blue"] = rgb.T
+    v["alpha"] = 255
+    head = ["ply", "format binary_little_endian 1.0", "comment VCGLIB generated", f"element vertex {n}"]
+    head += [f"property {'float' if k in 'xyz' else 'uchar'} {k}" for k in v.dtype.names] + ["element face 0",
+                                                                                             "property list uchar int vertex_indices", "end_header"]
+    with open(os.path.join(d, f"{name}_vh_clean_2.ply"), "wb") as f:
+        f.write(("\n".join(head) + "\n").encode("ascii"))
+        f.write(v.tobytes())
+    seg_ids = np.sort(rng.choice(20 * n, n_seg, replace=False))
+    seg = seg_ids[rng.integers(0, n_seg, n)]
+    seg[:n_seg] = seg_ids                               # every segment has a vertex
+    segs_out = seg.tolist()[: n - 1] if fault == "vertex_count" else seg.tolist()
+    with open(os.path.join(d, f"{name}_vh_clean_2.0.010000.segs.json"), "w") as f:
+        json.dump({"params": {"kThresh": "0.0001", "segMinVerts": "20"}, "sceneId": name, "segIndices": segs_out}, f)
+    labels = [lab for lab, _ in SCANNET_DET_LABELS]
+    groups = []
+    for k in range(n_obj):
+        take = rng.choice(n_seg, int(rng.integers(1, max(2, n_seg // n_obj))), replace=False)
+        groups.append({"id": k, "objectId": k, "segments": seg_ids[take].tolist(), "label": labels[int(rng.integers(0, len(labels)))]})
+    groups[3]["label"] = groups[1]["label"]             # aliasing: object 1's list grows by object 3's segments
+    groups[5]["segments"] = groups[6]["segments"][:1]   # object 5's only segment goes to object 6: an instance without vertices
+    groups.append({"id": n_obj, "objectId": 2, "segments": seg_ids[rng.choice(n_seg, 3, replace=False)].tolist(), "label": "sofa"})
+    if fault == "unknown_seg":
+        groups[4]["segments"].append(int(20 * n + 7))
+    elif fault == "unknown_label":
+        groups[4]["label"] = "spaceship"
+    elif fault == "no_segments":
+        groups.append({"id": n_obj + 1, "objectId": n_obj + 1, "segments": [], "label": "pillow"})
+    elif fault == "id_range":
+        groups[7]["objectId"] = n_obj + 5
+    with open(os.path.join(d, f"{name}.aggregation.json"), "w") as f:
+        json.dump({"sceneId": f"scannet.{name}", "appId": "Aggregator.v2", "segGroups": groups, "segmentsFile": f"scannet.{name}"}, f)
+    a = rng.uniform(-np.pi, np.pi)
+    m = np.array([[np.cos(a), -np.sin(a), 0, rng.uniform(-3, 3)], [np.sin(a), np.cos(a), 0, rng.uniform(-3, 3)], [0, 0, 1, -0.05],
+                  [0, 0, 0, 1]])
+    with open(os.path.join(d, f"{name}.txt"), "w") as f:
+        f.write("colorHeight = 968\ncolorWidth = 1296\n")
+        if fault != "no_align":
+            f.write("axisAlignment = " + " ".join("%.6f" % x if x not in (0, 1) else "%d" % x for x in m.ravel()) + " \n")
+        f.write("numColorFrames = 1000\nsceneType = Bedroom / Hotel\n")
+    return d
+
+
+def _sunrgbd_line(cls, c, l, w, h, heading_dir):
+    """A `label*/%06d.txt` line: classname, 2D box, centroid, w, l, h, orientation (as `SUNObject3d` reads them)."""
+    vals = [12, 34, 56, 78, c[0], c[1], c[2], w, l, h, heading_dir[0], heading_dir[1]]
+    return cls + " " + " ".join(repr(float(x)) for x in vals)
+
+
+def write_sunrgbd_export(root, seed, n_scenes=6, n_points=3000, big_points=60000, n_boxes=4):
+    """`<root>/` as the MATLAB export leaves `sunrgbd_trainval`: `depth/%06d.mat` ('instance', fp64 [N, 6]), `label/` and `label_v1/`
+    (`SUNObject3d` lines), `calib/` and `train_data_idx.txt` / `val_data_idx.txt`.  Scene 1 has boxes nested around one centre (points in
+    up to five boxes), an axis-aligned box with points exactly on its faces, a zero-size box, a 1e-9-thin box and classes outside the
+    whitelist; scene 2 has no box; scene 0 has `big_points` points (more than the 50000 drawn), the others `n_points`."""
+    import os
+    from scipy.io import savemat
+    rng = np.random.default_rng(seed)
+    for sub in ("depth", "label", "label_v1", "calib"):
+        os.makedirs(os.path.join(root, sub), exist_ok=True)
+    idxs = list(range(1, n_scenes + 1))
+    for k, idx in enumerate(idxs):
+        n = big_points if k == 0 else n_points
+        pc = np.concatenate([rng.uniform((-2, 0.5, -1), (2, 5, 1.5), (n, 3)), rng.random((n, 3))], 1)
+        lines = []
+        for j in range(n_boxes if k != 2 else 0):
+            cls = ("chair", "bed", "table", "lamp", "desk", "sofa")[(j + k) % 6]
+            t = rng.uniform(-np.pi, np.pi)
+            lines.append(_sunrgbd_line(cls, rng.uniform((-1.5, 1, -0.5), (1.5, 4.5, 1)), *rng.uniform(0.2, 1.0, 3), (np.cos(t), np.sin(t))))
+        if k == 1:
+            c = np.array([0.25, 2.5, 0.125])
+            for j in range(5):                          # nested: the centre lies in all five
+                t = rng.uniform(-np.pi, np.pi)
+                lines.append(_sunrgbd_line(("bed", "table", "sofa", "chair", "toilet")[j], c + 0.01 * j, 0.4 + 0.1 * j, 0.5, 0.3 + 0.05 * j,
+                                           (np.cos(t), np.sin(t))))
+            face = np.array([1.0, 3.0, 0.5])           # axis-aligned, dyadic: points exactly on faces, edges and corners
+            lines.append(_sunrgbd_line("desk", face, 0.25, 0.5, 0.125, (1.0, 0.0)))
+            on = face + np.array([[0.25, 0, 0], [-0.25, 0, 0], [0, 0.5, 0], [0, -0.5, 0], [0, 0, 0.125], [0, 0, -0.125], [0.25, 0.5, 0.125],
+                                  [0.25 + 2 ** -20, 0, 0]])
+            pc[:len(on), :3] = on
+            pc[len(on):len(on) + 20, :3] = c + rng.uniform(-0.05, 0.05, (20, 3))
+            lines.append(_sunrgbd_line("dresser", (0.0, 2.0, 0.0), 0.0, 0.5, 0.5, (1.0, 0.0)))        # zero size: Qhull raises
+            lines.append(_sunrgbd_line("night_stand", (-0.5, 2.0, 0.0), 0.5, 0.5, 1e-9, (0.6, 0.8)))  # thin
+            lines.append(_sunrgbd_line("lamp", (0.0, 3.0, 0.0), 0.5, 0.5, 0.5, (1.0, 0.0)))           # not whitelisted
+            lines.append(_sunrgbd_line("pillow", (0.3, 2.6, 0.1), 0.5, 0.5, 0.5, (1.0, 0.0)))
+        savemat(os.path.join(root, "depth", "%06d.mat" % idx), {"instance": pc})
+        for sub in ("label", "label_v1"):
+            ls = lines if sub == "label_v1" else lines[::-1]
+            with open(os.path.join(root, sub, "%06d.txt" % idx), "w") as f:
+                f.write("".join(ln + "\n" for ln in ls))
+        with open(os.path.join(root, "calib", "%06d.txt" % idx), "w") as f:
+            f.write("1 0 0 0 1 0 0 0 1\n529.5 0 0 0 529.5 0 365 265 1\n")
+    with open(os.path.join(root, "train_data_idx.txt"), "w") as f:
+        f.write("".join("%d\n" % i for i in idxs[: n_scenes - 2]))
+    with open(os.path.join(root, "val_data_idx.txt"), "w") as f:
+        f.write("".join("%d\n" % i for i in idxs[n_scenes - 2:]))
+    return idxs
