@@ -711,6 +711,36 @@ int pcb_furthest_point_sampling_ragged(const float* xyz, const int64_t* offsets,
 int pcb_gather_rows_grad(const float* grad_out, const int32_t* idx, int64_t L, int64_t C, int64_t M, float* grad_rows, void* ws,
                          size_t ws_bytes, void* stream);
 
+/* ----------------------------------------------------------------------------------------------- PointNet++ shared MLPs (8f-16) */
+/* The two ends of a set-abstraction module's shared MLP (`pointnet2_modules.py` PointnetSAModuleVotes, `pytorch_utils.py` SharedMLP) that
+ * differ from a plain 1x1 convolution; the layers between are pcb_unit_* calls on a K = 1 identity table.  Rows are point-major: row
+ * r = (b npoint + i) S + s is sample s of centre i of scene b (M = B npoint centres, R = M S rows).  All fp32 with one rounding per
+ * operation, no contraction except inside the BatchNorm expression; nothing synchronises.
+ *
+ * pcb_sa_layer0: the first layer without the grouped [R, 3 + C] input.  rel[r] (fp32 [R, 3]) = (xyz[b, j] - new_xyz[b, i]), then / radius
+ *   when radius > 0 (the original's normalize_xyz; 0: no division), j = idx[r] (int32 [B, npoint, S], ball query), and
+ *   z[r, c] = P[b N + j, c] + ((rel_0 Wx[0][c] + rel_1 Wx[1][c]) + rel_2 Wx[2][c]) for c < C0 (row stride ldz), where Wx (fp32 [3][C0])
+ *   holds the layer's three xyz columns and P (fp32 [B N, C0], row stride ldp, or NULL for a module without features) = the feature
+ *   columns applied to every point once.  gidx[r] = b N + j (int32 [R]), -1 where j lies outside [0, N) (that row then reads zeros).
+ * pcb_sa_pool: the last layer's BatchNorm -> ReLU -> max over the S samples of each centre, by selection: sel[i, c] (int32 [M, C]) = the
+ *   slot of the largest z (gamma[c] >= 0) or of the smallest z (gamma[c] < 0), the smallest slot among equals, and
+ *   out[i, c] (row stride ldo) = max(0, (z - mean) invstd gamma + beta) at that slot.  invstd > 0 and every rounding is monotone, so out
+ *   equals the maximum of the same expression over all S slots bit for bit.  mean / invstd: pcb_bn_stats_seg (training) or the running
+ *   statistics.
+ * pcb_sa_pool_grad: dY (fp32 [R, C], written in full) = g[i, c] (row stride ldg) on the selected slot where out[i, c] > 0, else 0: the
+ *   gradient of the pre-pool activation, for pcb_bn_backward_seg on z.
+ * pcb_sa_xyz_rows: rows (fp32 [R + M, 3]) for pcb_gather_rows_grad over the index list [gidx | b N + inds]: rows[r] = grel[r] / radius
+ *   (radius > 0; grel[r] itself otherwise), grel = the gradient of rel, and rows[R + i] = d_new_xyz[i] (fp32 [M, 3] or NULL: 0) minus the
+ *   sum of centre i's S rows in ascending s.
+ * Sizes below 1, R, M C or B N >= 2^31, a NaN radius, strides below the widths and NULL pointers return PCB_ERR_ARG before the launch. */
+int pcb_sa_layer0(const float* xyz, const float* new_xyz, const int32_t* idx, int64_t B, int64_t N, int64_t npoint, int S, float radius,
+                  const float* P, int ldp, const float* Wx, int C0, float* rel, int32_t* gidx, float* z, int ldz, void* stream);
+int pcb_sa_pool(const float* z, int ldz, int64_t M, int S, int C, const float* mean, const float* invstd, const float* gamma,
+                const float* beta, int32_t* sel, float* out, int ldo, void* stream);
+int pcb_sa_pool_grad(const float* g, int ldg, const int32_t* sel, const float* out, int ldo, int64_t M, int S, int C, float* dY,
+                     void* stream);
+int pcb_sa_xyz_rows(const float* grel, const float* d_new_xyz, int64_t M, int S, float radius, float* rows, void* stream);
+
 /* ----------------------------------------------------------------------------------------------- optimiser */
 /* torch.optim.SGD semantics on a flat buffer:  d = g*grad_scale + wd*p;  buf = first ? d : momentum*buf + (1-dampening)*d;  p -= lr*buf
  * (pretraining: dampening 0, `lib/ddp_trainer.py:107-111`; semseg finetuning: 0.1, `downstream/semseg/lib/solvers.py:50-57`) */

@@ -160,6 +160,10 @@ _SIGS = {
     "pcb_furthest_point_sampling_ragged_ws_bytes": (_sz, [_l, _l, _l]),
     "pcb_furthest_point_sampling_ragged": (_i, [_p, _p, _l, _l, _l, _l, _p, _p, _sz, _p]),
     "pcb_gather_rows_grad": (_i, [_p, _p, _l, _l, _l, _p, _p, _sz, _p]),
+    "pcb_sa_layer0": (_i, [_p, _p, _p, _l, _l, _l, _i, _f, _p, _i, _p, _i, _p, _p, _p, _i, _p]),
+    "pcb_sa_pool": (_i, [_p, _i, _l, _i, _i, _p, _p, _p, _p, _p, _p, _i, _p]),
+    "pcb_sa_pool_grad": (_i, [_p, _i, _p, _p, _i, _l, _i, _i, _p, _p]),
+    "pcb_sa_xyz_rows": (_i, [_p, _p, _l, _i, _f, _p, _p]),
     "pcb_voxel_down_sample_ws_bytes": (_sz, [_l, _l]),
     "pcb_voxel_down_sample": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _p, _sz, _p]),
     "pcb_frame_overlap_ws_bytes": (_sz, [_l, _l]),
