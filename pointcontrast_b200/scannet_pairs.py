@@ -147,16 +147,29 @@ def default_collate_pair_fn(list_data):
             "len_batch": lens}
 
 
-class DistributedInfSampler:
-    """`lib/data_sampler.py:13-70`: an endless permutation; rank r of R takes entries it*R + r."""
+def shared_randperm(n, seed, count):
+    """A permutation of range(n): from the global torch RNG when `seed` is None, else the `count`-th one of `seed`'s own sequence
+    (the same on every process)."""
+    if seed is None:
+        return torch.randperm(n)
+    g = torch.Generator()
+    g.manual_seed((int(seed) * 1_000_003 + int(count)) % (1 << 63))
+    return torch.randperm(n, generator=g)
 
-    def __init__(self, n, num_replicas=1, rank=0, shuffle=True):
-        self.n, self.num_replicas, self.rank, self.shuffle = n, num_replicas, rank, shuffle
-        self.it = 0
+
+class DistributedInfSampler:
+    """`lib/data_sampler.py:13-70`: an endless permutation; rank r of R takes entries it*R + r.  The permutations come from the
+    global torch RNG, or with `seed` from a generator of their own seeded by (seed, permutation count): ranks that draw different
+    amounts from the global RNG between two permutations still share them, so their shards stay disjoint."""
+
+    def __init__(self, n, num_replicas=1, rank=0, shuffle=True, seed=None):
+        self.n, self.num_replicas, self.rank, self.shuffle, self.seed = n, num_replicas, rank, shuffle, seed
+        self.it = self.permutations = 0
         self.reset_permutation()
 
     def reset_permutation(self):
-        self._perm = (torch.randperm(self.n) if self.shuffle else torch.arange(self.n)).tolist()
+        self._perm = (shared_randperm(self.n, self.seed, self.permutations) if self.shuffle else torch.arange(self.n)).tolist()
+        self.permutations += 1
 
     def __iter__(self):
         return self

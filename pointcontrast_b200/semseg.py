@@ -10,13 +10,21 @@ dampening, PolyLR) and `lib/utils.py:19-43` (lenient loading of pretraining chec
 Everything numerical runs on libpcb200: the fused executor (the 13 / 20-class head on the exact fp32 kernels), the cross-entropy
 kernels (`pcb_ce_forward_backward`), the flat SGD kernel with dampening.
 
-Evaluation (`lib/test.py:62-196`) and the training loop around the step (`lib/train.py:22-232`, without tensorboard or DDP):
+Evaluation (`lib/test.py:62-196`) and the training loop around the step (`lib/train.py:22-232`, without tensorboard):
 
     metrics = SegmentationMetrics(num_labels, ignore_label, "cuda")
     metrics.update(logits, target)                          # per batch: two kernel calls, nothing read back
     r = metrics.result()                                    # one device -> host read: r.loss, r.score, r.mAP, r.mIoU, r.iou, ...
     loss, score, mAP, mIoU = test(model, val_loader, config)
     trainer.train(train_loader, val_loader)                 # stat / save / val frequencies, best_val checkpoint, resume
+
+Data parallel on several GPUs (`lib/train.py` under DistributedDataParallel, `lib/dataset.py:374-378`): one process per GPU
+(torchrun), `torch.distributed.init_process_group("nccl")` before the trainer is built, and per-rank loaders:
+
+    train_loader = semseg_data.initialize_data_loader(..., repeat=True)           # this rank's shard, batch_size scenes per rank
+    val_loader = semseg_data.initialize_data_loader(..., repeat=False, rank=rank, world=world)
+    trainer = SegmentationTrainer(model, config)            # rank 0's weights everywhere; gradient mean over the ranks
+    trainer.train(train_loader, val_loader)                 # global logged stats and validation; rank 0 writes the checkpoints
 
 On the original point cloud (`lib/utils.py:304-349`, `lib/datasets/scannet.py:131-172`, `stanford.py:41-84`; `pcb_nearest`,
 `pcb_label_transfer`):
@@ -33,10 +41,12 @@ import warnings
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from . import _lib, losses, me as ME
 from ._lib import check, lib, ptr, stream, workspace
 from .optim import FlatSGD, PolyLR
+from .trainer import GradientAllReduce, broadcast_state, get_rank, get_world_size
 
 
 def load_state_with_same_shape(model, weights):
@@ -74,6 +84,11 @@ def initialize_scheduler(optimizer, config, last_step=-1):
 
 
 class SegmentationTrainer:
+    """The finetune loop on this process's rank.  With torch.distributed initialised and more than one rank (the caller's
+    `init_process_group`, e.g. under torchrun) it is data parallel as `lib/train.py` under DistributedDataParallel: rank 0's weights
+    and buffers at construction and after `resume`, the gradient mean over the ranks (the flat gradient's sum all-reduce, launched
+    during the last sub-batch's backward sweep, and 1/world in the SGD kernel), BatchNorm statistics per rank."""
+
     def __init__(self, model, config, device=None):
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.model = model.to(self.device)
@@ -83,16 +98,23 @@ class SegmentationTrainer:
         self.ignore_label = config.data.ignore_label
         self.iter_size = config.optimizer.iter_size
         self.curr_iter = 1
+        self.world, self.rank = get_world_size(), get_rank()
+        if self.world > 1:
+            broadcast_state(self.model, self.optimizer)
+            self.optimizer.grad_scale = 1.0 / self.world
+        # the gradient all-reduce; its `timing` (a dict) collects the CUDA events of each all-reduce
+        self.grads = GradientAllReduce(self.model, self.optimizer, self.world, self.device, every_backward=False)
 
     def train_step(self, sub_batches, shift_coords=True, metrics=None):
         """One optimiser step = `iter_size` sub-batches of (coords int32 [N,4], feats fp32 [N,3], target int [N]), gradients
-        accumulated (`lib/train.py:97-160`).  Returns the summed (already 1/iter_size-scaled) loss as a device scalar.
-        `metrics` (a SegmentationMetrics): each sub-batch's training logits are added to it (loss, precision@1, histogram; no AP)."""
+        accumulated (`lib/train.py:97-160`).  Returns the summed (already 1/iter_size-scaled) loss of this rank as a device scalar.
+        `metrics` (a SegmentationMetrics): each sub-batch's training logits are added to it (loss, precision@1, histogram; no AP).
+        On several ranks the gradient sum over the ranks is reduced during the last sub-batch's backward and before the step."""
         assert len(sub_batches) == self.iter_size
         self.model.train()
         self.optimizer.zero_grad()
         total = None
-        for coords, feats, target in sub_batches:
+        for i, (coords, feats, target) in enumerate(sub_batches):
             if shift_coords:          # `lib/train.py:110`: even/odd-coordinate invariance (shifts the batch column too: SURVEY.md appendix B)
                 coords = coords.clone()
                 coords[:, :3] += (torch.rand(3) * 100).type_as(coords)
@@ -100,10 +122,13 @@ class SegmentationTrainer:
             soutput = self.model(sinput)
             target = target.to(self.device, non_blocking=True)
             loss = losses.cross_entropy(soutput.F, target, self.ignore_label) / self.iter_size
+            if i == len(sub_batches) - 1:
+                self.grads.arm()
             loss.backward()
             total = loss.detach() if total is None else total + loss.detach()
             if metrics is not None:
                 metrics.update(soutput.F.detach(), target, average_precision=False)
+        self.grads.finish()
         self.optimizer.step()
         self.scheduler.step()
         self.curr_iter += 1
@@ -112,7 +137,7 @@ class SegmentationTrainer:
     def resume(self, directory):
         """`lib/train.py:75-92`: restores from `directory/weights.pth` the weights, the iteration (the next one to run is
         `curr_iter`), epoch and best_val, and -- unless `config.train.resume_optimizer` is false -- the optimiser state and the
-        scheduler position."""
+        scheduler position.  Every rank reads the file; then rank 0's weights and buffers are broadcast."""
         fn = os.path.join(directory, "weights.pth")
         if not os.path.isfile(fn):
             raise ValueError(f"=> no checkpoint found at '{fn}'")
@@ -121,6 +146,8 @@ class SegmentationTrainer:
         self.curr_iter, self.epoch = state["iteration"] + 1, state["epoch"]
         self.model.load_state_dict(state["state_dict"])
         ME.bump_weights_epoch()
+        if self.world > 1:
+            broadcast_state(self.model, self.optimizer)
         if self.config.train.get("resume_optimizer", True):
             # the reference passes the whole config here (`train.py:85`).  Constructing a scheduler takes one step from `last_step`,
             # so it stands where it stood after `iteration` steps.
@@ -131,17 +158,23 @@ class SegmentationTrainer:
         logging.info(f"=> loaded checkpoint '{fn}' (epoch {state['epoch']})")
 
     def train(self, data_loader, val_data_loader):
-        """`lib/train.py:46-232` on one GPU without tensorboard: `iter_size` sub-batches per step from `data_loader` (an endless
+        """`lib/train.py:46-232` without tensorboard: `iter_size` sub-batches per step from `data_loader` (an endless
         `semseg_data.VoxelizationLoader`), `_set_seed` before every step, loss / precision@1 / learning rate logged every
         `config.train.stat_freq` steps, a checkpoint every `save_freq` (`checkpoint`), `validate` on `val_data_loader` every `val_freq`
         with a "best_val" checkpoint whenever the mIoU improves, and a final checkpoint and validation at `optimizer.max_iter`.
         `config.train.resume`: a directory whose `weights.pth` restores iteration, epoch, weights, optimiser, scheduler position and
-        best_val.  Returns (best_val mIoU, its iteration)."""
+        best_val.  Returns (best_val mIoU, its iteration).
+
+        On several ranks `data_loader` is this rank's shard; the logged loss and score are sums over the ranks (one all-reduce at
+        each `stat_freq`) logged by rank 0, which alone writes checkpoints.  `val_data_loader` may be a sharded pass loader: `test`
+        reduces its metrics, so every rank gets the same mIoU and takes the same best_val decision."""
         config, model = self.config, self.model
         self.curr_iter, self.epoch, self.best_val, self.best_val_iter = 1, 1, 0, 0
         if config.train.get("resume"):
             self.resume(config.train.resume)
         curr_iter, epoch, best_val_miou, best_val_iter = self.curr_iter, self.epoch, self.best_val, self.best_val_iter
+        if self.rank == 0:
+            logging.info("===> Start training on {} GPUs, batch-size={}".format(self.world, data_loader.batch_size * self.world))
         num_labels = data_loader.dataset.NUM_LABELS
         scores = SegmentationMetrics(num_labels, self.ignore_label, self.device)
         loss_sum = torch.zeros(2, dtype=torch.float64, device=self.device)              # sum of step loss * rows, rows
@@ -158,10 +191,14 @@ class SegmentationTrainer:
                     is_training = False
                     break
                 if curr_iter % config.train.stat_freq == 0 or curr_iter == 1:
-                    host = torch.cat([loss_sum, scores.stats]).cpu().numpy()
+                    stats = torch.cat([loss_sum, scores.stats])
+                    if self.world > 1:
+                        dist.all_reduce(stats)
+                    host = stats.cpu().numpy()
                     lrs = ", ".join("{:.3e}".format(x) for x in self.scheduler.get_last_lr())
-                    logging.info("===> Epoch[{}]({}/{}): Loss {:.4f}\tLR: {}\tScore {:.3f}".format(
-                        epoch, curr_iter, steps_per_epoch, host[0] / host[1], lrs, host[3] / host[4]))
+                    if self.rank == 0:
+                        logging.info("===> Epoch[{}]({}/{}): Loss {:.4f}\tLR: {}\tScore {:.3f}".format(
+                            epoch, curr_iter, steps_per_epoch, host[0] / host[1], lrs, host[3] / host[4]))
                     loss_sum.zero_()
                     scores.reset()
                 if curr_iter % config.train.save_freq == 0:
@@ -171,7 +208,8 @@ class SegmentationTrainer:
                     if val_miou > best_val_miou:
                         best_val_miou, best_val_iter = val_miou, curr_iter
                         checkpoint(model, self.optimizer, epoch, curr_iter, config, best_val_miou, best_val_iter, "best_val")
-                    logging.info("Current best mIoU: {:.3f} at iter {}".format(best_val_miou, best_val_iter))
+                    if self.rank == 0:
+                        logging.info("Current best mIoU: {:.3f} at iter {}".format(best_val_miou, best_val_iter))
                     model.train()
                 curr_iter += 1
             epoch += 1                    # also after the last step, as `train.py:219` counts it
@@ -180,7 +218,8 @@ class SegmentationTrainer:
         if val_miou > best_val_miou:
             best_val_miou, best_val_iter = val_miou, curr_iter
             checkpoint(model, self.optimizer, epoch, curr_iter, config, best_val_miou, best_val_iter, "best_val")
-        logging.info("Current best mIoU: {:.3f} at iter {}".format(best_val_miou, best_val_iter))
+        if self.rank == 0:
+            logging.info("Current best mIoU: {:.3f} at iter {}".format(best_val_miou, best_val_iter))
         self.best_val, self.best_val_iter, self.epoch = best_val_miou, best_val_iter, epoch
         return best_val_miou, best_val_iter
 
@@ -194,7 +233,10 @@ def _set_seed(config, step):
 
 def checkpoint(model, optimizer, epoch, iteration, config, best_val=None, best_val_iter=None, postfix=None):
     """`lib/utils.py:78-114`: `weights/checkpoint_{wrapper_type}{model}[postfix].pth` under the working directory (`_iter_{iteration}`
-    instead of the postfix when `config.train.overwrite_weights` is false), and the relative link `weights/weights.pth` to it."""
+    instead of the postfix when `config.train.overwrite_weights` is false), and the relative link `weights/weights.pth` to it.  On
+    several ranks only rank 0 writes."""
+    if get_rank() > 0:
+        return
     os.makedirs("weights", exist_ok=True)
     stem = f"checkpoint_{config.net.get('wrapper_type')}{config.net.model}"
     if config.train.get("overwrite_weights", True):
@@ -217,7 +259,8 @@ def checkpoint(model, optimizer, epoch, iteration, config, best_val=None, best_v
 def validate(model, val_data_loader, curr_iter, config):
     """`lib/train.py:30-35` without tensorboard: `test`, the three scalars logged, the mIoU returned."""
     v_loss, v_score, v_mAP, v_mIoU = test(model, val_data_loader, config)
-    logging.info(f"validation at iter {curr_iter}: mIoU {v_mIoU:.3f} loss {v_loss:.4f} precision@1 {v_score:.3f} mAP {v_mAP:.3f}")
+    if get_rank() == 0:
+        logging.info(f"validation at iter {curr_iter}: mIoU {v_mIoU:.3f} loss {v_loss:.4f} precision@1 {v_score:.3f} mAP {v_mAP:.3f}")
     return v_mIoU
 
 
@@ -258,6 +301,13 @@ class SegmentationMetrics:
 
     def reset(self):
         self._buf.zero_()
+
+    def all_reduce(self):
+        """In place: every field summed over the ranks -- two all-reduces, the fp64 words (stats, ap_sum) as fp64 and the int64 ones
+        (hist, ap_cnt) as int64 (an integer sum of the fp64 bit patterns would be meaningless)."""
+        C = self.C
+        dist.all_reduce(self._buf[:3 + C].view(torch.float64))
+        dist.all_reduce(self._buf[3 + C:])
 
     def update(self, logits, target, average_precision=True):
         """Adds one batch: logits fp32 [n, C], target int [n] (device).  Returns pred (int32 [n]) and prob (fp32 [n, C], None
@@ -323,11 +373,19 @@ def test(model, data_loader, config, has_gt=True, evaluator=None):
     `config.test.test_original_pointcloud`: the predictions go, on the device, into a `PointCloudEvaluator` (`evaluator`, else a new
     one writing ScanNet's submission files under `<save_pred_dir>/fulleval`, or under a new temporary directory without
     `save_prediction`; the directory is logged), which logs the full-resolution IoU.  Both need `data.return_transformation` and a
-    loader in dataset order."""
+    loader in dataset order, unsharded.
+
+    A sharded loader (`world` > 1, e.g. `VoxelizationPassLoader(..., rank, world)` on each rank): each rank runs its batches, the
+    metrics are summed over the ranks before the final line and the result, which are then those of the whole pass; the
+    intermediate lines are rank 0's own batches.  Only rank 0 logs."""
     if config.test.get("evaluate_original_pointcloud"):
         raise NotImplementedError("test.evaluate_original_pointcloud")          # the reference raises it too (`test.py:126-127`)
     dataset = data_loader.dataset
     save, full = bool(config.test.get("save_prediction")), bool(config.test.get("test_original_pointcloud"))
+    sharded = getattr(data_loader, "world", 1) > 1
+    if sharded and (save or full):
+        raise ValueError(f"test.{'save_prediction' if save else 'test_original_pointcloud'} needs an unsharded loader")
+    master = get_rank() == 0
     save_pred_dir = None
     if save or full:
         if not getattr(dataset, "IS_FULL_POINTCLOUD_EVAL", False):
@@ -350,7 +408,8 @@ def test(model, data_loader, config, has_gt=True, evaluator=None):
         logging.info(f"Full pointcloud evaluation: submission files go to {eval_path}")
         evaluator = PointCloudEvaluator(dataset, device, eval_path=eval_path)
     class_names = getattr(dataset, "CLASS_LABELS", None)
-    logging.info("===> Start testing")
+    if master:
+        logging.info("===> Start testing")
     t_start = time.time()
     max_iter = len(data_loader)
     model.eval()
@@ -381,11 +440,14 @@ def test(model, data_loader, config, has_gt=True, evaluator=None):
                     for b, (centres, labels) in enumerate(pieces):
                         evaluator.add(first + b, centres, labels)
                 first += getattr(data_loader, "batch_size", len(pieces))
-            if iteration % config.test.test_stat_freq == 0 and iteration > 0:
+            if iteration % config.test.test_stat_freq == 0 and iteration > 0 and master:
                 print_info(iteration, max_iter, data_time, iter_time, has_gt, metrics.result(), class_names)
+    if sharded:
+        metrics.all_reduce()
     r = metrics.result()
-    print_info(iteration, max_iter, data_time, iter_time, has_gt, r, class_names)
-    logging.info("Finished test. Elapsed time: {:.4f}".format(time.time() - t_start))
+    if master:
+        print_info(iteration, max_iter, data_time, iter_time, has_gt, r, class_names)
+        logging.info("Finished test. Elapsed time: {:.4f}".format(time.time() - t_start))
     if full:
         evaluator.finish()
     return r.tuple()

@@ -762,16 +762,33 @@ class cflt_collate_fn_factory:
         return coords_batch, feats_batch, labels_batch, torch.from_numpy(np.stack(rows).astype(np.float32))
 
 
+def _rank_world(rank, world):
+    from .trainer import get_rank, get_world_size
+    rank = get_rank() if rank is None else int(rank)
+    world = get_world_size() if world is None else int(world)
+    if world < 1 or not 0 <= rank < world:
+        raise ValueError(f"rank {rank} of world {world}")
+    return rank, world
+
+
 class VoxelizationLoader:
     """The training loader (`dataset.py:311-385` with `repeat=True`): endless; each item is a list of `iter_size` collated sub-batches
     (coords, feats, target) -- what `semseg.SegmentationTrainer.train_step` takes.  `normalize_color` applies `lib/train.py:114`
-    (colour / 255 - 0.5) to each sub-batch."""
+    (colour / 255 - 0.5) to each sub-batch.
 
-    def __init__(self, dataset, batch_size, collate_fn, iter_size=1, shuffle=True, normalize_color=False):
+    Data parallel (`dataset.py:374-376`): rank `rank` of `world` (default: torch.distributed's, else 0 of 1) takes every world-th
+    entry of the shared endless permutation, `batch_size` scenes per sub-batch on each rank (the global batch is batch_size * world),
+    `ceil(n / world) // batch_size` items per epoch.  `seed`: the permutations come from their own generator (`shared_randperm`),
+    which the ranks need to draw the same ones; None draws them from the global torch RNG."""
+
+    def __init__(self, dataset, batch_size, collate_fn, iter_size=1, shuffle=True, normalize_color=False, rank=None, world=None, seed=None):
         from .scannet_pairs import DistributedInfSampler
         self.dataset, self.batch_size, self.collate_fn = dataset, batch_size, collate_fn
         self.iter_size, self.normalize_color = iter_size, normalize_color
-        self.sampler = DistributedInfSampler(len(dataset), 1, 0, shuffle)
+        self.rank, self.world = _rank_world(rank, world)
+        if self.world > 1 and shuffle and seed is None:
+            raise ValueError("a shuffled loader on several ranks needs a seed shared by the ranks")
+        self.sampler = DistributedInfSampler(len(dataset), self.world, self.rank, shuffle, seed=seed)
 
     def __len__(self):
         return len(self.sampler) // self.batch_size
@@ -791,18 +808,33 @@ class VoxelizationPassLoader:
     """The evaluation loader (`dataset.py:311-385` with `repeat=False`): one pass over the dataset in sampler order (a fresh permutation
     per pass when `shuffle`), `ceil(n / batch_size)` items, the last one possibly short.  Each item is one collated (coords, feats,
     target), colours normalised once when `normalize_color` -- what `semseg.test` takes.  With `cflt_collate_fn_factory` the items are
-    (coords, feats, target, transformation)."""
+    (coords, feats, target, transformation).
 
-    def __init__(self, dataset, batch_size, collate_fn, shuffle=False, normalize_color=False):
+    Sharded (`rank` / `world`, default 0 of 1): rank r gets batches b = r, r + world, ... of the batch sequence one process makes --
+    the same order and batch composition, so the per-batch AP means are the same numbers -- possibly none.  `seed`: each pass's
+    permutation comes from its own generator (`shared_randperm`, seeded by (seed, pass count)), which shuffled shards need; None
+    draws it from the global torch RNG."""
+
+    def __init__(self, dataset, batch_size, collate_fn, shuffle=False, normalize_color=False, rank=0, world=1, seed=None):
         self.dataset, self.batch_size, self.collate_fn = dataset, batch_size, collate_fn
         self.shuffle, self.normalize_color = shuffle, normalize_color
+        self.rank, self.world = _rank_world(rank, world)
+        if self.world > 1 and shuffle and seed is None:
+            raise ValueError("a shuffled sharded pass needs a seed shared by the ranks")
+        self.seed, self.passes = seed, 0
 
-    def __len__(self):
+    def num_batches(self):
+        """The number of batches of the whole pass (all ranks)."""
         return (len(self.dataset) + self.batch_size - 1) // self.batch_size
 
+    def __len__(self):
+        return len(range(self.rank, self.num_batches(), self.world))
+
     def __iter__(self):
-        order = torch.randperm(len(self.dataset)).tolist() if self.shuffle else list(range(len(self.dataset)))
-        for b in range(len(self)):
+        from .scannet_pairs import shared_randperm
+        order = shared_randperm(len(self.dataset), self.seed, self.passes).tolist() if self.shuffle else list(range(len(self.dataset)))
+        self.passes += 1
+        for b in range(self.rank, self.num_batches(), self.world):
             item = self.collate_fn([self.dataset[i] for i in order[b * self.batch_size:(b + 1) * self.batch_size]])
             if self.normalize_color:
                 input_transform(None, item[1], normalize=True)
@@ -810,11 +842,15 @@ class VoxelizationPassLoader:
 
 
 def initialize_data_loader(DatasetClass, config, phase, shuffle, augment_data, batch_size, limit_numpoints, iter_size=1, normalize_color=True,
-                           input_transform=None, target_transform=None, device="cuda", draws=None, repeat=True, **dataset_kwargs):
+                           input_transform=None, target_transform=None, device="cuda", draws=None, repeat=True, rank=None, world=None,
+                           **dataset_kwargs):
     """`dataset.py:311-385`: elastic distortion before voxelisation, then dropout, flip, auto-contrast, colour translation and jitter
     (`config.augmentation.data_aug_color_trans_ratio` / `data_aug_color_jitter_std`).  `repeat=True`: the endless training loader;
     `repeat=False`: one pass (`VoxelizationPassLoader`, `iter_size` unused), whose items carry the transformations
-    (`cflt_collate_fn_factory`) when `config.data.return_transformation` is set."""
+    (`cflt_collate_fn_factory`) when `config.data.return_transformation` is set.
+
+    `rank` / `world`: the training loader's shard (default: torch.distributed's); the pass loader is sharded only when they are given.
+    On several ranks the permutations come from a generator seeded by `config.misc.seed`; on one, from the global torch RNG."""
     prevoxel = [ElasticDistortion(DatasetClass.ELASTIC_DISTORT_PARAMS, draws=draws)] if augment_data else []
     transforms = list(input_transform or [])
     if augment_data:
@@ -826,6 +862,9 @@ def initialize_data_loader(DatasetClass, config, phase, shuffle, augment_data, b
                            augment_data=augment_data, phase=phase, device=device, draws=draws, **dataset_kwargs)
     if not repeat:
         collate = cflt_collate_fn_factory if config.data.get("return_transformation") else cfl_collate_fn_factory
-        return VoxelizationPassLoader(dataset, batch_size, collate(limit_numpoints), shuffle=shuffle, normalize_color=normalize_color)
+        rank, world = _rank_world(rank or 0, world or 1)
+        return VoxelizationPassLoader(dataset, batch_size, collate(limit_numpoints), shuffle=shuffle, normalize_color=normalize_color,
+                                      rank=rank, world=world, seed=config.misc.seed if world > 1 else None)
+    rank, world = _rank_world(rank, world)
     return VoxelizationLoader(dataset, batch_size, cfl_collate_fn_factory(limit_numpoints), iter_size=iter_size, shuffle=shuffle,
-                              normalize_color=normalize_color)
+                              normalize_color=normalize_color, rank=rank, world=world, seed=config.misc.seed if world > 1 else None)

@@ -51,6 +51,88 @@ def load_state(model, weights, lenient_weight_loading=False):
     model.load_state_dict(weights, strict=True)
 
 
+def broadcast_state(model, optimizer):
+    """DistributedDataParallel's construction: rank 0's parameters (the flat buffer) and buffers on every rank."""
+    dist.broadcast(optimizer.flat_param, 0)
+    ME.bump_weights_epoch()                      # the cached weight tiles are of the old values
+    for b in model.buffers():
+        dist.broadcast(b, 0)
+
+
+class GradientAllReduce:
+    """Sum all-reduce of `FlatSGD.flat_grad` over the ranks, overlapped with the backward pass (`ddp_trainer.py:96-102`:
+    DistributedDataParallel's buckets); the 1/world of the mean is folded into the SGD kernel through `grad_scale`.
+
+    Parameters are registered in forward order, so the fused backward sweep completes the flat gradient buffer from its END:
+    [decoder: convtr4p16s2 .. final] is complete once convtr4p16s2's unit has run backward (~85 % of the bytes together with the
+    next chunk, while the costly stride-1/2 encoder layers are still to come), [conv4p8s2 .. block4] after conv4p8s2's unit, the
+    rest at the end.  Each chunk's all-reduce is launched on a side stream as soon as its last weight gradient is enqueued (the
+    executor's `_fused_after_unit` hook); `finish` reduces the rest and makes the compute stream wait for every chunk.  A model
+    whose registration order is not this one gets one all-reduce in `finish`.
+
+    every_backward=False: the hook launches chunks only during a backward pass that `arm` announced -- with gradient accumulation,
+    the last sub-batch's; the earlier ones accumulate locally.  At world 1 nothing is installed and `finish` does nothing.
+    `timing` (a dict, else None): CUDA events of each all-reduce ("allreduce": [(start, end)]) and the start of `finish`
+    ("tail")."""
+
+    def __init__(self, model, optimizer, world, device, every_backward=True):
+        self.optimizer, self.world, self.every_backward = optimizer, world, every_backward
+        self.armed = every_backward
+        self.timing = None
+        self.chunk_after, self.comm = {}, None
+        self.pending_hi = optimizer.flat_grad.numel()
+        if world <= 1:
+            return
+        m = model
+        if fused.matches(m):
+            off = {id(p): o for p, o in zip(optimizer.param_groups[0]["params"], optimizer._offsets)}
+            b1, b2 = off[id(m.convtr4p16s2.kernel)], off[id(m.conv4p8s2.kernel)]
+            late = {id(p) for mod in (m.convtr4p16s2, m.bntr4, m.block5, m.convtr5p8s2, m.bntr5, m.block6, m.convtr6p4s2, m.bntr6,
+                                      m.block7, m.convtr7p2s2, m.bntr7, m.block8, m.final) for p in mod.parameters()}
+            mid = {id(p) for mod in (m.conv4p8s2, m.bn4, m.block4) for p in mod.parameters()}
+            if all((o >= b1) == (pid in late) and (b2 <= o < b1) == (pid in mid) for pid, o in off.items()):
+                self.chunk_after = {id(m.convtr4p16s2): b1, id(m.conv4p8s2): b2}
+                m.__dict__["_fused_after_unit"] = self._on_unit_backward_done
+        self.comm = torch.cuda.Stream(device=device)
+
+    def arm(self):
+        """The next backward pass is the last before `finish`: it launches the chunks it completes."""
+        self.armed = True
+
+    def _on_unit_backward_done(self, conv):
+        lo = self.chunk_after.get(id(conv))
+        if lo is not None and self.armed:
+            self._reduce_range(lo, self.pending_hi)
+
+    def _reduce_range(self, lo, hi):
+        if hi <= lo:
+            return
+        ev = torch.cuda.Event()
+        ev.record()                              # everything that wrote flat_grad[lo:hi] is enqueued before this point
+        self.comm.wait_event(ev)
+        with torch.cuda.stream(self.comm):
+            if self.timing is not None:
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+            dist.all_reduce(self.optimizer.flat_grad[lo:hi])
+            if self.timing is not None:
+                e1.record()
+                self.timing.setdefault("allreduce", []).append((e0, e1))
+        self.pending_hi = lo
+
+    def finish(self):
+        """The part of the flat gradient not yet reduced during the backward pass, then the compute stream waits for all chunks."""
+        if self.world <= 1:
+            return
+        if self.timing is not None:
+            t0 = torch.cuda.Event(enable_timing=True); t0.record()
+            self.timing["tail"] = [t0, None]
+        self._reduce_range(0, self.pending_hi)
+        self.pending_hi = self.optimizer.flat_grad.numel()
+        self.armed = self.every_backward
+        torch.cuda.current_stream().wait_stream(self.comm)
+
+
 class ContrastiveLossTrainer:
     def __init__(self, config, data_loader):
         assert config.misc.use_gpu and torch.cuda.is_available(), "DDP mode must support GPU"
@@ -92,13 +174,24 @@ class ContrastiveLossTrainer:
             if self.is_master:
                 logging.info("=> loaded checkpoint '%s' (curr_iter %d)", checkpoint_fn, state["curr_iter"])
         if self.world > 1:                       # DDP construction semantics: every rank starts from rank 0's state
-            dist.broadcast(self.optimizer.flat_param, 0)
-            ME.bump_weights_epoch()
-            for b in model.buffers():
-                dist.broadcast(b, 0)
+            broadcast_state(model, self.optimizer)
             self.optimizer.grad_scale = 1.0 / self.world
+        self._grads = GradientAllReduce(model, self.optimizer, self.world, self.device)
         self.timing = None                       # bench.py: dict -> CUDA events of one step (per-rank breakdown)
-        self._setup_gradient_chunks()
+
+    @property
+    def timing(self):
+        return self.__dict__.get("_timing")
+
+    @timing.setter
+    def timing(self, value):
+        self._timing = value
+        if "_grads" in self.__dict__:
+            self._grads.timing = value
+
+    @property
+    def _chunk_after(self):
+        return self._grads.chunk_after
 
     # -- checkpoint (`ddp_trainer.py:151-169`)
     def _save_checkpoint(self, curr_iter, filename="checkpoint"):
@@ -149,62 +242,8 @@ class ContrastiveLossTrainer:
         except StopIteration:
             self._staged = None
 
-    # -- gradient all-reduce, overlapped with the backward pass (`ddp_trainer.py:96-102`: DistributedDataParallel's buckets)
-    def _setup_gradient_chunks(self):
-        """Parameters are registered in forward order, so the backward sweep completes the flat gradient buffer from its END:
-        [decoder: convtr4p16s2 .. final] is complete once convtr4p16s2's unit has run backward (~85 % of the bytes together
-        with the next chunk, while the costly stride-1/2 encoder layers are still to come), [conv4p8s2 .. block4] after
-        conv4p8s2's unit, the rest at the end.  Each chunk's NCCL all-reduce (sum; 1/world is folded into the SGD kernel) is
-        launched on a side stream as soon as its last weight gradient is enqueued."""
-        self._chunk_after = {}
-        self._comm = None
-        m = self.model
-        if self.world <= 1 or not fused.matches(m):
-            return
-        off = {id(p): o for p, o in zip(self.optimizer.param_groups[0]["params"], self.optimizer._offsets)}
-        b1, b2 = off[id(m.convtr4p16s2.kernel)], off[id(m.conv4p8s2.kernel)]
-        late = {id(p) for mod in (m.convtr4p16s2, m.bntr4, m.block5, m.convtr5p8s2, m.bntr5, m.block6, m.convtr6p4s2, m.bntr6, m.block7,
-                                  m.convtr7p2s2, m.bntr7, m.block8, m.final) for p in mod.parameters()}
-        mid = {id(p) for mod in (m.conv4p8s2, m.bn4, m.block4) for p in mod.parameters()}
-        ok = all((o >= b1) == (pid in late) and (b2 <= o < b1) == (pid in mid) for pid, o in off.items())
-        if ok:                                   # else (unexpected registration order): one all-reduce after the backward pass
-            self._chunk_after = {id(m.convtr4p16s2): b1, id(m.conv4p8s2): b2}
-            m.__dict__["_fused_after_unit"] = self._on_unit_backward_done
-        self._comm = torch.cuda.Stream(device=self.device)
-        self._pending_hi = self.optimizer.flat_grad.numel()
-
-    def _on_unit_backward_done(self, conv):
-        lo = self._chunk_after.get(id(conv))
-        if lo is not None:
-            self._reduce_range(lo, self._pending_hi)
-
-    def _reduce_range(self, lo, hi):
-        if hi <= lo:
-            return
-        ev = torch.cuda.Event()
-        ev.record()                              # everything that wrote flat_grad[lo:hi] is enqueued before this point
-        comm = self._comm if self._comm is not None else torch.cuda.current_stream()
-        comm.wait_event(ev)
-        with torch.cuda.stream(comm):
-            if self.timing is not None:
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-            dist.all_reduce(self.optimizer.flat_grad[lo:hi])
-            if self.timing is not None:
-                e1.record()
-                self.timing.setdefault("allreduce", []).append((e0, e1))
-        self._pending_hi = lo
-
     def _all_reduce_grads(self):
-        """The part of the flat gradient not yet reduced during the backward pass, then the compute stream waits for all chunks."""
-        if self.world > 1:
-            if self.timing is not None:
-                t0 = torch.cuda.Event(enable_timing=True); t0.record()
-                self.timing["tail"] = [t0, None]
-            self._reduce_range(0, self._pending_hi)
-            self._pending_hi = self.optimizer.flat_grad.numel()
-            if self._comm is not None:
-                torch.cuda.current_stream().wait_stream(self._comm)
+        self._grads.finish()
 
     MAX_STEPS_IN_FLIGHT = 2
 
