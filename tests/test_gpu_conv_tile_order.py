@@ -16,10 +16,9 @@ from tests import exact_conv as X
 BM = 128
 
 
-def _order(tbl, n, window, ws=None):
+def _order(tbl, n, window):
     from pointcontrast_b200._lib import check, lib, ptr, stream
-    wsb = lib.pcb_conv_tile_order_ws_bytes(n)
-    ws = torch.empty(wsb, dtype=torch.uint8, device="cuda") if ws is None else ws
+    ws = torch.empty(lib.pcb_conv_tile_order_ws_bytes(n), dtype=torch.uint8, device="cuda")
     perm = torch.empty(n, dtype=torch.int32, device="cuda")
     check(lib.pcb_conv_tile_order(ptr(tbl), tbl.shape[1], tbl.shape[0], n, window, ptr(perm), ptr(ws), ws.numel(), stream()))
     return perm
@@ -41,14 +40,13 @@ def offsets_per_tile(mask, order):
 
 
 def test_tile_order_rejects_bad_arguments():
-    """Window not a multiple of 128, short workspace, too many offsets: PCB_ERR_ARG before the device is touched."""
+    """Window not a multiple of 128, too many offsets, a table narrower than n_out: PCB_ERR_ARG before the device is touched."""
     L = _lib.lib
     n = 1000
     wsb = L.pcb_conv_tile_order_ws_bytes(n)
     assert wsb > 0
     fake = 1 << 20          # never dereferenced: the checks return first
     assert L.pcb_conv_tile_order(fake, n, 27, n, 1000, fake, fake, wsb, None) == _lib.ERR_ARG
-    assert L.pcb_conv_tile_order(fake, n, 27, n, 1024, fake, fake, wsb - 1, None) == _lib.ERR_ARG
     assert L.pcb_conv_tile_order(fake, n, 28, n, 1024, fake, fake, wsb, None) == _lib.ERR_ARG
     assert L.pcb_conv_tile_order(fake, n - 1, 27, n, 1024, fake, fake, wsb, None) == _lib.ERR_ARG
     assert L.pcb_conv_tile_order(None, n, 27, 0, 1024, None, None, 0, None) == _lib.OK
@@ -76,8 +74,8 @@ def scene():
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind", ["k27", "down", "up"])
 def test_tile_order_matches_numpy_recount(scene, kind):
-    """perm is the stable (window, mask) sort, a permutation whose tiles stay inside one window, the same bytes on every build and
-    whatever the workspace size; the offsets per tile equal the numpy recount and never exceed the identity order's."""
+    """perm is the stable (window, mask) sort, a permutation whose tiles stay inside one window, the same bytes on every build; the
+    offsets per tile equal the numpy recount and never exceed the identity order's."""
     from pointcontrast_b200 import me
     tbl = scene[(kind, "fwd")][0]
     n_full = tbl.shape[1]
@@ -91,10 +89,6 @@ def test_tile_order_matches_numpy_recount(scene, kind):
             assert np.array_equal(got, want), what
             # position i holds a row of window i // window; windows are whole tiles, so every tile stays inside one window
             assert np.array_equal(got // window, np.arange(n) // window), what
-            big = torch.full((_lib.lib.pcb_conv_tile_order_ws_bytes(n) + (64 << 10),), 0xA5, dtype=torch.uint8, device="cuda")
-            tail = big[-(64 << 10):].clone()
-            assert torch.equal(_order(tbl, n, window, ws=big), perm), what
-            assert torch.equal(big[-(64 << 10):], tail), what + ": workspace tail touched"
             ordered, ident = offsets_per_tile(mask, got), offsets_per_tile(mask, np.arange(n))
             assert np.array_equal(ordered, offsets_per_tile(mask, want)), what
             if window >= 1024:

@@ -1,6 +1,6 @@
 """Semantic-segmentation evaluation on the GPU (`downstream/semseg/lib/test.py:62-196`, `lib/train.py:22-232`): `pcb_average_precision`
-and `pcb_seg_metrics` against the fp64 oracle (oracle/semseg_eval_cpu.py) and torch, their workspace contract, `SegmentationMetrics` on
-the reference's golden run, `semseg.test` on synthetic rooms, and `SegmentationTrainer.train` with checkpoints, validation and resume."""
+and `pcb_seg_metrics` against the fp64 oracle (oracle/semseg_eval_cpu.py) and torch, `SegmentationMetrics` on the reference's golden
+run, `semseg.test` on synthetic rooms, and `SegmentationTrainer.train` with checkpoints, validation and resume."""
 import os
 import warnings
 
@@ -10,7 +10,6 @@ import torch
 
 from oracle import semseg_eval_cpu as O
 from tests import refload
-from tests.test_workspace import TAIL, _In, _outputs, _st
 
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "semseg_eval.npz")
@@ -83,47 +82,6 @@ def test_average_precision_scannet_size():
     x = torch.from_numpy(g.standard_normal((n, C)).astype(np.float32))
     x[torch.arange(n), torch.from_numpy(np.minimum(t, C - 1))] += 1.5
     _check_ap(torch.softmax(x, 1).numpy(), t)
-
-
-def _seg_case(n, C):
-    i = _In(21)
-    x, t = i.rand(n, C, scale=4.0), i.randint(0, C + 3, n, dtype=torch.int64)
-    pred, prob = _In.zeros(n, dtype=torch.int32), _In.zeros(n, C)
-    hist, stats = _In.zeros(C * C, dtype=torch.int64), _In.zeros(3, dtype=torch.float64)
-    L = _L().lib
-    return (L.pcb_seg_metrics_ws_bytes(n),
-            lambda ws, b: L.pcb_seg_metrics(x.data_ptr(), t.data_ptr(), n, C, C, pred.data_ptr(), prob.data_ptr(), hist.data_ptr(),
-                                            stats.data_ptr(), ws, b, _st()),
-            _outputs(pred, prob, hist, stats))
-
-
-def _ap_case(n, C):
-    i = _In(22)
-    s, t = i.rand(n, C), i.randint(0, C, n, dtype=torch.int64)
-    ap_sum, ap_cnt = _In.zeros(C, dtype=torch.float64), _In.zeros(C, dtype=torch.int64)
-    L = _L().lib
-    return (L.pcb_average_precision_ws_bytes(n, C),
-            lambda ws, b: L.pcb_average_precision(s.data_ptr(), t.data_ptr(), n, C, ap_sum.data_ptr(), ap_cnt.data_ptr(), ws, b, _st()),
-            _outputs(ap_sum, ap_cnt))
-
-
-@pytest.mark.parametrize("case,args", [(_seg_case, (300, 20)), (_seg_case, (100_000, 20)), (_ap_case, (300, 20)), (_ap_case, (100_000, 20))],
-                         ids=["seg300", "seg100000", "ap300", "ap100000"])
-def test_workspace_tail_untouched_and_size_independent(case, args):
-    """the same check as tests/test_workspace.py, plus a second call into the same workspace"""
-    q, call, outputs = case(*args)
-    ws = torch.full((q + TAIL,), 0xA5, dtype=torch.uint8, device="cuda")
-    _L().check(call(ws.data_ptr(), q))
-    torch.cuda.synchronize()
-    assert bool((ws[q:] == 0xA5).all()), "bytes at or beyond the query were written"
-    exact = outputs()
-    for size in (q, max(64 << 20, q + 1)):
-        q2, call2, outputs2 = case(*args)
-        big = torch.full((size,), 0x5A, dtype=torch.uint8, device="cuda")
-        _L().check(call2(big.data_ptr(), size))
-        torch.cuda.synchronize()
-        for a, b in zip(exact, outputs2()):
-            assert a.tobytes() == b.tobytes()
 
 
 def test_seg_metrics_against_torch():

