@@ -1,50 +1,19 @@
-"""Stages the original VoteNet detection datasets next to the oracle, so that the tests, tests/golden/make_det_data_golden.py and
-profiles/bench_det_data.py can run their `__getitem__` unmodified against pointcontrast_b200.det_data:
-
-    python oracle/det_data_ref.py       (also run by __graft_entry__.build(), after oracle/det_eval_ref.py, which clears and stages
-                                         oracle/_ref/votenet/lib/ with the model-util modules these files import)
-
-Copies, byte for byte, `lib/datasets/scannet/scannet_detection_dataset.py`, `lib/datasets/sunrgbd/sunrgbd_detection_dataset.py` and
-`lib/utils/pc_util.py` from `<root>/downstream/votenet_det_new/` into `oracle/_ref/votenet/` (git-ignored).  <root> is
-$PCB_REFERENCE_ROOT, with the same default as oracle/stage_ref.py; where the original is absent nothing is staged.  Nothing under
-pointcontrast_b200/ imports this.
+"""The original VoteNet detection datasets, staged by oracle/stage_ref.py under `oracle/_ref/votenet/lib/` beside the model-util
+modules they import, so that the tests, tests/golden/make_det_data_golden.py and profiles/bench_det_data.py can run their `__getitem__`
+unmodified against pointcontrast_b200.det_data.  Nothing under pointcontrast_b200/ imports this.
 
 load() imports both modules the way the original runs them, through oracle/det_eval_ref.load() (its root and `lib/utils` on sys.path,
 stubs for trimesh, matplotlib and cv2, which `pc_util` and `sunrgbd_utils` import but these paths never call).
 """
 import importlib
-import os
-import shutil
 
 from oracle import det_eval_ref
-
-SRC = det_eval_ref.SRC
-ROOT = det_eval_ref.ROOT
-FILES = (os.path.join("lib", "datasets", "scannet", "scannet_detection_dataset.py"),
-         os.path.join("lib", "datasets", "sunrgbd", "sunrgbd_detection_dataset.py"),
-         os.path.join("lib", "utils", "pc_util.py"))
-
-
-def stage(verbose=False):
-    if not os.path.isfile(os.path.join(SRC, FILES[0])) or not det_eval_ref.available():
-        return False
-    for f in FILES:
-        os.makedirs(os.path.dirname(os.path.join(ROOT, f)), exist_ok=True)
-        shutil.copyfile(os.path.join(SRC, f), os.path.join(ROOT, f))
-    if verbose:
-        print("staged", SRC, "(detection datasets) ->", ROOT)
-    return True
-
-
-def available():
-    return det_eval_ref.available() and all(os.path.isfile(os.path.join(ROOT, f)) for f in FILES)
 
 
 def load():
     """(scannet_detection_dataset, sunrgbd_detection_dataset) modules of the original, or None where nothing is staged."""
-    if not available():
+    if det_eval_ref.load() is None:
         return None
-    det_eval_ref.load()
     return (importlib.import_module("lib.datasets.scannet.scannet_detection_dataset"),
             importlib.import_module("lib.datasets.sunrgbd.sunrgbd_detection_dataset"))
 
@@ -63,7 +32,3 @@ def item(module_cls, data_path, scan_names, num_points, use_color, use_height, a
         return ds[idx]
     finally:
         np.random.random, np.random.choice = saved
-
-
-if __name__ == "__main__":
-    print("staged" if stage(True) else f"{SRC} not present (or the evaluation code is not staged): nothing staged")

@@ -1,40 +1,21 @@
-"""Stages the original pair-list scripts next to the oracle, so that tests/test_oracle_pair_list.py can run them unmodified:
-
-    python oracle/pair_list_ref.py      (also run by __graft_entry__.build())
-
-Copies `<root>/pretrain/data_preprocess/scannet_pair/{compute_full_overlapping.py, generate_list.py}` byte for byte into
-`oracle/_ref/data_preprocess/` (git-ignored).  <root> is $PCB_REFERENCE_ROOT, with the same default as oracle/stage_ref.py; where the
-original is absent nothing is staged.  Nothing under pointcontrast_b200/ imports this.
+"""The original pair-list scripts (`compute_full_overlapping.py`, `generate_list.py`), staged by oracle/stage_ref.py under
+`oracle/_ref/data_preprocess/`, so that tests/test_oracle_pair_list.py can run them unmodified.  Nothing under pointcontrast_b200/
+imports this.
 
 run(script, argv) executes a staged script as `python <script> <argv>` would, with stub `open3d` and `SensorData` modules in place of
 the absent packages: the stub's `voxel_down_sample` and `KDTreeFlann.search_radius_vector_3d` are oracle/pair_list_cpu.py's.
 """
 import os
 import runpy
-import shutil
-import sys
 import types
 
 import numpy as np
 
-SRC = os.path.join(os.environ.get("PCB_REFERENCE_ROOT", "/root/reference"), "pretrain", "data_preprocess", "scannet_pair")
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref", "data_preprocess")
-FILES = ("compute_full_overlapping.py", "generate_list.py")
-
-
-def stage(verbose=False):
-    if not all(os.path.isfile(os.path.join(SRC, f)) for f in FILES):
-        return False
-    os.makedirs(ROOT, exist_ok=True)
-    for f in FILES:
-        shutil.copyfile(os.path.join(SRC, f), os.path.join(ROOT, f))
-    if verbose:
-        print("staged", SRC, "(pair list) ->", ROOT)
-    return True
+from oracle import stage_ref
 
 
 def available():
-    return all(os.path.isfile(os.path.join(ROOT, f)) for f in FILES)
+    return stage_ref.available("data_preprocess")
 
 
 class PointCloud:
@@ -56,7 +37,7 @@ class KDTreeFlann:
     (oracle decision, ascending distance)."""
 
     def __init__(self, pcd):
-        from scipy.spatial import cKDTree             # only where the stub runs: stage() needs no scipy
+        from scipy.spatial import cKDTree
         self.points = np.asarray(pcd.points, np.float64)
         self.tree = cKDTree(self.points)
 
@@ -80,20 +61,8 @@ def _stubs():
 
 
 def run(script, argv):
-    """Runs the staged `script` (a name of FILES) with command-line arguments `argv` under the stubs."""
-    saved_argv, saved_mods = sys.argv, {k: sys.modules.get(k) for k in ("open3d", "SensorData")}
-    sys.argv = [os.path.join(ROOT, script)] + list(argv)
-    sys.modules.update(_stubs())
-    try:
-        runpy.run_path(os.path.join(ROOT, script), run_name="__main__")
-    finally:
-        sys.argv = saved_argv
-        for k, v in saved_mods.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
-
-
-if __name__ == "__main__":
-    print("staged" if stage(True) else f"{SRC} not present: nothing staged")
+    """Runs the staged `script` (`compute_full_overlapping.py` or `generate_list.py`) with command-line arguments `argv` under the
+    stubs."""
+    script = stage_ref.path("data_preprocess", script)
+    with stage_ref.installed(_stubs(), argv=[script] + list(argv)):
+        runpy.run_path(script, run_name="__main__")

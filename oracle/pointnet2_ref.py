@@ -1,27 +1,24 @@
 """Compiles the original repository's PointNet++ extension (`downstream/votenet_det_new/models/backbone/pointnet2/_ext_src`) for sm_90a,
-so that the GPU tests and profiles/bench_pointnet2.py can run the reference's own kernels next to this library's, and stages its Python
-layer (`pointnet2_utils.py`, `pointnet2_modules.py`, `pytorch_utils.py`) into `oracle/_ref/votenet/pointnet2/`, where the tests run
-it unmodified on pointcontrast_b200.pointnet2 and on oracle.pointnet2_cpu.
+so that the GPU tests and profiles/bench_pointnet2.py can run the reference's own kernels next to this library's.  Its Python layer is
+staged by oracle/stage_ref.py under `oracle/_ref/votenet/pointnet2/`, where the tests run it unmodified on pointcontrast_b200.pointnet2
+and on oracle.pointnet2_cpu.
 
-    python oracle/pointnet2_ref.py       (also run by __graft_entry__.build())
+    python -m oracle.pointnet2_ref       (also run by __graft_entry__.build())
 
 Builds `oracle/_ref/pointnet2_ext/_ext*.so` (git-ignored) with torch.utils.cpp_extension, TORCH_CUDA_ARCH_LIST=9.0a and
 `-O3 --fmad=false`: with one rounding per operation the reference's distance predicates are reproducible on the host (DESIGN.md §6).
-The original repository is found at $PCB_REFERENCE_ROOT, with the same default as oracle/stage_ref.py.  Where it is absent
-nothing is built or staged and load() returns None; where it is present, a failing compile raises.
-Nothing under pointcontrast_b200/ imports this.
+The original repository is found at oracle/stage_ref.py's REFERENCE.  Where it is absent nothing is built; where it is present, a
+failing compile raises.  Nothing under pointcontrast_b200/ imports this.
 """
 import glob
 import importlib.machinery
 import importlib.util
 import os
-import shutil
 
-PN2 = os.path.join(os.environ.get("PCB_REFERENCE_ROOT", "/root/reference"), "downstream", "votenet_det_new", "models", "backbone", "pointnet2")
-SRC = os.path.join(PN2, "_ext_src")
-OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref", "pointnet2_ext")
-PY_DST = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref", "votenet", "pointnet2")
-PY_FILES = ("pointnet2_utils.py", "pointnet2_modules.py", "pytorch_utils.py")
+from oracle import stage_ref
+
+SRC = os.path.join(stage_ref.REFERENCE, "downstream", "votenet_det_new", "models", "backbone", "pointnet2", "_ext_src")
+OUT = os.path.join(stage_ref.STAGED, "pointnet2_ext")
 
 
 def _built():
@@ -30,14 +27,9 @@ def _built():
 
 
 def build(verbose=False):
-    """Stage the Python layer and compile (or bring up to date) the reference extension; False where the original repository is absent."""
+    """Compile (or bring up to date) the reference extension; False where the original repository is absent."""
     if not os.path.isdir(SRC):
         return False
-    os.makedirs(PY_DST, exist_ok=True)
-    for f in PY_FILES:
-        shutil.copyfile(os.path.join(PN2, f), os.path.join(PY_DST, f))
-    if verbose:
-        print("staged", PN2, PY_FILES, "->", PY_DST)
     from torch.utils import cpp_extension
     os.makedirs(OUT, exist_ok=True)
     os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0a"

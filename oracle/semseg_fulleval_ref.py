@@ -1,11 +1,6 @@
-"""Stages the original semantic-segmentation full point-cloud evaluation next to the oracle, so that
-tests/golden/make_semseg_fulleval_golden.py can run it unmodified:
-
-    python oracle/semseg_fulleval_ref.py      (also run by __graft_entry__.build())
-
-Copies, byte for byte, `<root>/downstream/semseg/lib/{utils.py, datasets/scannet.py, datasets/stanford.py}` into
-`oracle/_ref/semseg/lib/` (git-ignored).  <root> is $PCB_REFERENCE_ROOT, with the same default as oracle/stage_ref.py; where the
-original is absent nothing is staged.  Nothing under pointcontrast_b200/ imports this.
+"""The original semantic-segmentation full point-cloud evaluation (`lib/{utils.py, datasets/scannet.py, datasets/stanford.py}`),
+staged by oracle/stage_ref.py under `oracle/_ref/semseg/lib/`, so that tests/golden/make_semseg_fulleval_golden.py can run it
+unmodified.  Nothing under pointcontrast_b200/ imports this.
 
 load() imports the three staged modules under the package name `lib`, with stand-ins for what they import but this path does not
 compute with: `omegaconf`, `plyfile`, `lib.distributed_utils`, `lib.transforms`, `lib.dataset` (the base classes, `DatasetPhase`,
@@ -27,31 +22,13 @@ import contextlib
 import enum
 import importlib.util
 import os
-import shutil
 import sys
 import types
 from pathlib import Path
 
 import numpy as np
 
-SRC = os.path.join(os.environ.get("PCB_REFERENCE_ROOT", "/root/reference"), "downstream", "semseg", "lib")
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref", "semseg", "lib")
-FILES = ("utils.py", os.path.join("datasets", "scannet.py"), os.path.join("datasets", "stanford.py"))
-
-
-def stage(verbose=False):
-    if not all(os.path.isfile(os.path.join(SRC, f)) for f in FILES):
-        return False
-    for f in FILES:
-        os.makedirs(os.path.dirname(os.path.join(ROOT, f)), exist_ok=True)
-        shutil.copyfile(os.path.join(SRC, f), os.path.join(ROOT, f))
-    if verbose:
-        print("staged", SRC, "(semseg full point-cloud evaluation) ->", ROOT)
-    return True
-
-
-def available():
-    return all(os.path.isfile(os.path.join(ROOT, f)) for f in FILES)
+from oracle import stage_ref
 
 
 class _Anything:
@@ -94,6 +71,7 @@ class OnlineVoxelizationDatasetBase:
 
 
 _MODS = {}
+# the stand-in and staged modules, in sys.modules while the original runs (it imports `lib.dataset` inside a function)
 _STUBS = {}
 
 
@@ -102,9 +80,9 @@ def load():
     if _MODS:
         return _MODS["utils"], _MODS["scannet"], _MODS["stanford"]
     lib = types.ModuleType("lib")
-    lib.__path__ = [ROOT]
+    lib.__path__ = [stage_ref.path("semseg/lib")]
     datasets = types.ModuleType("lib.datasets")
-    datasets.__path__ = [os.path.join(ROOT, "datasets")]
+    datasets.__path__ = [stage_ref.path("semseg/lib", "datasets")]
     stubs = {"lib": lib, "lib.datasets": datasets, "omegaconf": _module("omegaconf"), "plyfile": _module("plyfile"),
              "lib.distributed_utils": _module("lib.distributed_utils", get_world_size=lambda: 1, get_rank=lambda: 0),
              "lib.transforms": _module("lib.transforms"),
@@ -113,32 +91,17 @@ def load():
              "lib.dataset": _module("lib.dataset", VoxelizationDataset=_Base, DatasetPhase=DatasetPhase, cache=lambda f: f,
                                     str2datasetphase_type=lambda s: DatasetPhase[s], OnlineVoxelizationDatasetBase=OnlineVoxelizationDatasetBase)}
     _STUBS.update(stubs)
-    with _installed():
-        for name, f in (("utils", FILES[0]), ("scannet", FILES[1]), ("stanford", FILES[2])):
-            full = "lib.utils" if name == "utils" else "lib.datasets." + name
-            spec = importlib.util.spec_from_file_location(full, os.path.join(ROOT, f))
+    staged = (("utils", "lib.utils", "utils.py"), ("scannet", "lib.datasets.scannet", "datasets/scannet.py"),
+              ("stanford", "lib.datasets.stanford", "datasets/stanford.py"))
+    with stage_ref.installed({**_STUBS, **{full: None for _, full, _ in staged}}):
+        for name, full, f in staged:
+            spec = importlib.util.spec_from_file_location(full, stage_ref.path("semseg/lib", f))
             m = importlib.util.module_from_spec(spec)
             sys.modules[full] = m
             spec.loader.exec_module(m)
             _MODS[name] = m
             _STUBS[full] = m
     return _MODS["utils"], _MODS["scannet"], _MODS["stanford"]
-
-
-@contextlib.contextmanager
-def _installed():
-    """The stand-in and staged modules in sys.modules while the original runs (it imports `lib.dataset` inside a function)."""
-    names = list(_STUBS) + ["lib.utils", "lib.datasets.scannet", "lib.datasets.stanford"]
-    saved = {k: sys.modules.get(k) for k in names}
-    sys.modules.update(_STUBS)
-    try:
-        yield
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
 
 
 @contextlib.contextmanager
@@ -190,7 +153,7 @@ def save_predictions(coords_batch_first, pred, transformation, ds, iteration, sa
     utils, _, _ = load()
     c = np.asarray(coords_batch_first)
     coords = torch.from_numpy(np.ascontiguousarray(np.concatenate([c[:, 1:4], c[:, :1]], 1)))
-    with _np_int(), _installed():
+    with _np_int(), stage_ref.installed(_STUBS):
         utils.save_predictions(coords, np.asarray(pred, np.int64), torch.as_tensor(np.asarray(transformation, np.float32)), ds, None,
                                iteration, save_pred_dir)
 
@@ -202,12 +165,8 @@ def test_pointcloud(ds, pred_dir):
     sink = []
     inner = _recording(module, sink)
     try:
-        with _np_int(), _installed():
+        with _np_int(), stage_ref.installed(_STUBS):
             ds.test_pointcloud(pred_dir)
     finally:
         module.fast_hist = inner
     return sink
-
-
-if __name__ == "__main__":
-    print("staged" if stage(True) else f"{SRC} not present: nothing staged")

@@ -1,11 +1,6 @@
-"""Stages the original `.sens` extraction scripts next to the oracle, so that tests/test_oracle_sens.py,
-tests/golden/make_sens_golden.py and profiles/bench_sens.py can run them unmodified:
-
-    python oracle/sens_ref.py      (also run by __graft_entry__.build())
-
-Copies `<root>/pretrain/data_preprocess/scannet_pair/{SensorData.py, reader.py, point_cloud_extractor.py, plyfile.py}` byte for byte
-into `oracle/_ref/sens/` (git-ignored).  <root> is $PCB_REFERENCE_ROOT, with the same default as oracle/stage_ref.py; where the
-original is absent nothing is staged.  Nothing under pointcontrast_b200/ imports this.
+"""The original `.sens` extraction scripts (`SensorData.py`, `reader.py`, `point_cloud_extractor.py`, `plyfile.py`), staged by
+oracle/stage_ref.py under `oracle/_ref/sens/`, so that tests/test_oracle_sens.py, tests/golden/make_sens_golden.py and
+profiles/bench_sens.py can run them unmodified.  Nothing under pointcontrast_b200/ imports this.
 
 run(script, argv) executes a staged script as `python <script> <argv>` would (the staged directory first on sys.path, so that
 `from SensorData import SensorData` and `from plyfile import ...` find the staged files), with two stand-ins, neither of which
@@ -19,31 +14,15 @@ touches the arithmetic:
 import contextlib
 import os
 import runpy
-import shutil
-import sys
 import types
 
 import numpy as np
 
-SRC = os.path.join(os.environ.get("PCB_REFERENCE_ROOT", "/root/reference"), "pretrain", "data_preprocess", "scannet_pair")
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref", "sens")
-FILES = ("SensorData.py", "reader.py", "point_cloud_extractor.py", "plyfile.py")
-_MODULES = ("SensorData", "plyfile", "imageio", "cv2")
-
-
-def stage(verbose=False):
-    if not all(os.path.isfile(os.path.join(SRC, f)) for f in FILES):
-        return False
-    os.makedirs(ROOT, exist_ok=True)
-    for f in FILES:
-        shutil.copyfile(os.path.join(SRC, f), os.path.join(ROOT, f))
-    if verbose:
-        print("staged", SRC, "(.sens extraction) ->", ROOT)
-    return True
+from oracle import stage_ref
 
 
 def available():
-    return all(os.path.isfile(os.path.join(ROOT, f)) for f in FILES)
+    return stage_ref.available("sens")
 
 
 def _imwrite(path, a):
@@ -67,39 +46,25 @@ def _stubs():
 @contextlib.contextmanager
 def installed():
     """The stand-ins, the staged directory on sys.path and the fromstring bridge, for code that imports the staged modules."""
-    saved_mods = {k: sys.modules.get(k) for k in _MODULES}
-    saved_path = list(sys.path)
     had = "fromstring" in np.__dict__
     saved_fromstring = np.__dict__.get("fromstring")
-    for k in ("SensorData", "plyfile"):
-        sys.modules.pop(k, None)                     # oracle/pair_list_ref.py installs a stub SensorData while it runs
-    sys.modules.update(_stubs())
-    sys.path.insert(0, ROOT)
-    np.fromstring = lambda b, dtype=float, *a, **k: np.frombuffer(b, dtype).copy()
-    try:
-        yield
-    finally:
-        sys.path[:] = saved_path
-        if had:
-            np.fromstring = saved_fromstring
-        else:
-            del np.fromstring
-        for k, v in saved_mods.items():
-            if v is None:
-                sys.modules.pop(k, None)
+    # SensorData and plyfile are removed so that the staged ones are imported: oracle/pair_list_ref.py installs a stub SensorData
+    with stage_ref.installed({"SensorData": None, "plyfile": None, **_stubs()}, path=[stage_ref.path("sens")]):
+        np.fromstring = lambda b, dtype=float, *a, **k: np.frombuffer(b, dtype).copy()
+        try:
+            yield
+        finally:
+            if had:
+                np.fromstring = saved_fromstring
             else:
-                sys.modules[k] = v
+                del np.fromstring
 
 
 def run(script, argv):
-    """Runs the staged `script` (a name of FILES) with command-line arguments `argv`."""
-    saved_argv = sys.argv
-    sys.argv = [os.path.join(ROOT, script)] + list(argv)
-    try:
-        with installed():
-            runpy.run_path(os.path.join(ROOT, script), run_name="__main__")
-    finally:
-        sys.argv = saved_argv
+    """Runs the staged `script` (`reader.py` or `point_cloud_extractor.py`) with command-line arguments `argv`."""
+    script = stage_ref.path("sens", script)
+    with installed(), stage_ref.installed(argv=[script] + list(argv)):
+        runpy.run_path(script, run_name="__main__")
 
 
 def sensor_data(path):
@@ -115,7 +80,3 @@ def extract(sens_path, scene_dir, frame_skip):
     run("reader.py", ["--filename", sens_path, "--output_path", scene_dir, "--frame_skip", str(frame_skip), "--export_depth_images",
                       "--export_poses", "--export_intrinsics"])
     run("point_cloud_extractor.py", ["--input_path", scene_dir, "--output_path", os.path.join(scene_dir, "pcd"), "--save_npz"])
-
-
-if __name__ == "__main__":
-    print("staged" if stage(True) else f"{SRC} not present: nothing staged")

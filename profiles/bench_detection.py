@@ -18,6 +18,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from oracle import stage_ref  # noqa: E402
 from pointcontrast_b200 import detection, pointnet2, synth  # noqa: E402
 
 VOXEL = 0.025
@@ -54,13 +55,12 @@ def alternate(fns, rounds=2):
 
 def original_module():
     """The original `models/backbone_module.py` staged by build(), on this library; None where it was not staged."""
-    staged = os.path.join(ROOT, "oracle", "_ref", "votenet")
-    if not os.path.isfile(os.path.join(staged, "models", "backbone_module.py")):
+    if not stage_ref.available("votenet"):
         return None
     from pointcontrast_b200 import me
     me.install()
     pointnet2.install()
-    sys.path.insert(0, staged)
+    sys.path.insert(0, stage_ref.path("votenet"))
     import importlib
     return importlib.import_module("models.backbone_module")
 

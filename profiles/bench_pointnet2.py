@@ -16,6 +16,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from oracle import pointnet2_ref, stage_ref  # noqa: E402
 from pointcontrast_b200 import pointnet2  # noqa: E402
 
 HBM = 3.35e12
@@ -25,21 +26,6 @@ B = 8
 def gpu_info():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
-
-
-def load_ref():
-    """The compiled reference `_ext` (what build() produced), or None; the original repository itself is never read."""
-    import glob
-    import importlib.machinery
-    import importlib.util
-    so = glob.glob(os.path.join(ROOT, "oracle", "_ref", "pointnet2_ext", "_ext*.so"))
-    if not so:
-        return None
-    loader = importlib.machinery.ExtensionFileLoader("_ext", so[0])
-    spec = importlib.util.spec_from_file_location("_ext", so[0], loader=loader)
-    mod = importlib.util.module_from_spec(spec)
-    loader.exec_module(mod)
-    return mod
 
 
 def time_ms(fn, min_window_s=1.0):
@@ -88,11 +74,10 @@ def workloads(N):
 
 def sa1_ms(N):
     """The reference's PointnetSAModuleVotes(2048, 0.2, 64, [3, 64, 64, 128]) forward + backward on this library, when staged."""
-    mods_dir = os.path.join(ROOT, "oracle", "_ref", "votenet", "pointnet2")
-    if not os.path.isfile(os.path.join(mods_dir, "pointnet2_modules.py")):
+    if not stage_ref.available("votenet"):
         return None
     pointnet2.install()
-    sys.path.insert(0, mods_dir)
+    sys.path.insert(0, stage_ref.path("votenet", "pointnet2"))
     import pointnet2_modules
     sa = pointnet2_modules.PointnetSAModuleVotes(npoint=2048, radius=0.2, nsample=64, mlp=[3, 64, 64, 128], use_xyz=True,
                                                  normalize_xyz=True).cuda().train()
@@ -108,7 +93,7 @@ def sa1_ms(N):
 
 def main():
     torch.backends.cudnn.benchmark = True
-    ref = load_ref()
+    ref = pointnet2_ref.load()                # what build() compiled; the original repository itself is never read
     out = {"gpu": gpu_info(), "B": B, "reference_kernels": ref is not None, "ops": {}}
     for N in (20000, 40000):
         tag = "sunrgbd_N20000" if N == 20000 else "scannet_N40000"

@@ -21,9 +21,9 @@ import torch  # noqa: E402
 
 from pointcontrast_b200 import pointnet2, pointnet2_modules  # noqa: E402
 from pointcontrast_b200._lib import check, lib, ptr, stream  # noqa: E402
+from oracle import stage_ref  # noqa: E402
 from profiles.bench_pointnet2 import gpu_info, time_ms  # noqa: E402
 
-STAGED = os.path.join(ROOT, "oracle", "_ref", "votenet", "pointnet2")
 # name: (B, N, C_in, npoint, nsample, radius, mlp) -- backbone_module.py / proposal_module.py
 SA = {"sa1_sunrgbd": (8, 20000, 0, 2048, 64, 0.2, [0, 64, 64, 128]), "sa1_scannet": (8, 40000, 0, 2048, 64, 0.2, [0, 64, 64, 128]),
       "sa2": (8, 2048, 128, 1024, 32, 0.4, [128, 128, 128, 256]), "sa3": (8, 1024, 256, 512, 16, 0.8, [256, 128, 128, 256]),
@@ -33,12 +33,12 @@ FP = {"fp1": (8, 512, 256), "fp2": (8, 1024, 512)}       # (B, n unknown, m know
 
 
 def original():
-    if not os.path.isfile(os.path.join(STAGED, "pointnet2_modules.py")):
+    if not stage_ref.available("votenet"):
         raise SystemExit("the original modules are not staged under oracle/_ref/votenet/pointnet2 (run __graft_entry__.build())")
     for m in ("pointnet2_utils", "pointnet2_modules", "pytorch_utils"):
         sys.modules.pop(m, None)
     pointnet2.install()
-    sys.path.insert(0, STAGED)
+    sys.path.insert(0, stage_ref.path("votenet", "pointnet2"))
     return importlib.import_module("pointnet2_modules")
 
 

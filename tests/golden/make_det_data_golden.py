@@ -1,5 +1,6 @@
-"""Writes tests/golden/det_data.npz: the original VoteNet detection `__getitem__`s (staged by oracle/det_data_ref.py), run unmodified
-on small synthetic scenes (pointcontrast_b200.synth) from a seeded RandomState, their draws recorded.
+"""Writes tests/golden/det_data.npz: the original VoteNet detection `__getitem__`s (staged by oracle/stage_ref.py, loaded by
+oracle/det_data_ref.py), run unmodified on small synthetic scenes (pointcontrast_b200.synth) from a seeded RandomState, their draws
+recorded.
 
     python tests/golden/make_det_data_golden.py
 
@@ -49,7 +50,7 @@ def write_scenes(path):
 
 def main():
     mods = det_data_ref.load()
-    assert mods is not None, "the original is not staged: run oracle/det_data_ref.py"
+    assert mods is not None, "the original is not staged: run oracle/stage_ref.py"
     out = {}
     with tempfile.TemporaryDirectory() as d:
         write_scenes(d)

@@ -12,7 +12,7 @@ import tempfile
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
-from oracle import det_prep_ref as R  # noqa: E402
+from oracle import det_prep_ref as R, stage_ref  # noqa: E402
 from pointcontrast_b200 import synth  # noqa: E402
 
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "det_prep.npz")
@@ -42,7 +42,7 @@ def digests(root):
 
 
 def main():
-    assert R.available() or R.stage(), "the original is not present"
+    assert R.available() or "det_prep" in stage_ref.stage(), "the original is not present"
     with tempfile.TemporaryDirectory() as d:
         write_inputs(os.path.join(d, "in"))
         files = sorted(os.path.relpath(os.path.join(a, f), os.path.join(d, "in")) for a, _, fs in os.walk(os.path.join(d, "in")) for f in fs)

@@ -1,8 +1,8 @@
 """Generates tests/golden/semseg_fulleval.npz: the reference's own `save_predictions` (`downstream/semseg/lib/utils.py:304-349`) and
-`test_pointcloud` (`lib/datasets/scannet.py:131-172`, `stanford.py:41-84`), unmodified, staged by oracle/semseg_fulleval_ref.py with the
-shims its docstring lists, on synthetic rooms:
+`test_pointcloud` (`lib/datasets/scannet.py:131-172`, `stanford.py:41-84`), unmodified, staged by oracle/stage_ref.py and run by
+oracle/semseg_fulleval_ref.py with the shims its docstring lists, on synthetic rooms:
 
-    python oracle/semseg_fulleval_ref.py && python tests/golden/make_semseg_fulleval_golden.py
+    python oracle/stage_ref.py && python tests/golden/make_semseg_fulleval_golden.py
 
 * ScanNet: 4 rooms (`synth.synth_labelled_room`), 2 cm voxels, each under its own rotation about z, scale and translation (the float32
   4x4 the voxelizer returns), seeded masked predictions over 20 classes, batch size 1;

@@ -1,5 +1,5 @@
 """Writes tests/golden/semseg_prep.npz: a small S3DIS tree with adversarial annotation text and the output the original converter
-(oracle/semseg_prep_ref.py, staged by `python oracle/semseg_prep_ref.py`) writes for it -- each room's PLY bytes and the split files.
+(oracle/semseg_prep_ref.py, staged by `python oracle/stage_ref.py`) writes for it -- each room's PLY bytes and the split files.
 
     python tests/golden/make_semseg_prep_golden.py
 
@@ -12,7 +12,7 @@ import tempfile
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
-from oracle import semseg_prep_ref as R  # noqa: E402
+from oracle import semseg_prep_ref as R, stage_ref  # noqa: E402
 
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "semseg_prep.npz")
 
@@ -42,7 +42,7 @@ def tree():
 
 
 def main():
-    assert R.available() or R.stage(), "the original is not present"
+    assert R.available() or "semseg_prep" in stage_ref.stage(), "the original is not present"
     files = tree()
     with tempfile.TemporaryDirectory() as d:
         for rel, data in files.items():

@@ -1,7 +1,7 @@
 """Generates tests/golden/sens_extract.npz: what the reference's own `reader.py` + `point_cloud_extractor.py`, unmodified, staged by
-oracle/sens_ref.py with the stand-ins its docstring lists, extract from a small synthetic `.sens` file:
+oracle/stage_ref.py and run by oracle/sens_ref.py with the stand-ins its docstring lists, extract from a small synthetic `.sens` file:
 
-    python oracle/sens_ref.py && python tests/golden/make_sens_golden.py
+    python oracle/stage_ref.py && python tests/golden/make_sens_golden.py
 
 The scan (`synth.synth_sens_scan`, 64 x 48 depth, 9 frames, frame_skip 2, so 5 frames kept and 4 seeked past) holds zero-depth holes
 and depth-65535 pixels in every frame, an all-zero frame (2), a frame with a block of depth 65535 (6) and a frame stored with an
@@ -34,7 +34,7 @@ def main():
     from oracle import sens_ref
     from pointcontrast_b200 import synth
     if not sens_ref.available():
-        raise SystemExit("the reference's .sens scripts are not staged: run oracle/sens_ref.py")
+        raise SystemExit("the reference's .sens scripts are not staged: run oracle/stage_ref.py")
     depth, poses, K = scan()
     with tempfile.TemporaryDirectory() as tmp:
         sens = os.path.join(tmp, "scene0000_00.sens")

@@ -7,11 +7,12 @@ import os
 import sys
 import types
 
+from oracle import stage_ref
+
 REF_PC = os.path.join(os.environ.get("PCB_REFERENCE_ROOT", ""), "pretrain", "pointcontrast")
-if not os.environ.get("PCB_REFERENCE_ROOT") or not os.path.isdir(REF_PC):       # the model package staged by oracle/stage_ref.py
-    _staged = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "pointcontrast")
-    if os.path.isdir(os.path.join(_staged, "model")):
-        REF_PC = _staged
+if not os.environ.get("PCB_REFERENCE_ROOT") or not os.path.isdir(REF_PC):
+    if stage_ref.available("pointcontrast/model"):
+        REF_PC = os.path.dirname(stage_ref.path("pointcontrast/model"))
 
 
 def available():
@@ -27,11 +28,8 @@ def load_reference_model_module(me_module_installer):
     """Returns the reference's `model` package imported against the ME surface installed by `me_module_installer()`."""
     _purge()
     me_module_installer()
-    sys.path.insert(0, REF_PC)
-    try:
+    with stage_ref.installed(path=[REF_PC]):
         return importlib.import_module("model")
-    finally:
-        sys.path.remove(REF_PC)
 
 
 def load_reference_trainer_module(me_module_installer):
@@ -43,11 +41,8 @@ def load_reference_trainer_module(me_module_installer):
             m.SummaryWriter = object
             m.OmegaConf = object
             sys.modules[name] = m
-    sys.path.insert(0, REF_PC)
-    try:
+    with stage_ref.installed(path=[REF_PC]):
         return importlib.import_module("lib.ddp_trainer")
-    finally:
-        sys.path.remove(REF_PC)
 
 
 class Cfg(dict):

@@ -1,7 +1,6 @@
 """Host checks of the PointNet++ oracle (oracle/pointnet2_cpu.py) against independent computations, and of the argument checks of the
 pcb_* PointNet++ entry points, which reject bad input before touching a device."""
 import importlib
-import os
 import sys
 
 import numpy as np
@@ -9,16 +8,15 @@ import pytest
 import torch
 from scipy.spatial import cKDTree
 
-from oracle import pointnet2_cpu as O
+from oracle import pointnet2_cpu as O, stage_ref
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-VOTENET = os.path.join(ROOT, "oracle", "_ref", "votenet", "pointnet2")
+VOTENET = stage_ref.path("votenet", "pointnet2")
 
 
 def reference_modules(install):
     """Fresh imports of the staged, unmodified pointnet2_utils / pointnet2_modules bound to the `_ext` that `install()` registers
     (pointnet2_utils binds `pointnet2._ext` at import time, so each backend needs its own import)."""
-    if not os.path.isfile(os.path.join(VOTENET, "pointnet2_modules.py")):
+    if not stage_ref.available("votenet"):
         pytest.skip("oracle/_ref/votenet not staged (the original repository is absent)")
     for m in ("pointnet2_utils", "pointnet2_modules", "pytorch_utils"):
         sys.modules.pop(m, None)
