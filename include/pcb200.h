@@ -741,6 +741,44 @@ int pcb_sa_pool_grad(const float* g, int ldg, const int32_t* sel, const float* o
                      void* stream);
 int pcb_sa_xyz_rows(const float* grel, const float* d_new_xyz, int64_t M, int S, float radius, float* rows, void* stream);
 
+/* ----------------------------------------------------------------------------------------------- VoteNet heads (8f-18) */
+/* The elementwise ends of VoteNet's voting module (`models/voting_module.py`) and proposal head (`models/proposal_module.py`
+ * decode_scores) around their last 1x1 convolution, whose output z (fp32, point-major rows, row stride ldz) the caller computes with
+ * pcb_conv_forward_split; the layers before it are pcb_unit_* calls on a K = 1 identity table.  Forward arithmetic is the original's
+ * torch expressions on the same z, one rounding per operation: the outputs are bit-identical to them.  Every output element is written
+ * by one thread (deterministic, no atomics).  Gradients are read through pcb_strided element strides (NULL, or a NULL `p`: absent, read
+ * as 0); the gradient of z comes out as bf16 hi/lo planes (the gradient operand of pcb_conv_wgrad_split / pcb_conv_forward_split).
+ *
+ * pcb_vote_epilogue: seed rows r = b S + s, V votes per seed, C feature channels, z [B S, >= (3 + C) V] with vote v in columns
+ *   [v (3 + C), (v + 1)(3 + C)): vote_xyz (fp32 [B, S V, 3], contiguous) = seed_xyz[b, s] + z[r, v (3 + C) + 0..2], and vote_features
+ *   (fp32 [B S V, C], point-major: row r V + v) = seed_features[r] (row stride ldf) + z[r, v (3 + C) + 3 + c].
+ * pcb_vote_epilogue_grad: d_vote_xyz (scene, vote, axis) and d_vote_features (scene, vote, channel) -> dz_hi / dz_lo [B S, ldz], columns
+ *   [0, Cpad) written (0 beyond (3 + C) V); d_seed_features (fp32 [B S, C], row stride ldd, or NULL) = sum over v of d_vote_features
+ *   and d_seed_xyz (fp32 [B, S, 3] or NULL) = sum over v of d_vote_xyz, in ascending v: the residual paths.
+ * pcb_proposal_epilogue: z [B K, >= X] in decode_scores' column order (objectness 2, center 3, heading scores NH, heading residuals NH,
+ *   size scores NS, size residuals 3 NS, semantic classes), aggregated_vote_xyz fp32 [B, K, 3]: center [B, K, 3] = aggregated_vote_xyz +
+ *   z[:, 2:5]; heading_residuals [B, K, NH] = z[:, 5+NH : 5+2NH] * heading_unit (fp32(pi / NH): torch's fp32 tensor times a Python
+ *   float); size_residuals [B, K, NS, 3] = the size-residual columns * mean_size (HOST fp32 [NS, 3], NS <= 64, copied into the launch).
+ * pcb_proposal_epilogue_grad: grads = HOST array of 9 pcb_strided in decode_scores' end_points order -- objectness_scores, center,
+ *   heading_scores, heading_residuals_normalized, heading_residuals, size_scores, size_residuals_normalized (sx: the axis stride),
+ *   size_residuals (sx too), sem_cls_scores -- each with strides (scene, proposal, channel).  dz (columns [0, Xpad), 0 beyond X =
+ *   5 + 2 NH + 4 NS + C) = the gradient of the view reading each column, the residual columns plus heading_unit x d heading_residuals
+ *   and mean_size x d size_residuals; written as bf16 hi/lo planes (dz_hi / dz_lo) and / or fp32 (dz), each NULL to skip, row stride ldz.
+ *   d_aggregated_vote_xyz (fp32 [B, K, 3] or NULL) = the center gradient.
+ * Sizes below 1, B S V or B K >= 2^31, NS > 64, strides below the widths and NULL required pointers return PCB_ERR_ARG before the
+ * launch. */
+int pcb_vote_epilogue(const float* seed_xyz, const float* seed_features, int ldf, const float* z, int ldz, int64_t B, int64_t S, int V,
+                      int C, float* vote_xyz, float* vote_features, void* stream);
+int pcb_vote_epilogue_grad(const pcb_strided* d_vote_xyz, const pcb_strided* d_vote_features, int64_t B, int64_t S, int V, int C,
+                           uint16_t* dz_hi, uint16_t* dz_lo, int ldz, int Cpad, float* d_seed_features, int ldd, float* d_seed_xyz,
+                           void* stream);
+int pcb_proposal_epilogue(const float* z, int ldz, const float* aggregated_vote_xyz, int64_t B, int64_t K, int NH, int NS,
+                          float heading_unit, const float* mean_size, float* center, float* heading_residuals, float* size_residuals,
+                          void* stream);
+int pcb_proposal_epilogue_grad(const pcb_strided* grads, int64_t B, int64_t K, int NH, int NS, int C, float heading_unit,
+                               const float* mean_size, uint16_t* dz_hi, uint16_t* dz_lo, float* dz, int ldz, int Xpad,
+                               float* d_aggregated_vote_xyz, void* stream);
+
 /* ----------------------------------------------------------------------------------------------- optimiser */
 /* torch.optim.SGD semantics on a flat buffer:  d = g*grad_scale + wd*p;  buf = first ? d : momentum*buf + (1-dampening)*d;  p -= lr*buf
  * (pretraining: dampening 0, `lib/ddp_trainer.py:107-111`; semseg finetuning: 0.1, `downstream/semseg/lib/solvers.py:50-57`) */

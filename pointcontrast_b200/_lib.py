@@ -65,6 +65,7 @@ class PcbDetBatch(C.Structure):
 
 _DLA = C.POINTER(PcbDetLossArgs)
 _DDB = C.POINTER(PcbDetBatch)
+_PS = C.POINTER(PcbStrided)
 _SIGS = {
     "pcb_last_error": (C.c_char_p, []),
     "pcb_version": (C.c_char_p, []),
@@ -164,6 +165,10 @@ _SIGS = {
     "pcb_sa_pool": (_i, [_p, _i, _l, _i, _i, _p, _p, _p, _p, _p, _p, _i, _p]),
     "pcb_sa_pool_grad": (_i, [_p, _i, _p, _p, _i, _l, _i, _i, _p, _p]),
     "pcb_sa_xyz_rows": (_i, [_p, _p, _l, _i, _f, _p, _p]),
+    "pcb_vote_epilogue": (_i, [_p, _p, _i, _p, _i, _l, _l, _i, _i, _p, _p, _p]),
+    "pcb_vote_epilogue_grad": (_i, [_PS, _PS, _l, _l, _i, _i, _p, _p, _i, _i, _p, _i, _p, _p]),
+    "pcb_proposal_epilogue": (_i, [_p, _i, _p, _l, _l, _i, _i, _f, _p, _p, _p, _p, _p]),
+    "pcb_proposal_epilogue_grad": (_i, [_PS, _l, _l, _i, _i, _i, _f, _p, _p, _p, _p, _i, _i, _p, _p]),
     "pcb_voxel_down_sample_ws_bytes": (_sz, [_l, _l]),
     "pcb_voxel_down_sample": (_i, [_p, _l, _p, _l, _d, _p, _p, _p, _p, _sz, _p]),
     "pcb_frame_overlap_ws_bytes": (_sz, [_l, _l]),

@@ -98,15 +98,28 @@ def _identity(n, device):
     return t
 
 
+def _pad32(n):
+    return (n + 31) // 32 * 32
+
+
 def _tiles(conv):
-    """(weights [Cin][Cout], forward tiles (fp16 x 2^10), data-gradient tiles) of a 1x1 conv, rebuilt whenever the weight changes: its
-    version counter moves on every in-place update (an optimiser step), a raw-pointer rewrite bumps me's weights epoch."""
-    w = conv.weight
-    tag = (w.data_ptr(), w._version, me._WEIGHTS_EPOCH[0])
+    """(weights [Cin][Cout], forward tiles (fp16 x 2^10), data-gradient tiles) of a 1x1 conv, rebuilt whenever the weight or bias
+    changes: its version counter moves on every in-place update (an optimiser step), a raw-pointer rewrite bumps me's weights epoch.
+    A conv with a bias gets 32 more input rows: row Cin holds the bias (its input column is constant 1), the rest are zero; output
+    columns are padded with zeros to a multiple of 32."""
+    w, bias = conv.weight, conv.bias
+    tag = (w.data_ptr(), w._version, me._WEIGHTS_EPOCH[0]) + (() if bias is None else (bias.data_ptr(), bias._version))
     cache = conv.__dict__.get("_pcb_tiles")
     if cache is None or cache[0] != tag:
         cout, cin = w.shape[:2]
         wl = w.detach().reshape(cout, cin).t().contiguous()
+        if bias is not None or cout % 32:
+            full = torch.zeros(cin + (0 if bias is None else 32), _pad32(cout), dtype=torch.float32, device=w.device)
+            full[:cin, :cout] = wl
+            if bias is not None:
+                full[cin, :cout] = bias.detach()
+            wl = full
+        cin, cout = wl.shape
         f = torch.empty(lib.pcb_weight_tile_bytes(1, cin, cout, 0), dtype=torch.uint8, device=w.device)
         d = torch.empty(lib.pcb_weight_tile_bytes(1, cin, cout, 1), dtype=torch.uint8, device=w.device)
         check(lib.pcb_weight_tile(ptr(wl), 1, cin, cout, ptr(f), ptr(d), _lib.PLANES_B_FP16, stream()))
@@ -142,9 +155,10 @@ def _stats(bn, z, n, C, train, ws_dev):
 
 
 def _unit(n, tbl, conv, bn, x, out, z, mean, invstd, train, out_p=None):
-    """pcb_unit of one K = 1 layer over n rows: x / out are _Planes, z fp32 [n, Cout]."""
-    cout, cin = conv.weight.shape[:2]
+    """pcb_unit of one K = 1 layer over n rows: x / out are _Planes, z fp32 [n, Cout].  With a conv bias, x carries the constant
+    columns _tiles' bias row reads (x.C = Cin + 32)."""
     wl, tf, td = _tiles(conv)
+    cin, cout = wl.shape
     u = PcbUnit()
     u.keep = (tbl, wl, tf, td)                # the backward call reads the table and the tiles of the forward's weights
     u.n_in = u.n_out = u.n0 = n
@@ -158,10 +172,10 @@ def _unit(n, tbl, conv, bn, x, out, z, mean, invstd, train, out_p=None):
     u.eps, u.momentum = bn.eps, _momentum(bn)
     u.mean, u.invstd = mean.data_ptr(), invstd.data_ptr()
     u.x_hi, u.x_lo, u.x_bhi, u.x_blo = x.ptrs()
-    u.x_lds = cin
+    u.x_lds = x.C
     u.z_p, u.z_ld = z.data_ptr(), cout
     u.out_hi, u.out_lo, u.out_bhi, u.out_blo = out.ptrs()
-    u.out_lds = cout
+    u.out_lds = out.C
     if out_p is not None:
         u.out_p, u.out_ld = out_p.data_ptr(), cout
     u.flags = _lib.UNIT_FP16_FORWARD | (0 if train else _lib.UNIT_EVAL)
@@ -175,21 +189,28 @@ def _run_unit(u, dev, backward=False):
     check((lib.pcb_unit_backward if backward else lib.pcb_unit_forward)(ctypes.byref(u), stream()))
 
 
-def _unit_backward(u, conv, bn, g, gin, dev):
-    """Backward of a forward unit `u`: g = gradient of its output (fp32 [n, Cout]) -> gin (fp32 [n, Cin], written) and the parameter
-    gradients (returned: dW as [Cout, Cin, 1, 1], dgamma, dbeta)."""
+def _conv_grads(conv, dW):
+    """The parameter gradients of a 1x1 conv from dW [Cin(+32)][Cout(pad)] in _tiles' layout: (weight,) or (weight, bias)."""
+    cout, cin = conv.weight.shape[:2]
+    dw = dW[:cin, :cout].t().reshape(conv.weight.shape)
+    return (dw,) if conv.bias is None else (dw, dW[cin, :cout])
+
+
+def _unit_backward(u, conv, bn, g, gin, dev, gin_mode=1):
+    """Backward of a forward unit `u`: g = gradient of its output (fp32 [n, Cout], row stride g.stride(0)) -> gin (fp32 [n, Cin],
+    written (gin_mode 1) or accumulated (2)) and the parameter gradients (returned: _conv_grads, then dgamma, dbeta)."""
     n, cin, cout = u.n_out, u.Cin, u.Cout
     dzt = torch.empty(2, n, cout, dtype=torch.int16, device=dev)
     dW = torch.zeros(cin, cout, dtype=torch.float32, device=dev)
     dgamma = torch.zeros(cout, dtype=torch.float32, device=dev)
     dbeta = torch.zeros_like(dgamma)
-    u.g_p, u.g_ld = g.data_ptr(), cout
+    u.g_p, u.g_ld = g.data_ptr(), g.stride(0)
     u.dz_hi, u.dz_lo, u.dz_ld = dzt[0].data_ptr(), dzt[1].data_ptr(), cout
     u.dW, u.dgamma, u.dbeta = dW.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr()
-    u.gin_p, u.gin_ld, u.gin_mode = gin.data_ptr(), cin, 1
+    u.gin_p, u.gin_ld, u.gin_mode = gin.data_ptr(), cin, gin_mode
     u.gres_mode = 0
     _run_unit(u, dev, backward=True)
-    return dW.t().reshape(cout, cin, 1, 1), dgamma, dbeta
+    return _conv_grads(conv, dW) + (dgamma, dbeta)
 
 
 def _eval_forward_only(params):
