@@ -101,11 +101,16 @@ class _B:
 def model_units(name):
     """Static signatures (fp16 off, training, two views) of every unit of the model as fused.Runner.forward issues them and its
     backward sweep gives them gradient modes, in forward order.  Built on the meta device: no data."""
-    from pointcontrast_b200 import me
     from pointcontrast_b200.model import load_model
     from tests.refload import default_config
     with torch.device("meta"):
         m = load_model(name)(3, 32, default_config(), D=3)
+    return net_units(m)
+
+
+def net_units(m):
+    """`model_units` of a built network (any output width: a final layer the tensor cores do not take asks for the fp32 plane of
+    its input)."""
     units = []
 
     def kind(conv):
