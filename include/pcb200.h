@@ -451,7 +451,11 @@ size_t pcb_nce_ws_bytes(int64_t n);
 int pcb_nce_forward_backward(const float* q, const float* k, int64_t n, int D, float inv_T, float* loss, float* dq,
                              float* dk, void* ws, size_t ws_bytes, void* stream);
 /* nn.CrossEntropyLoss(ignore_index) on logits [n, C] with int64 targets (`downstream/semseg/lib/train.py:68,120`): writes the mean loss
- * over the non-ignored rows (device float) and dlogits = grad_scale * d loss / d logits.  ws: pcb_ce_ws_bytes(n). */
+ * over the non-ignored rows (device float) and dlogits = grad_scale * d loss / d logits.  ws: pcb_ce_ws_bytes(n).  n >= 1, 1 <= C <= 1024.
+ * A row counts when its target t is in [0, C) and != ignore_index.  A target outside [0, C) is treated as ignored (torch raises): its
+ * logit x[t] is never read, and the row adds nothing to the loss or the count and gets a zero gradient.  With no counted row the loss is
+ * NaN (0 / 0, as torch) and dlogits is all zero.  A NaN logit in a counted row makes the loss NaN and that row's gradient NaN (as
+ * torch); in a row that does not count it changes nothing (torch's backward gives that row NaN times a zero incoming gradient). */
 size_t pcb_ce_ws_bytes(int64_t n);
 int pcb_ce_forward_backward(const float* logits, const int64_t* target, int64_t n, int C, int64_t ignore_index, float grad_scale,
                             float* loss, float* dlogits, void* ws, size_t ws_bytes, void* stream);
@@ -646,7 +650,11 @@ size_t pcb_det_points_ws_bytes(int64_t B, int64_t k);
 int pcb_det_points(const pcb_det_batch* a, void* ws, size_t ws_bytes, void* stream);
 int pcb_det_boxes(const pcb_det_batch* a, void* stream);
 /* Row-wise L2 normalisation of the output features, y = x / ||x||_2 with no epsilon (`model/res16unet.py:262-266`), and its
- * backward dx = (dy - y (y.dy)) / ||x||.  inv_norm: [n] scratch written by forward, read by backward. */
+ * backward dx = (dy - y (y.dy)) / ||x||.  inv_norm: [n] scratch written by forward, read by backward.
+ * Without an epsilon a row whose fp32 sum of squares is 0 -- a zero row, or one whose squares all underflow -- gets inv_norm = +inf
+ * and y = x * inf (NaN at its zeros, +-inf elsewhere); a row whose sum of squares overflows gets inv_norm = 0 and y = +-0.  These are
+ * the bits of x / torch.norm(x, p=2, dim=1, keepdim=True) in fp32 on CUDA for C >= 2 (at C = 1 torch's norm is |x|, so its
+ * expression gives +-1 where this gives x / sqrt(x^2) with the same edges). */
 int pcb_l2norm_forward(const float* X, int64_t n, int C, float* Y, float* inv_norm, void* stream);
 int pcb_l2norm_backward(const float* dY, const float* Y, const float* inv_norm, int64_t n, int C, float* dX, void* stream);
 /* minval[i] = min_j sqrt(sum_d (A[i,d]-B[j,d])^2 + 1e-7), argmin[i] = smallest such j.   packed: u64 scratch [P]. */
